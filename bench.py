@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - the driver's measurement contract for nunif_b200.
+"""bench.py - the measurement of nunif_b200's flagship workload (one JSON result line).
 
 Default workload (BASELINE.json configs[1]): waifu2x swin_unet/art scale4x, one synthetic 4K
 (3x2160x3840) frame per step through `tiled_render(tile_size=256, batch_size=16)` = 170 tiles,
@@ -9,6 +9,8 @@ random-init weights (seed 0), fp16 tensor-core compute.  Metric = input megapixe
   python bench.py --impl reference ...                      # the reference algorithm on the host CPU cores (oracle port)
 
 One JSON line is printed by rank 0.  See DESIGN.md "Measurement" for every field.
+--dump-outputs DIR writes what the timed path returned in its last step as DIR/<name>.npy (float32; a large output as a fixed
+seeded sample, see dump_outputs), so that two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -46,11 +48,35 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16/BF16 - not reached figures
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data-sheet"
+
+
+DUMP_SAMPLES = 1 << 21   # values kept of an output larger than this (8 MB float32 + 16 MB float64 indices)
+DUMP_CROP = 512          # plus a full-resolution corner crop of the last two dimensions
+
+
+def dump_outputs(path, outputs):
+    """--dump-outputs: write each output tensor as <path>/<name>.npy (float32).  An output with more than DUMP_SAMPLES values is
+    written as a fixed seeded sample of its flattened values (<name>.npy) with the flat indices taken (<name>_index.npy, float64,
+    exact below 2**53) and a corner crop (<name>_crop.npy), which keeps the files of one call well under 64 MB."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    for name, t in outputs.items():
+        t = t.detach().float()
+        if t.numel() <= DUMP_SAMPLES:
+            np.save(os.path.join(path, name + ".npy"), t.cpu().numpy())
+            continue
+        idx = np.unique(np.random.default_rng(0).integers(0, t.numel(), DUMP_SAMPLES, dtype=np.int64))
+        vals = t.reshape(-1)[torch.from_numpy(idx).to(t.device)].cpu().numpy()
+        np.save(os.path.join(path, name + ".npy"), vals)
+        np.save(os.path.join(path, name + "_index.npy"), idx.astype(np.float64))
+        np.save(os.path.join(path, name + "_crop.npy"), t[..., :DUMP_CROP, :DUMP_CROP].cpu().numpy())
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -566,7 +592,7 @@ def _init_b200(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py needs a B200: the engine has no CPU fallback (use --impl reference for the CPU arm)")
+        raise RuntimeError("bench.py needs an H100: the engine has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -626,6 +652,8 @@ def run_b200_iw3(args):
         launches = lib.nb200_launch_count() - launches0
         ms = e0.elapsed_time(e1)
         out_shape = list(y.shape)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"stereo": y})
     # ---- end to end from host uint8 frames (outside inference_mode: the pipeline enters it around the callback itself)
     u8_in = (c.permute(0, 2, 3, 1) * 255.0).round().to(torch.uint8).contiguous().cpu().pin_memory()   # contiguous HWC, like a decoder's frame
     frames_host = [u8_in[i] for i in range(B)]
@@ -681,10 +709,10 @@ def run_b200_iw3(args):
     else:
         ach = d["work"] / (d["ms"] / 1e3) / 1e9
         roof = {"bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": ach / peaks["hbm_gbs"]}
-    roof.update({"kernel": {"gemm": "gemm_conv_persistent (tcgen05 implicit GEMM: every Linear / conv of the depth network)",
+    roof.update({"kernel": {"gemm": "gemm_conv_kernel (wgmma implicit GEMM: every Linear / conv of the depth network)",
                             "window_attention": "flash_attention_kernel (mma.sync, d = 64, relative-position bias for BEiT)"}.get(dom, dom),
                  "class": dom, "launches": d.get("launches"), "avg_launch_us": d["ms"] * 1e3 / max(1, d.get("launches", 1)),
-                 "share_of_step": d["ms"] / total, "peak_source": f"{peak_src} MEASURED_PEAKS.json", "traffic": None,
+                 "share_of_step": d["ms"] / total, "peak_source": f"{peak_src}", "traffic": None,
                  "note": "achieved = algorithmic FLOPs (2*M*N*K per GEMM launch; 4*T*N*d per attention launch) or bytes of every launch of the "
                          "dominant kernel class in one step / their CUDA-event time (nb200_profile_report)"})
     line = {
@@ -692,7 +720,7 @@ def run_b200_iw3(args):
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
         "config": {"workload": f"{wl['text']}, {w}x{h} frames, {B} frames/GPU/step", "workload_key": args.workload,
                    "parallelism": f"frame-parallel x{world} (no data-path collective)", "weights": "random-init seed 0 (nunif_b200.synth)",
-                   "l2": "frames + activations per step exceed the 126 MB L2; no explicit flush", "output_shape": out_shape,
+                   "l2": "frames + activations per step exceed the 50 MB L2; no explicit flush", "output_shape": out_shape,
                    "input_megapixels_per_sec": fps * h * w / 1e6},
         "e2e": {"value": fps_e2e, "unit": "frames/s", "h2d_bytes_per_step": int(u8_in.numel()),
                 "d2h_bytes_per_step": int(out_shape[0] * out_shape[1] * out_shape[2] * out_shape[3]), "steps": e2e_steps,
@@ -722,7 +750,7 @@ def run_b200(args):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py needs a B200: the engine has no CPU fallback (use --impl reference for the CPU arm)")
+        raise RuntimeError("bench.py needs an H100: the engine has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -741,7 +769,7 @@ def run_b200(args):
     _lib.check(lib.nb200_check_device(local))
     if os.environ.get("NB200_GRAPHS"):
         _lib.check(lib.nb200_tune_set(9, int(os.environ["NB200_GRAPHS"])))   # CUDA-graph replay of the tile-batch forward (A/B)
-    for kv in filter(None, os.environ.get("NB200_TUNE", "").split(",")):    # A/B knobs of csrc/gemm.cu g_tune, e.g. NB200_TUNE=12=1
+    for kv in filter(None, os.environ.get("NB200_TUNE", "").split(",")):    # A/B knobs of csrc/gemm.cu g_tune, e.g. NB200_TUNE=7=1
         k, v = kv.split("=")
         _lib.check(lib.nb200_tune_set(int(k), int(v)))
 
@@ -773,6 +801,7 @@ def run_b200(args):
         torch.cuda.synchronize()
 
     with torch.no_grad():
+        y = None
         for _ in range(args.warmup):
             y = step()
         del y
@@ -787,6 +816,8 @@ def run_b200(args):
             barrier()
         launches = lib.nb200_launch_count() - launches0
         ms = e0.elapsed_time(e1)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"image": y})
         del y
         # ---- end-to-end through the public API with host buffers (H2D + render + D2H every step)
         e2e_steps = max(1, min(args.steps, 3))
@@ -818,7 +849,7 @@ def run_b200(args):
             except Exception as e:  # noqa: BLE001
                 torch.cuda.synchronize()
                 return {"error": f"{type(e).__name__}: {e}"}
-        secondaries = rank == 0 and args.workload == "swin4x_4k" and not os.environ.get("NB200_BENCH_MINIMAL")   # (set for the ncu launch-list pass)
+        secondaries = rank == 0 and args.workload == "swin4x_4k" and not os.environ.get("NB200_BENCH_MINIMAL")   # (set to time the headline workload alone)
         to2x = guarded(bench_to2x_4k, dev, model4x, x) if secondaries else None
         iw3 = guarded(bench_iw3, dev, lib, peaks_gbs=load_peaks()[0]["hbm_gbs"]) if secondaries else None
         upc = guarded(bench_upcunet, dev, lib, x) if secondaries else None
@@ -834,9 +865,8 @@ def run_b200(args):
     peaks, peak_src = load_peaks()
     peak_tf = peaks.get("bf16_tflops_sustained", peaks["bf16_tflops"])     # kernels timed inside a long step: the sustained figure
     total_prof_ms = sum(v["ms"] for v in prof.values())
-    KERNEL_OF = {"fused_attn": "swin_attn_tc_kernel (tcgen05 qkv GEMM, QK^T and PV; q/k/v/S/P in shared / tensor memory)",
-                 "fused_mlp": "swin_mlp_fused2_kernel / swin_mlp_fused_kernel (tcgen05 [proj +] fc1 + GELU + fc2, hidden in smem/TMEM)",
-                 "gemm": "gemm_conv_persistent (tcgen05 implicit GEMM: convs, patch up/down, proj of the C=192 blocks, to_image)"}
+    KERNEL_OF = {"gemm": "gemm_conv_kernel (wgmma implicit GEMM: convs, patch up/down, every Linear of the Swin blocks, to_image)",
+                 "window_attention": "window_attention_mma_kernel (mma.sync shifted-window attention core)"}
 
     def tensor_view(name):
         c = prof.get(name)
@@ -852,15 +882,7 @@ def run_b200(args):
     views = {k: tensor_view(k) for k in KERNEL_OF}
     views = {k: v for k, v in views.items() if v}
     dom = max(views, key=lambda k: views[k]["ms_per_frame"]) if views else None
-    # dram__bytes_read.sum + dram__bytes_write.sum of the shipped kernels, parsed from an ncu --set full capture by
-    # profiles/ncu_traffic.py into profiles/r2/ncu_traffic.json (per launch of the largest launch class); null until captured
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r2", "ncu_traffic.json")
-    if dom and os.path.exists(tpath):
-        try:
-            traffic = json.load(open(tpath)).get(dom)
-        except (OSError, ValueError):
-            traffic = None
+    traffic = None   # measured DRAM bytes per launch: not measured
     line = {
         "metric": "waifu2x_input_megapixels_per_sec", "value": value, "unit": "MP/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",
@@ -870,7 +892,7 @@ def run_b200(args):
                    "workload_key": args.workload,
                    "parallelism": f"frame-parallel x{world} (no data-path collective; NCCL weight broadcast at load)",
                    "weights": "random-init seed 0 (nunif_b200.synth)",
-                   "l2": "inputs/activations per step (>1 GB) exceed the 126 MB L2; no explicit flush",
+                   "l2": "inputs/activations per step (>1 GB) exceed the 50 MB L2; no explicit flush",
                    "frames_per_sec": world * args.steps / (ms / 1e3),
                    "output_megapixels_per_sec": value * oscale * oscale,
                    "model_tflops_per_sec": world * args.steps * ntiles * SWIN4X_TILE_GFLOP / 1e3 / (ms / 1e3)},
@@ -881,7 +903,7 @@ def run_b200(args):
         "clocks": clocks.summary(),
         "roofline": ({"bound": "tensor", "kernel": views[dom]["kernel"], "class": dom,
                       "achieved": views[dom]["tflops"], "peak": peak_tf, "unit": "TFLOP/s", "frac": views[dom]["tensor_frac"],
-                      "peak_source": f"{peak_src} MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)",
+                      "peak_source": f"{peak_src} bf16_tflops",
                       "launches": views[dom]["launches"], "avg_launch_us": views[dom]["avg_launch_us"],
                       "share_of_step": views[dom]["share_of_step"],
                       "note": "SURVEY 8(d): path A is judged against the tensor roofline.  achieved = algorithmic FLOPs of every launch of "
@@ -920,7 +942,11 @@ def main():
     ap.add_argument("--frame", default=None, choices=list(FRAME), help="frame size (default: the workload's)")
     ap.add_argument("--workload", default="swin4x_4k", choices=list(WORKLOADS) + list(IW3_WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's output(s) as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     if args.cpu_worker:
         cpu_worker_main(*args.cpu_worker)
     elif args.workload in IW3_WORKLOADS:

@@ -1,5 +1,5 @@
 /*
- * nunif_b200 - C ABI of the B200-native engine for nunif's two hot paths.
+ * nunif_b200 - C ABI of the H100 (sm_90a) engine for nunif's two hot paths.
  *
  * The reference (nagadomi/nunif) is pure Python; it has no FFI.  The boundary a
  * maintainer binds is therefore "one C entry point per reference callable on
@@ -16,7 +16,7 @@
  *     Python floats (e.g. float(shift_size * convergence)), and bit-exactness needs the same rounding
  *   - every function returns 0 on success, non-zero on error;
  *     nb200_last_error() returns a thread-local message
- *   - there is no CPU fallback: a call without a usable sm_100 device fails
+ *   - there is no CPU fallback: a call without a usable sm_90 device fails
  */
 #ifndef NUNIF_B200_H
 #define NUNIF_B200_H
@@ -252,7 +252,7 @@ int nb200_anaglyph_dubois(const float* l, const float* r, int B, int H, int W, i
  * materialises it). depth [B][1][h][w] -> out [B][1][H][W]. */
 int nb200_depth_resize_aa(const float* depth, int B, int h, int w, int H, int W, float* out, void* stream);
 
-/* tcgen05 implicit GEMM on NHWC fp16 activations (csrc/gemm_tcgen05.cuh).
+/* wgmma implicit GEMM on NHWC fp16 activations (csrc/gemm_wgmma.cuh).
  * kind: 0 linear over flattened pixels, 1 linear with 2-D tiling, 2 conv3x3 valid (4 = conv3x3 zero-padded by 1),
  *       3 conv2x2 stride 2.  Wt: fp16 [N][taps*Cin] with K ordered (ky, kx, c).
  * act: 0 none, 1 LeakyReLU(0.1), 2 GELU(erf), 3 ReLU.
@@ -270,26 +270,21 @@ int nb200_conv_gemm_f16(const void* A, int B, int Hi, int Wi, int Ci, int Cin, i
 int nb200_window_attention_f16(const void* qkv, const float* bias_table, void* out, int B,
                                int H, int W, int C, int heads, int shift, void* stream);
 
-/* Fused tail of one SwinTransformerBlock (torchvision swin_transformer.py:228 proj, :453-455; MLP = Linear-GELU-Linear,
- * ratio 2, Identity norms: waifu2x/models/swin_unet.py:16-17,31), one tcgen05 kernel (csrc/swin_fused_mlp.cu):
+/* Tail of one SwinTransformerBlock (torchvision swin_transformer.py:228 proj, :453-455; MLP = Linear-GELU-Linear,
+ * ratio 2, Identity norms: waifu2x/models/swin_unet.py:16-17,31), on the engine's GEMM (csrc/swin_block.cu):
  *   x1 = x + att @ wp^T + bp   (att == NULL: x1 = x);   x <- x1 + gelu(x1 @ w1^T + b1) @ w2^T + b2
  * x, att: [T][C] fp16 (x updated in place); wp [C][C], w1 [2C][C], w2 [C][2C] fp16; biases fp32.  C in {96, 192}. */
 int nb200_swin_mlp_fused_f16(void* x, const void* att, long long T, int C, const void* wp,
                              const float* bp, const void* w1, const float* b1, const void* w2,
                              const float* b2, void* stream);
 
-/* Fused head of one SwinTransformerBlock: qkv Linear + shifted 6x6 window attention (swin_transformer.py:166-221;
- * everything but the proj Linear), one kernel (csrc/swin_fused_attn.cu): the qkv GEMM runs on tcgen05, q/k/v stay in
- * shared memory.  x, att: [B][H][W][C] fp16; wqkv [3C][C] fp16 and bqkv [3C] fp32 in the reference's row order
- * (q | k | v); bias_table fp32 [121][6] (relative_position_bias_table).  C in {96, 192}, 6 heads. */
+/* Head of one SwinTransformerBlock: qkv Linear + shifted 6x6 window attention (swin_transformer.py:166-221;
+ * everything but the proj Linear), the engine's GEMM and window-attention kernels (csrc/swin_block.cu).
+ * x, att: [B][H][W][C] fp16; wqkv [3C][C] fp16 and bqkv [3C] fp32 in the reference's row order
+ * (q | k | v), bias_table = relative_position_bias_table [121][6] fp32.  C in {96, 192}, H and W multiples of 6. */
 int nb200_swin_attn_fused_f16(const void* x, const void* wqkv, const float* bqkv,
                               const float* bias_table, void* att, int B, int H, int W, int C,
                               int shift, void* stream);
-/* The same operator and operands with QK^T and PV on tcgen05 as well (csrc/swin_attn_tc.cu: S and P live in tensor
- * memory / shared memory, three windows per 128-row UMMA); this is the kernel the model path launches. */
-int nb200_swin_attn_tc_f16(const void* x, const void* wqkv, const float* bqkv,
-                           const float* bias_table, void* att, int B, int H, int W, int C,
-                           int shift, void* stream);
 
 /* Frame-edge conversions (nunif/utils/video.py:218-223 to_tensor, :236-246 from_tensor,
  * iw3/utils.py:274-289 hwc_to_chw_float): x [B][H][W][3] uint8 (bits=8) or uint16 (bits=16)
@@ -332,9 +327,8 @@ int nb200_equirectangular(const float* c, int C, int H, int W, float* out, void*
 /* Kernel-class device timing (CUDA events around every launch of this library) used by
  * bench.py for the live roofline figure.  report writes a JSON object
  * {"gemm": {"launches": n, "ms": t, "work": flops_or_bytes}, ...} and synchronises the device. */
-int nb200_tune_set(int key, int value);   /* GEMM scheduling knobs for profiles/gemm_bench.py */
-int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermediate `id` of nb200_zoedepth_forward to dev_buf (profiles/debug_zoe.py) */
-int nb200_debug_timeline(void* dev_buf);  /* per-role clock64 timeline of CTA 0 (profiles/gemm_timeline.py) */
+int nb200_tune_set(int key, int value);   /* kernel-selection knobs (csrc/gemm.cu g_tune), for tests and A/B runs */
+int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermediate `id` of nb200_zoedepth_forward to dev_buf */
 int nb200_profile_enable(int on);
 int nb200_profile_report(char* buf, size_t cap);
 int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launch: class,ms,work,read_bytes,write_bytes */

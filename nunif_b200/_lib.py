@@ -2,7 +2,7 @@
 
 PyTorch is only used for device memory and streams: tensors are passed to the
 library as raw device pointers.  There is NO fallback: if the shared library is
-missing, or no sm_100 device is present, calls raise RuntimeError.
+missing, or no sm_90 device is present, calls raise RuntimeError.
 """
 import ctypes
 import os
@@ -95,7 +95,6 @@ SIGNATURES = {
                                     c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),
     "nb200_tune_set": (c_int, [c_int, c_int]),
-    "nb200_debug_timeline": (c_int, [c_void_p]),
     "nb200_debug_tap": (c_int, [c_int, c_void_p, ctypes.c_size_t]),
     "nb200_profile_enable": (c_int, [c_int]),
     "nb200_profile_report": (c_int, [ctypes.c_char_p, c_size_t]),
@@ -104,8 +103,6 @@ SIGNATURES = {
                                          c_void_p, c_void_p, c_void_p]),
     "nb200_swin_attn_fused_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                           c_void_p]),
-    "nb200_swin_attn_tc_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                       c_void_p]),
     "nb200_window_attention_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
 }
 
@@ -121,7 +118,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} is missing: build it with `python -m nunif_b200.build` "
-                "(nvcc, sm_100a).  nunif_b200 has no CPU / PyTorch fallback.")
+                "(nvcc, sm_90a).  nunif_b200 has no CPU / PyTorch fallback.")
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(l, name)
@@ -139,7 +136,7 @@ def check(status):
 def require_cuda(t, name="tensor"):
     import torch
     if not torch.is_tensor(t) or not t.is_cuda:
-        raise RuntimeError(f"nunif_b200: {name} must be a CUDA tensor (the B200 engine has no CPU fallback)")
+        raise RuntimeError(f"nunif_b200: {name} must be a CUDA tensor (the engine has no CPU fallback)")
 
 
 def stream_ptr(device=None):

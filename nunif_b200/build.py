@@ -1,4 +1,4 @@
-"""Build nunif_b200/libnunif_b200.so (sm_100a) with nvcc, in-tree.
+"""Build nunif_b200/libnunif_b200.so (sm_90a, H100) with nvcc, in-tree.
 
 No torch dependency: the library is a plain C-ABI shared object (include/nunif_b200.h),
 cudart is linked statically and libcuda is resolved at run time through
@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libnunif_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I", os.path.join(HERE, "..", "include")]
 
 
@@ -56,7 +56,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=8) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

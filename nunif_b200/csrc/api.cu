@@ -13,10 +13,9 @@ std::atomic<uint64_t> g_launches{0};
 std::atomic<int> g_prof_enabled{0};
 
 struct ProfRec { cudaEvent_t a, b; int cat; double work, rb, wb; };
-// measured HBM rates of this pool (profiles/r1/hbm_microbench.json): copy, write-only, read-only, bytes/s
-// streaming-kernel ceilings measured on this pool (profiles/r1/hbm_mix.json): copy 6.6-6.7, write-only 7.4, read-heavy 7.0 TB/s.
-// (An earlier 3.92 TB/s "write-only limit" was torch's fill_ kernel, not the HBM.)
-static double g_bw_copy = 6.6e12, g_bw_write = 7.4e12, g_bw_read = 7.0e12;
+// HBM rates the per-launch floors are computed with (copy, write-only, read-only, bytes/s): the H100 SXM data-sheet HBM3
+// bandwidth, not a measured ceiling
+static double g_bw_copy = 3.35e12, g_bw_write = 3.35e12, g_bw_read = 3.35e12;
 static std::mutex g_prof_mu;
 static std::vector<ProfRec> g_prof_recs;
 static std::vector<cudaEvent_t> g_prof_pool;
@@ -83,9 +82,9 @@ extern "C" int nb200_check_device(int device) {
     NB_CHECK(device >= 0 && device < n, "device index out of range");
     cudaDeviceProp prop;
     NB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
+    if (prop.major != 9 || prop.minor != 0)   // sm_90a code (wgmma) loads on compute capability 9.0 only
         return fail(std::string("device '") + prop.name + "' is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) +
-                    "; this library is built for sm_100a (B200) only");
+                    "; this library is built for sm_90a (H100) only");
     return 0;
 }
 
@@ -134,7 +133,7 @@ extern "C" int nb200_profile_report(char* buf, size_t cap) {
 }
 
 // Per-launch records of the current profile (one CSV line per timed launch: class,ms,work,read_bytes,write_bytes);
-// profiles/launch_floor.py turns this into the per-launch roofline table.  Synchronises the device.
+// a per-launch roofline table is built from them.  Synchronises the device.
 extern "C" int nb200_profile_dump(char* buf, size_t cap) {
     NB_CHECK(buf && cap > 0, "null buffer");
     NB_CUDA(cudaDeviceSynchronize());

@@ -1,4 +1,4 @@
-// Shared helpers for the nunif_b200 CUDA sources (sm_100a only).
+// Shared helpers for the nunif_b200 CUDA sources (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -63,8 +63,8 @@ struct ProfScope {
 int tile_gather_blend_rows(const void* z_all, int z_f32, int C, const ::nb200_tile_config* cfg, int scale, int offset, int tile_size,
                            int blend_size, float* out, int y0, int y1, void* stream);
 
-// Programmatic dependent launch (sm_90+): a kernel that executes this lets a PDL-attributed successor (the persistent
-// GEMM, gemm.cu launch_p) be scheduled as soon as every CTA of this grid has issued it or exited; the successor blocks in
+// Programmatic dependent launch (sm_90+): a kernel that executes this lets a PDL-attributed successor (the
+// GEMM, gemm.cu launch_t) be scheduled as soon as every CTA of this grid has issued it or exited; the successor blocks in
 // griddepcontrol.wait until this grid has completed and flushed.  A no-op for ordinary successors.
 #define NB_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
 

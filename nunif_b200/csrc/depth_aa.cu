@@ -1,6 +1,6 @@
 // Kernels of `iw3.depth_aa` (iw3/models/depth_aa.py:11-87), the learned anti-aliasing filter Depth-Anything's output goes
 // through when `depth_aa=True` (iw3/depth_anything_model.py:153-154): everything except its Linears / 1x1 / 3x3 convs, which run
-// on the tcgen05 GEMM.  The network works on a pixel_unshuffle(2) grid of 32-channel tokens with three 8x8 window-attention
+// on the wgmma GEMM.  The network works on a pixel_unshuffle(2) grid of 32-channel tokens with three 8x8 window-attention
 // blocks (2 heads of 16; the first and the last shifted by zero padding); ~0.3 GFLOP per 392x686 map: latency kernels.
 #include "depth_aa_kernels.h"
 

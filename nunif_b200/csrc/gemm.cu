@@ -1,7 +1,6 @@
-// Host side of the tcgen05 implicit-GEMM: tensor-map construction and dispatch.
+// Host side of the wgmma implicit-GEMM: tensor-map construction and dispatch.
 #include "gemm.h"
-#include "gemm_tcgen05.cuh"
-#include "gemm_persistent.cuh"
+#include "gemm_wgmma.cuh"
 #include "tmap.h"
 #include <mutex>
 #include <cstdlib>
@@ -45,7 +44,17 @@ template <int BN, int BK>
 static int launch_t(cudaStream_t st, const GemmMaps& maps, const GemmParams& p, int m_tiles, int n_tiles) {
     using Cfg = GemmCfg<BN, BK>;
     if (ensure_dyn_smem((const void*)gemm_conv_kernel<BN, BK>, Cfg::SMEM_BYTES)) return 1;
-    gemm_conv_kernel<BN, BK><<<dim3((unsigned)m_tiles * n_tiles), GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(maps, p);
+    // programmatic dependent launch: this grid may be scheduled while the previous kernel of the stream drains (that kernel
+    // executes griddepcontrol.launch_dependents); barrier set-up and tensor-map prefetch then overlap the predecessor's tail,
+    // and the producer warp blocks in griddepcontrol.wait before the first load.
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)m_tiles * n_tiles); cfg.blockDim = dim3(GEMM_THREADS); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+    cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    NB_CUDA(cudaLaunchKernelEx(&cfg, gemm_conv_kernel<BN, BK>, maps, p));
     NB_LAUNCHED();
     return 0;
 }
@@ -59,103 +68,16 @@ static int launch_bn(int bn, cudaStream_t st, const GemmMaps& maps, const GemmPa
         case 64: return launch_t<64, BK>(st, maps, p, m_tiles, n_tiles);
         case 96: return launch_t<96, BK>(st, maps, p, m_tiles, n_tiles);
         case 128: return launch_t<128, BK>(st, maps, p, m_tiles, n_tiles);
-        case 192: return launch_t<192, BK>(st, maps, p, m_tiles, n_tiles);
-        case 256: return launch_t<256, BK>(st, maps, p, m_tiles, n_tiles);
     }
     return fail("unsupported BLOCK_N");
 }
 
 static int num_sms() { return device_sm_count(); }
 
-constexpr int PG_SMEM_BUDGET = 227 * 1024 - 1024 /*alignment slack*/ - 512 /*barriers*/;
-
-// tuning knobs for profiles/gemm_bench.py (nb200_tune_set); defaults are the shipped configuration
-unsigned long long* g_timeline = nullptr;
+// knobs of nb200_tune_set, read by the kernels' host code; defaults are the shipped configuration
 std::atomic<int> g_tune_epoch{0};
-int g_tune[16] = {/*0 epilogue quads without residual*/ 4, /*1 max A stages*/ PG_MAX_STAGES, /*2 grid cap (0 = #SMs)*/ 0, /*3 force gather backward warp*/ 0,
-                 /*4 forced BLOCK_N*/ 0, /*5 disable GELU->128 rule*/ 0,
-                 /*6 attention smem carveout %*/ 0, /*7 SIMT stem / tail convs*/ 0,
-                  /*8 programmatic dependent launch of the GEMMs*/ 1,
-                  /*9 CUDA-graph replay of nb200_model_forward*/ 0,
-                  /*10 unfused Swin blocks (round-1 launch sequence)*/ 0,
-                  /*11 one-CTA-per-SM fused MLP instead of the half-SM kernel*/ 0,
-                  /*12 mma.sync attention warps (swin_fused_attn.cu) instead of swin_attn_tc.cu*/ 0, 0, 0, 0};
-
-template <int BN, int BK, bool RES>
-static int launch_p(cudaStream_t st, const GemmMaps& maps, PersistParams& pp, int stages, size_t smem, int grid) {
-    if (ensure_dyn_smem((const void*)gemm_conv_persistent<BN, BK, RES>, smem)) return 1;
-    pp.stages = stages;
-    // programmatic dependent launch: this grid may be scheduled while the previous kernel of the stream drains (that kernel
-    // must have executed griddepcontrol.launch_dependents); its prologue (barriers, TMEM, tensor-map prefetch, the static
-    // weight tile) then overlaps the predecessor's tail, and the producer warp blocks in griddepcontrol.wait before the first
-    // activation load.  Without an early trigger in the predecessor this degenerates to ordinary stream order.
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(PG_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = g_tune[8] ? 1 : 0;
-    NB_CUDA(cudaLaunchKernelEx(&cfg, gemm_conv_persistent<BN, BK, RES>, maps, pp));
-    NB_LAUNCHED();
-    return 0;
-}
-
-template <int BN, int BK>
-static int launch_persistent_t(cudaStream_t st, const GemmMaps& maps, const GemmParams& p, int m_tiles) {
-    using Cfg = GemmCfg<BN, BK>;
-    PersistParams pp;
-    pp.g = p;
-    pp.m_tiles = m_tiles;
-    pp.k_iters = p.taps * p.cpt;
-    int grid_m = (g_tune[2] > 0 ? g_tune[2] : num_sms()) / p.n_tiles;
-    if (grid_m < 1) grid_m = 1;
-    if (grid_m > m_tiles) grid_m = m_tiles;
-    pp.grid_m = grid_m;
-    const int grid = grid_m * p.n_tiles;
-    constexpr int b_chunk = ((Cfg::B_BYTES + 1023) / 1024) * 1024;
-    pp.nq = p.has_res ? 3 : g_tune[0];
-    // the quads' chunks in flight must never span more than the TMEM accumulator ring (mbarrier phases are 1 bit)
-    if (pp.nq > PgAcc<BN>::NACC * Cfg::NCH) pp.nq = PgAcc<BN>::NACC * Cfg::NCH;
-    pp.timeline = g_timeline;
-    const int stg = pp.nq * (p.has_res ? 2 : 1) * Cfg::CH_BYTES + BN * 4 /*bias*/;
-    // weights resident in shared memory when they fit next to >= 3 activation stages
-    const long long bres = (long long)pp.k_iters * b_chunk;
-    const long long room_res = (long long)PG_SMEM_BUDGET - stg - bres;
-    if (room_res >= 3LL * Cfg::A_BYTES) {
-        int stages = (int)(room_res / Cfg::A_BYTES);
-        if (stages > g_tune[1]) stages = g_tune[1];
-        const size_t smem = (size_t)bres + (size_t)stages * Cfg::A_BYTES + stg + 1024 + 512;
-        return launch_p<BN, BK, true>(st, maps, pp, stages, smem, grid);
-    }
-    const int stage_bytes = Cfg::A_BYTES + b_chunk;
-    int stages = (PG_SMEM_BUDGET - stg) / stage_bytes;
-    if (stages > PG_MAX_STAGES) stages = PG_MAX_STAGES;
-    if (stages < 2) return fail("persistent GEMM: tile does not fit shared memory");
-    const size_t smem = (size_t)stages * stage_bytes + stg + 1024 + 512;
-    return launch_p<BN, BK, false>(st, maps, pp, stages, smem, grid);
-}
-
-template <int BK>
-static int launch_persistent_bn(int bn, cudaStream_t st, const GemmMaps& maps, const GemmParams& p, int m_tiles) {
-    switch (bn) {
-        case 16: return launch_persistent_t<16, BK>(st, maps, p, m_tiles);
-        case 32: return launch_persistent_t<32, BK>(st, maps, p, m_tiles);
-        case 48: return launch_persistent_t<48, BK>(st, maps, p, m_tiles);
-        case 64: return launch_persistent_t<64, BK>(st, maps, p, m_tiles);
-        case 96: return launch_persistent_t<96, BK>(st, maps, p, m_tiles);
-        case 128: return launch_persistent_t<128, BK>(st, maps, p, m_tiles);
-        case 192: return launch_persistent_t<192, BK>(st, maps, p, m_tiles);
-        case 256: return launch_persistent_t<256, BK>(st, maps, p, m_tiles);
-    }
-    return fail("unsupported BLOCK_N");
-}
-
-int pick_block_n(int N) {
-    static const int cands[] = {256, 192, 128, 96, 64, 48, 32, 16};
-    for (int c : cands)
-        if (N % c == 0) return c;
-    return 0;
-}
+int g_tune[16] = {0, 0, 0, /*3 force gather backward warp*/ 0, 0, 0, /*6 attention smem carveout %*/ 0,
+                  /*7 SIMT stem / tail convs*/ 0, 0, /*9 CUDA-graph replay of nb200_model_forward*/ 0, 0, 0, 0, 0, 0, 0};
 
 // 4-D NHWC view (c, x, y, b) of an fp16 tensor for the epilogue's TMA stores / residual loads
 static int encode_nhwc4(CUtensorMap* m, const __half* base, int C, int X, int Y, int B, long long sx, long long sy, long long sb,
@@ -219,7 +141,6 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
     }
     NB_CHECK(ktap % 32 == 0, "K per tap must be a multiple of 32");
     const int BK = (ktap % 64 == 0) ? 64 : 32;
-    const int BKsel = BK;
     p.cpt = ktap / BK;
     p.tiles_x = cdiv(p.Wo, p.TW);
     p.tiles_y = cdiv(p.Ho, p.TH);
@@ -238,43 +159,20 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
         NB_CHECK(g.cout % 16 == 0 && g.N == 4 * g.cout, "pixel-shuffle: N must be 4*cout, cout % 16 == 0");
     }
     NB_CHECK(g.ldo % 8 == 0 && (!g.res || g.ldr % 8 == 0), "channel strides must be multiples of 8");
-    // largest BLOCK_N dividing N whose store chunk (64/32/16 columns) does not straddle a pixel-shuffle group
+    // largest BLOCK_N (<= 128: the accumulators live in registers) dividing N whose store chunk (64/32/16 columns) does not
+    // straddle a pixel-shuffle group or a split plane
     int bn = 0, cw = 0;
-    {
-        static const int cands[] = {256, 192, 128, 96, 64, 48, 32, 16};
-        // first choice: the largest BLOCK_N whose weight tile can stay resident in shared memory next to >= 3 activation
-        // stages and the epilogue staging (residual launches stage twice as much); else the largest valid one
-        const int Ktot = p.taps * ktap;
-        int first_bn = 0, first_cw = 0;
-        for (int c : cands) {
-            const int w = (c % 64 == 0) ? 64 : ((c % 32 == 0) ? 32 : 16);
-            if (!(g.N % c == 0 && (!shuf || g.cout % w == 0) && (!split || g.cout % c == 0))) continue;
-            if (!first_bn) { first_bn = c; first_cw = w; }
-            const long long stg = (long long)(g.res ? 3 * 2 : 4) * 128 * w * 2 + c * 4;
-            const long long bres = (long long)Ktot * (((c * BKsel * 2 + 1023) / 1024) * 1024) / BKsel;
-            // (only 64-column-chunk tiles of >= 128 columns are considered worth the extra n-tiles: fc2 with K = 384 is faster
-            //  streaming a 192-wide weight tile than resident at 96, profiles/r1/gemm_bench_v4.json)
-            if (c >= 128 && w == 64 && bres + 3LL * 128 * BKsel * 2 + stg <= PG_SMEM_BUDGET) { bn = c; cw = w; break; }
-        }
-        if (!bn) { bn = first_bn; cw = first_cw; }
-        // epilogue-heavy launches (GELU): narrower tiles give a 4-deep TMEM accumulator ring, so the quads
-        // rarely wait for the MMA (profiles/r1/timeline_fc1_*.txt); chunks never straddle a split plane (cout % 64 == 0)
-        // residual launches with K = N = 192 (the Swin proj Linear): 64-wide tiles keep 24 KB of weights resident instead
-        // of 72 KB, which doubles the activation ring (3 -> 6 stages) next to the residual/output staging;
-        // profiles/r1/gemm_bench_v4.json: 197 -> 177 us
-        const bool narrow_res = g.res && g.N == 192 && p.taps * ktap == 192 && g_tune[5] == 0;
-        const int forced = g_tune[4] > 0 ? g_tune[4] : ((g.act == ACT_GELU && g_tune[5] == 0) ? 128 : (narrow_res ? 64 : 0));
-        if (forced > 0 && g.N % forced == 0 && !shuf) {
-            const int w = (forced % 64 == 0) ? 64 : ((forced % 32 == 0) ? 32 : 16);
-            if (!split || g.cout % w == 0) { bn = forced; cw = w; }
-        }
+    static const int cands[] = {128, 96, 64, 48, 32, 16};
+    for (int c : cands) {
+        const int w = (c % 64 == 0) ? 64 : ((c % 32 == 0) ? 32 : 16);
+        if (g.N % c == 0 && (!shuf || g.cout % w == 0) && (!split || g.cout % c == 0)) { bn = c; cw = w; break; }
     }
     NB_CHECK(bn > 0, "no BLOCK_N divides N");
-    if (g_tune[4] == 0 && !shuf) {
-        // small-M launches (ViT tokens of a few frames, coarse DPT levels): prefer narrower tiles until the persistent grid
+    if (!shuf) {
+        // small-M launches (ViT tokens of a few frames, coarse DPT levels): prefer narrower tiles until the grid
         // (m-tiles x n-tiles) covers most SMs; the activation tile is then re-read from L2 by the extra n-tiles
         const long long m_tiles_est = (long long)p.tiles_x * p.tiles_y * p.B;
-        static const int narrower[] = {128, 96, 64};
+        static const int narrower[] = {96, 64};
         for (int c : narrower) {
             if ((long long)(g.N / bn) * m_tiles_est >= (long long)num_sms() * 3 / 4) break;
             if (c >= bn || g.N % c) continue;
@@ -331,9 +229,7 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
     ProfScope ps(st, PC_GEMM, 2.0 * Mrows * (double)g.N * (double)K,
                  in_px * (g.kind == CG_LINEAR_FLAT ? g.Cin * g.a_planes : g.Cin) * 2.0 + (g.res ? Mrows * g.N * 2.0 : 0.0) + (double)g.N * K * 2.0,
                  Mrows * (double)g.N * 2.0);
-    static const bool legacy = getenv("NB200_GEMM_NONPERSISTENT") != nullptr;  // A/B switch for profiling only
-    if (legacy) return BK == 64 ? launch_bn<64>(bn, st, maps, p, m_tiles, p.n_tiles) : launch_bn<32>(bn, st, maps, p, m_tiles, p.n_tiles);
-    return BK == 64 ? launch_persistent_bn<64>(bn, st, maps, p, m_tiles) : launch_persistent_bn<32>(bn, st, maps, p, m_tiles);
+    return BK == 64 ? launch_bn<64>(bn, st, maps, p, m_tiles, p.n_tiles) : launch_bn<32>(bn, st, maps, p, m_tiles, p.n_tiles);
 }
 
 }  // namespace nb200
@@ -353,12 +249,6 @@ extern "C" int nb200_conv_gemm_f16(const void* A, int B, int Hi, int Wi, int Ci,
     g.out_mode = out_mode; g.cout = cout; g.res = (const __half*)res; g.ldr = ldr; g.res_H = res_H; g.res_W = res_W;
     g.res_cy = res_cy; g.res_cx = res_cx; g.res_before_act = res_before_act;
     return conv_gemm((cudaStream_t)stream, g);
-}
-
-// debug: device buffer of 4096 u64 that CTA 0 of every following persistent GEMM fills with (event<<56 | clock)
-extern "C" int nb200_debug_timeline(void* dev_buf) {
-    g_timeline = (unsigned long long*)dev_buf;
-    return 0;
 }
 
 // profiling knobs (see g_tune in this file); not part of the reference-facing API

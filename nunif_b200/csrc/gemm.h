@@ -1,4 +1,4 @@
-// Host interface of the tcgen05 implicit-GEMM (see gemm_tcgen05.cuh).
+// Host interface of the wgmma implicit-GEMM (see gemm_wgmma.cuh).
 #pragma once
 #include "common.cuh"
 
@@ -30,6 +30,5 @@ struct ConvGemm {
 };
 
 int conv_gemm(cudaStream_t st, const ConvGemm& g);
-int pick_block_n(int N);
 
 }  // namespace nb200

@@ -1,5 +1,5 @@
 // Kernels of `sbs.mlbw` (iw3/models/mlbw.py:36-127), the multi-layer learned stereo warp (methods mlbw_l2 / mlbw_l4 [s]): everything
-// except its Linears / 1x1 / 3x3 convs, which run on the tcgen05 GEMM.  Like row_flow_v3 the network works on a (1, 8)
+// except its Linears / 1x1 / 3x3 convs, which run on the wgmma GEMM.  Like row_flow_v3 the network works on a (1, 8)
 // pixel-unshuffled token grid; it predicts L horizontal flow layers and L blending weights per pixel.
 #include "mlbw_kernels.h"
 

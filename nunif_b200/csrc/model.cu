@@ -1,9 +1,9 @@
 // Model containers: weight packing from the reference's state_dict keys and the
 // forward passes of SwinUNet (swin_unet.py:119-199) and CUNet/UpCUNet (cunet.py:10-203)
-// expressed as sequences of the sm_100a kernels.  Also the whole-image tiled render.
+// expressed as sequences of the sm_90a kernels.  Also the whole-image tiled render.
 #include "common.cuh"
 #include "gemm.h"
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "swin_kernels.h"
 #include "cunet_kernels.h"
 #include "depth_kernels.h"
@@ -11,7 +11,6 @@
 #include "depth_aa_kernels.h"
 #include "mlbw_kernels.h"
 #include "zoe_kernels.h"
-#include "swin_fused.h"
 #include "../../include/nunif_b200.h"
 #include <map>
 #include <vector>
@@ -25,7 +24,6 @@ namespace nb200 {
 
 extern int g_tune[16];                 // gemm.cu (nb200_tune_set)
 extern std::atomic<int> g_tune_epoch;  // gemm.cu: bumped by every nb200_tune_set (captured graphs bake the knobs in)
-extern unsigned long long* g_timeline;  // gemm.cu (nb200_debug_timeline)
 
 // ---------------------------------------------------------------------------------------------
 // weight packing
@@ -191,12 +189,7 @@ static Lin pack_stem(Packer& pk, const std::string& name, int cout, int cout_pad
 
 struct SwinBlockW {
     Lin qkv, proj, fc1, fc2;
-    Lin qkv_fused;        // rows regrouped per head pair for swin_fused_attn.cu
-    size_t fc1_cm = 0, proj_cm = 0;   // chunk-major [K/BK][rows][BK] fp16 copies for swin_fused_mlp2.cu
-    size_t table = 0;     // bias in accumulator-fragment order (unfused attention kernel)
-    size_t btab = 0;      // bias as [6][36][40] fp32 (fused attention kernel)
-    Lin qkv_tc;           // rows regrouped per 96-column unit for swin_attn_tc.cu
-    size_t btab_tc = 0;   // relative_position_bias_table [121][6] fp32 as stored
+    size_t table = 0;     // bias in accumulator-fragment order (attention kernel)
     int C = 0, shift = 0;
 };
 
@@ -292,49 +285,9 @@ static void pack_swin_blocks(Packer& pk, std::vector<SwinBlockW>& out, const std
         b.C = C;
         b.shift = (i % 2 == 0) ? 0 : 3;  // swin_unet.py:30
         b.qkv = pack_linear(pk, p + ".attn.qkv", 3 * C, C);
-        {   // the same Linear with rows ordered (head pair, {q,k,v}, head in pair, d): one N = 6d GEMM chunk per head pair
-            const float* w = pk.get(p + ".attn.qkv.weight", (int64_t)3 * C * C);
-            const float* bq = pk.get(p + ".attn.qkv.bias", 3 * C);
-            if (w && bq) {
-                const int D = C / 6;
-                std::vector<float> wv((size_t)3 * C * C), bv(3 * C);
-                for (int pr = 0; pr < 3 * C; ++pr) {
-                    const int c = pr / (6 * D), rem = pr % (6 * D);
-                    const int mm = rem / (2 * D), hh = (rem % (2 * D)) / D, d = rem % D;
-                    const int src = mm * C + (2 * c + hh) * D + d;
-                    memcpy(&wv[(size_t)pr * C], &w[(size_t)src * C], (size_t)C * 4);
-                    bv[pr] = bq[src];
-                }
-                b.qkv_fused.N = 3 * C; b.qkv_fused.K = C;
-                b.qkv_fused.w = pk.add_f16(wv);
-                b.qkv_fused.b = pk.add_f32(bv);
-                // swin_attn_tc.cu: 96 rows per unit = one head (C = 192) or a head pair (C = 96), [q | k | v] inside
-                for (int pr = 0; pr < 3 * C; ++pr) {
-                    const int src = swin_attn_tc_src_row(pr, C);
-                    memcpy(&wv[(size_t)pr * C], &w[(size_t)src * C], (size_t)C * 4);
-                    bv[pr] = bq[src];
-                }
-                b.qkv_tc.N = 3 * C; b.qkv_tc.K = C;
-                b.qkv_tc.w = pk.add_f16(wv);
-                b.qkv_tc.b = pk.add_f32(bv);
-            }
-        }
         b.proj = pack_linear(pk, p + ".attn.proj", C, C);
         b.fc1 = pack_linear(pk, p + ".mlp.0", 2 * C, C);
         b.fc2 = pack_linear(pk, p + ".mlp.3", C, 2 * C);
-        {   // chunk-major copies: all K-chunks of one GEMM chunk arrive with a single 3-D TMA box
-            const int bk = C == 192 ? 64 : 32;
-            auto cm = [&](const std::string& name, int rows, int K) -> size_t {
-                const float* w = pk.get(name, (int64_t)rows * K);
-                if (!w) return 0;
-                std::vector<float> v((size_t)rows * K);
-                for (int r = 0; r < rows; ++r)
-                    for (int k = 0; k < K; ++k) v[((size_t)(k / bk) * rows + r) * bk + (k % bk)] = w[(size_t)r * K + k];
-                return pk.add_f16(v);
-            };
-            b.fc1_cm = cm(p + ".mlp.0.weight", 2 * C, C);
-            b.proj_cm = cm(p + ".attn.proj.weight", C, C);
-        }
         const float* t = pk.get(p + ".attn.relative_position_bias_table", 121 * 6);
         if (t) {
             // relative-position bias expanded once into the attention kernel's accumulator-fragment order
@@ -357,16 +310,6 @@ static void pack_swin_blocks(Packer& pk, std::vector<SwinBlockW>& out, const std
                                 frag[((((size_t)head * 3 + mt) * 6 + nt) * 32 + lane) * 4 + r] = v;
                             }
             b.table = pk.add_f32(frag);
-            // [head][36 queries][40 keys]: log2(e) * bias, key columns 36..39 masked (swin_fused_attn.cu)
-            std::vector<float> tab((size_t)6 * 36 * 40, -1e30f);
-            for (int head = 0; head < 6; ++head)
-                for (int row = 0; row < 36; ++row)
-                    for (int col = 0; col < 36; ++col) {
-                        const int qy = row / 6, qx = row % 6, ky = col / 6, kx = col % 6;
-                        tab[((size_t)head * 36 + row) * 40 + col] = 1.4426950408889634f * t[((qy - ky + 5) * 11 + (qx - kx + 5)) * 6 + head];
-                    }
-            b.btab = pk.add_f32(tab);
-            b.btab_tc = pk.add_f32(std::vector<float>(t, t + 121 * 6));
         }
         pk.mark(p + ".attn.relative_position_index");  // buffer; the kernel recomputes the index (swin_transformer.py:267-279)
         out.push_back(b);
@@ -426,47 +369,13 @@ static int linear_flat(cudaStream_t st, const nb200_model* m, const Lin& l, cons
     return conv_gemm(st, g);
 }
 
-static int swin_block(cudaStream_t st, const nb200_model* m, const SwinBlockW& w, __half* X, int n, int H, __half* QKV, __half* ATT,
-                      __half* HID) {
+static int swin_block(cudaStream_t st, const nb200_model* m, const SwinBlockW& w, __half* X, int n, int H, __half* ATT) {
     const int C = w.C;
     const long long T = (long long)n * H * H;
-    if (g_tune[10] == 0) {
-        // two launches per block (swin_fused_attn.cu, swin_fused_mlp.cu): q/k/v, x1 and the hidden tensor never reach HBM
-        FusedAttn fa;
-        fa.x = X; fa.att = ATT; fa.B = n; fa.H = H; fa.W = H; fa.C = C; fa.shift = w.shift;
-        fa.wqkv = m->at<__half>(w.qkv_fused.w); fa.bqkv = m->at<float>(w.qkv_fused.b); fa.bias_tab = m->at<float>(w.btab);
-        fa.wqkv_tc = m->at<__half>(w.qkv_tc.w); fa.bqkv_tc = m->at<float>(w.qkv_tc.b); fa.bias_tab_tc = m->at<float>(w.btab_tc);
-        // g_tune[12] != 0: the round-2a kernel (mma.sync attention warps) for A/B measurements
-        if (g_tune[12] ? swin_attn_fused(st, fa) : swin_attn_tc(st, fa)) return 1;
-        FusedMlp fm;
-        fm.x = X; fm.att = ATT; fm.T = T; fm.C = C;
-        fm.wp = m->at<__half>(w.proj.w); fm.bp = m->at<float>(w.proj.b);
-        fm.w1 = m->at<__half>(w.fc1.w); fm.b1 = m->at<float>(w.fc1.b);
-        fm.w2 = m->at<__half>(w.fc2.w); fm.b2 = m->at<float>(w.fc2.b);
-        fm.w1_cm = m->at<__half>(w.fc1_cm); fm.wp_cm = m->at<__half>(w.proj_cm);
-        if (g_tune[11]) return swin_mlp_fused(st, fm);        // one CTA per SM, proj fused (A/B)
-        // half-SM kernels, two CTAs per SM (swin_fused_mlp2.cu).  C = 192 has no shared memory for the att tile next to a
-        // second CTA: its proj Linear (+ residual) runs on the persistent GEMM and the MLP kernel starts from x1.
-        if (C == 192) {
-            if (linear_flat(st, m, w.proj, ATT, T, C, X, C, ACT_NONE, X, C)) return 1;    // x = x + attn(x)   :453
-            fm.att = nullptr;
-        }
-        return swin_mlp_fused2(st, fm);
-    }
-    // unfused path (nb200_tune_set(10, 1); kept for A/B measurements).  q | k | v are written as three dense [T][C] planes: every CTA stores whole contiguous rows, and the
-    // attention kernel reads each matrix with unit stride
-    if (linear_flat(st, m, w.qkv, X, T, C, QKV, C, ACT_NONE, nullptr, 0, /*split=*/C)) return 1;
-    if (window_attention(st, QKV, m->at<float>(w.table), ATT, n, H, H, C, w.shift, (size_t)T * C)) return 1;
-    if (linear_flat(st, m, w.proj, ATT, T, C, X, C, ACT_NONE, X, C)) return 1;       // x = x + attn(x)   :453
-    if (C == 192) {
-        // hidden = 2 planes of [T][192] (same reason); fc2 consumes them as two K-taps
-        if (linear_flat(st, m, w.fc1, X, T, C, HID, C, ACT_GELU, nullptr, 0, /*split=*/C)) return 1;
-        if (linear_flat(st, m, w.fc2, HID, T, C, X, C, ACT_NONE, X, C, 0, /*a_planes=*/2)) return 1;  // x = x + mlp(x) :454
-    } else {
-        if (linear_flat(st, m, w.fc1, X, T, C, HID, 2 * C, ACT_GELU)) return 1;
-        if (linear_flat(st, m, w.fc2, HID, T, 2 * C, X, C, ACT_NONE, X, C)) return 1;
-    }
-    return 0;
+    // two launches per block: q/k/v, x1 and the hidden tensor stay in shared memory / registers
+    if (swin_attn_fused(st, X, m->at<__half>(w.qkv.w), m->at<float>(w.qkv.b), m->at<float>(w.table), ATT, n, H, H, C, w.shift)) return 1;
+    return swin_mlp_fused(st, X, ATT, T, C, m->at<__half>(w.proj.w), m->at<float>(w.proj.b), m->at<__half>(w.fc1.w), m->at<float>(w.fc1.b),
+                          m->at<__half>(w.fc2.w), m->at<float>(w.fc2.b));
 }
 
 static size_t swin_ws_bytes(const SwinW& w, int n, int T) {
@@ -476,9 +385,7 @@ static size_t swin_ws_bytes(const SwinW& w, int n, int T) {
     auto add = [&](size_t elems) { b += ((elems * 2 + 255) & ~(size_t)255) + 256; };
     add((size_t)n * (T - 2) * (T - 2) * 64);  // S1
     add(t1 * C);                              // X1
-    add(t1 * 3 * C5);                         // QKV (largest stage: swin5, or swin1)
     add(t1 * C5);                             // ATT
-    add(t1 * 2 * C5);                         // HID
     add(t1 / 4 * 2 * C);                      // X2
     add(t1 / 16 * 2 * C);                     // X3
     add(t1 / 4 * 2 * C);                      // X4
@@ -498,9 +405,7 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
     const size_t t1 = (size_t)n * Hc * Hc;
     __half* S1 = a.take<__half>((size_t)n * S1w * S1w * 64);
     __half* X1 = a.take<__half>(t1 * C);
-    __half* QKV = a.take<__half>(t1 * 3 * C5);
     __half* ATT = a.take<__half>(t1 * C5);
-    __half* HID = a.take<__half>(t1 * 2 * C5);
     __half* X2 = a.take<__half>(t1 / 4 * 2 * C);
     __half* X3 = a.take<__half>(t1 / 16 * 2 * C);
     __half* X4 = a.take<__half>(t1 / 4 * 2 * C);
@@ -517,21 +422,21 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
         g.Wt = m->at<__half>(w.conv2.w); g.N = C; g.bias = m->at<float>(w.conv2.b); g.act = ACT_LRELU01; g.out = X1; g.ldo = C;
         if (conv_gemm(st, g)) return 1;
     }
-    for (const auto& b : w.s1) if (swin_block(st, m, b, X1, n, Hc, QKV, ATT, HID)) return 1;   // x3
+    for (const auto& b : w.s1) if (swin_block(st, m, b, X1, n, Hc, ATT)) return 1;   // x3
     {   // down1 (swin_unet.py:45-62)
         ConvGemm g;
         g.A = X1; g.B = n; g.Hi = Hc; g.Wi = Hc; g.Ci = C; g.Cin = C; g.kind = CG_DOWN2;
         g.Wt = m->at<__half>(w.down1.w); g.N = 2 * C; g.bias = m->at<float>(w.down1.b); g.out = X2; g.ldo = 2 * C;
         if (conv_gemm(st, g)) return 1;
     }
-    for (const auto& b : w.s2) if (swin_block(st, m, b, X2, n, H2, QKV, ATT, HID)) return 1;   // x4
+    for (const auto& b : w.s2) if (swin_block(st, m, b, X2, n, H2, ATT)) return 1;   // x4
     {   // down2
         ConvGemm g;
         g.A = X2; g.B = n; g.Hi = H2; g.Wi = H2; g.Ci = 2 * C; g.Cin = 2 * C; g.kind = CG_DOWN2;
         g.Wt = m->at<__half>(w.down2.w); g.N = 2 * C; g.bias = m->at<float>(w.down2.b); g.out = X3; g.ldo = 2 * C;
         if (conv_gemm(st, g)) return 1;
     }
-    for (const auto& b : w.s3) if (swin_block(st, m, b, X3, n, H3, QKV, ATT, HID)) return 1;   // x5
+    for (const auto& b : w.s3) if (swin_block(st, m, b, X3, n, H3, ATT)) return 1;   // x5
     {   // up2 + skip: x = up2(x5) + x4   (swin_unet.py:190-191)
         ConvGemm g;
         g.A = X3; g.B = n; g.Hi = H3; g.Wi = H3; g.Ci = 2 * C; g.Cin = 2 * C; g.kind = CG_LINEAR_2D;
@@ -539,7 +444,7 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
         g.out_mode = OUT_PIXSHUF2; g.cout = 2 * C; g.res = X2; g.ldr = 2 * C; g.res_H = H2; g.res_W = H2;
         if (conv_gemm(st, g)) return 1;
     }
-    for (const auto& b : w.s4) if (swin_block(st, m, b, X4, n, H2, QKV, ATT, HID)) return 1;
+    for (const auto& b : w.s4) if (swin_block(st, m, b, X4, n, H2, ATT)) return 1;
     const __half* skip = X1;
     if (w.r == 4) {  // proj2(x3), swin_unet.py:159,195
         if (linear_flat(st, m, w.proj2, X1, (long long)t1, C, P2, 2 * C, ACT_NONE)) return 1;
@@ -552,7 +457,7 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
         g.out_mode = OUT_PIXSHUF2; g.cout = C5; g.res = skip; g.ldr = C5; g.res_H = Hc; g.res_W = Hc;
         if (conv_gemm(st, g)) return 1;
     }
-    for (const auto& b : w.s5) if (swin_block(st, m, b, X5, n, Hc, QKV, ATT, HID)) return 1;
+    for (const auto& b : w.s5) if (swin_block(st, m, b, X5, n, Hc, ATT)) return 1;
     if (linear_flat(st, m, w.toimg, X5, (long long)t1, C5, Y, w.cs, ACT_NONE)) return 1;      // ToImage.proj :109
     return to_image(st, Y, z, n, Hc, Hc, w.cs, w.r, down);
 }
@@ -560,7 +465,7 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
 }  // namespace nb200
 
 #include "cunet_model.inl"
-// debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth forward is copied to `g_tap_buf` (profiles/debug_zoe.py)
+// debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth forward is copied to `g_tap_buf`
 static int g_tap_id = -1;
 static void* g_tap_buf = nullptr;
 static size_t g_tap_cap = 0;
@@ -684,9 +589,9 @@ extern "C" int nb200_model_forward(nb200_model* m, const void* x, int n, int til
         return cunet_forward(m, st, (const __half*)x, n, tile_size, (__half*)z);
     };
     // CUDA graphs (g_tune[9]): the ~80 launches of one tile batch are replayed as one graph launch once the same
-    // (buffers, shape) has been seen twice; removes most of the inter-kernel launch latency (≈7 % of a 4K frame,
-    // profiles/r1/launches_bench_step_summary.txt).  Never while the event profiler or the timeline probe is on.
-    if (!g_tune[9] || g_prof_enabled.load(std::memory_order_relaxed) || g_timeline) return eager();
+    // (buffers, shape) has been seen twice; removes most of the inter-kernel launch latency.  Never while the event
+    // profiler is on.
+    if (!g_tune[9] || g_prof_enabled.load(std::memory_order_relaxed)) return eager();
     if (m->graph_epoch != g_tune_epoch.load()) {            // a tuning knob changed: the captured launch configurations are stale
         m->clear_graphs();
         m->graph_epoch = g_tune_epoch.load();

@@ -1,5 +1,5 @@
 // Kernels of `sbs.row_flow_v3` (iw3/models/row_flow_v3.py:14-68), the learned row-flow stereo warp that is iw3's CLI
-// default method: everything except its Linears / 1x1 / 3x3 convs, which run on the tcgen05 GEMM.  The network works on
+// default method: everything except its Linears / 1x1 / 3x3 convs, which run on the wgmma GEMM.  The network works on
 // a (1, 8) pixel-unshuffled grid of 64-channel tokens with two tiny window-attention blocks (4x4 and 3x3 windows,
 // 2 heads of 32); per frame it is ~1 GFLOP, so these are bandwidth/latency kernels.
 #include "rowflow_kernels.h"

@@ -9,13 +9,15 @@
 //   O = P V           : the S fragments are re-packed in registers as the A operand (no smem trip),
 //                       V fragments come from ldmatrix.trans
 // torchvision swin_transformer.py:166-221 (roll, partition, bias :190, mask :193-209, softmax :211,
-// attn@v :214, un-roll) - everything but the qkv / proj Linears, which run on the tcgen05 GEMM.
+// attn@v :214, un-roll) - everything but the qkv / proj Linears, which run on the wgmma GEMM.
 //
-// The 36x36 problem per head is far too small for a tcgen05 tile (M=128), and the op moves
+// The 36x36 problem per head is far too small for a 64-row wgmma tile, and the op moves
 // 8*C bytes/token for ~144*C FLOP/token: it is HBM/L2-bound, so the warp-level HMMA path is the
 // right instrument here (DESIGN.md 4.2).
 #include "common.cuh"
+#include "gemm_wgmma.cuh"
 #include "swin_kernels.h"
+#include "tmap.h"
 #include <map>
 #include <mutex>
 
@@ -333,6 +335,207 @@ int window_attention(cudaStream_t st, const __half* qkv, const float* bias_frag_
         const int want = g_tune[6] > 0 ? g_tune[6] : 86;
         if (set_attn_attrs((const void*)window_attention_mma_kernel<32>, attn_smem_bytes<32>(), want)) return 1;
         window_attention_mma_kernel<32><<<grid, 192, attn_smem_bytes<32>(), st>>>(qkv, bias_table, out, H, W, shift, plane);
+    }
+    NB_LAUNCHED();
+    return 0;
+}
+
+
+// ---------------------------------------------------------------------------------------------
+// Fused block head: att = window_attention_core(x . Wqkv^T + bqkv), q/k/v never leave shared memory.
+// One CTA = 3 windows = 108 tokens (+20 zero rows) = the 128 rows of two wgmma warpgroups.
+//   warp 8    : TMA producer of the weight blocks [96 rows][32] (64B swizzle), 3C/96 column chunks x C/32 K-blocks
+//   warps 0-7 : gather the rolled window tokens into a swizzled [128][C] A tile; per 96-column chunk of q|k|v one
+//               wgmma accumulation (M = 64 per warpgroup), bias, fp16 into the per-window q/k/v tiles of the
+//               mma.sync attention core (attn_mtile, the same code as window_attention_mma_kernel); then the 18
+//               (window, head) pairs on the 8 warps, and the un-rolled rows back to HBM.
+// ---------------------------------------------------------------------------------------------
+constexpr int FA_ROWS = 128, FA_WIN = 3, FA_THREADS = GEMM_CONSUMER_THREADS + 32, FA_SLOT = 96 * 64;
+
+template <int C>
+struct FaCfg {
+    // C = 96: 2 weight stages keep the CTA at ~104 KB so that two CTAs (and their GEMM / attention phases) share an SM
+    static constexpr int STAGES = C == 96 ? 2 : 4, MIN_CTAS = C == 96 ? 2 : 1;
+    static constexpr int LD = C + 8;
+    static constexpr int X_BYTES = FA_ROWS * C * 2;
+    static constexpr int QKV_BYTES = FA_WIN * 3 * WTOK * LD * 2;
+    static constexpr int SMEM = X_BYTES + STAGES * FA_SLOT + QKV_BYTES + FA_WIN * (WTOK + WPAD) * 4 + 2 * STAGES * 8 + 1024;
+};
+
+template <int C>
+__global__ void __launch_bounds__(FA_THREADS, FaCfg<C>::MIN_CTAS) swin_attn_fused_kernel(const __grid_constant__ CUtensorMap wmap,
+                                                                        const __half* __restrict__ x, const float* __restrict__ bqkv,
+                                                                        const float4* __restrict__ bias_frag, __half* __restrict__ out,
+                                                                        int H, int W, int shift, int nwin) {
+    using Cfg = FaCfg<C>;
+    constexpr int D = C / HEADS, LD = Cfg::LD, KB = C / 32, NCH = 3 * C / 96;
+    extern __shared__ uint8_t smem_dyn[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+    uint8_t* sx = smem;
+    uint8_t* ring = smem + Cfg::X_BYTES;
+    __half* sqkv = reinterpret_cast<__half*>(ring + Cfg::STAGES * FA_SLOT);   // [window][q|k|v][WTOK][LD]
+    int* stok = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(sqkv) + Cfg::QKV_BYTES);   // [window][WTOK], -1 = none
+    int* sreg = stok + FA_WIN * WTOK;                                                         // [window][WPAD]
+    uint64_t* full = reinterpret_cast<uint64_t*>(sreg + FA_WIN * WPAD);
+    uint64_t* empty = full + Cfg::STAGES;
+    const int tid = threadIdx.x, warp = tid >> 5;
+    const int nww = W / WS, nwy = H / WS;
+    if (tid < FA_WIN * WPAD) {
+        const int w = tid / WPAD, t = tid % WPAD, gw = blockIdx.x * FA_WIN + w;
+        int reg = -1;
+        if (t < WTOK) {
+            int tok = -1;
+            if (gw < nwin) {
+                const int b = gw / (nww * nwy), r = gw % (nww * nwy), wy = r / nww, wx = r % nww;
+                const int ry = wy * WS + t / WS, rx = wx * WS + t % WS;       // rolled coordinates
+                const int y = (ry + shift) % H, xx = (rx + shift) % W;        // torch.roll(-shift) :166-167
+                tok = (b * H + y) * W + xx;
+                int hr = 0, wr = 0;
+                if (shift > 0) {
+                    hr = ry < H - WS ? 0 : (ry < H - shift ? 1 : 2);
+                    wr = rx < W - WS ? 0 : (rx < W - shift ? 1 : 2);
+                }
+                reg = hr * 3 + wr;
+            }
+            stok[w * WTOK + t] = tok;
+        }
+        sreg[w * WPAD + t] = reg;
+    }
+    if (tid == GEMM_CONSUMER_THREADS) {
+        tma_prefetch_desc(&wmap);
+        for (int s = 0; s < Cfg::STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 2);   // one arrival per consumer warpgroup
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (warp == GEMM_CONSUMER_THREADS / 32) {
+        // ===================== weight producer =====================
+        if (elect_one()) {
+            for (int i = 0; i < NCH * KB; ++i) {
+                const int s = i % Cfg::STAGES;
+                mbar_wait(&empty[s], ((i / Cfg::STAGES) & 1) ^ 1);
+                mbar_expect_tx(&full[s], FA_SLOT);
+                tma_load_2d(&wmap, &full[s], ring + s * FA_SLOT, (i % KB) * 32, (i / KB) * 96);
+            }
+        }
+        return;
+    }
+
+    // ===================== gather: row r = window r/36, token r%36; rows >= 108 and missing windows are zero =====================
+    for (int i = tid; i < FA_ROWS * (C / 8); i += GEMM_CONSUMER_THREADS) {
+        const int r = i / (C / 8), u = i % (C / 8);
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (r < FA_WIN * WTOK) {
+            const int tok = stok[r];
+            if (tok >= 0) v = __ldg(reinterpret_cast<const uint4*>(x + (size_t)tok * C) + u);
+        }
+        *reinterpret_cast<uint4*>(sx + (u >> 2) * (FA_ROWS * 64) + stage_off<32>(r, u & 3)) = v;
+    }
+    fence_async_smem();   // generic-proxy writes of the A tile -> visible to wgmma
+    consumer_bar_sync();
+
+    // ===================== q | k | v = x Wqkv^T + b, 96 columns at a time =====================
+    const int wg = tid >> 7, t = tid & 127;
+    const int row0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+    const int cq = 2 * (t & 3);
+    const uint32_t a_base = smem_u32(sx) + wg * 64 * 64;
+#pragma unroll 1
+    for (int c = 0; c < NCH; ++c) {
+        float acc[48];
+#pragma unroll
+        for (int j = 0; j < 48; ++j) acc[j] = 0.f;
+#pragma unroll 1
+        for (int kb = 0; kb < KB; ++kb) {
+            const int it = c * KB + kb, s = it % Cfg::STAGES;
+            mbar_wait(&full[s], (it / Cfg::STAGES) & 1);
+            const uint32_t a = a_base + kb * (FA_ROWS * 64), bb = smem_u32(ring + s * FA_SLOT);
+            wgmma_fence();
+            wgmma_f16<96>(acc, make_kmajor_desc<64>(a), make_kmajor_desc<64>(bb), 1u);
+            wgmma_f16<96>(acc, make_kmajor_desc<64>(a + 32), make_kmajor_desc<64>(bb + 32), 1u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            if (t == 0) mbar_arrive(&empty[s]);
+        }
+        wgmma_fence_operands(acc);
+#pragma unroll
+        for (int j = 0; j < 12; ++j) {
+            const int n = 96 * c + 8 * j + cq;           // q | k | v column (reference row order of Wqkv)
+            const int m = n / C, col = n - m * C;
+            const float2 bq = __ldg(reinterpret_cast<const float2*>(bqkv + n));
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int r = row0 + 8 * i;
+                if (r < FA_WIN * WTOK) {
+                    const int w = r / WTOK, tk = r - w * WTOK;
+                    *reinterpret_cast<__half2*>(sqkv + ((size_t)(w * 3 + m) * WTOK + tk) * LD + col) =
+                        __floats2half2_rn(acc[4 * j + 2 * i] + bq.x, acc[4 * j + 2 * i + 1] + bq.y);
+                }
+            }
+        }
+    }
+    consumer_bar_sync();
+
+    // ===================== attention: (window, head) pairs on the 8 consumer warps =====================
+    const int lane = tid & 31, g = lane >> 2, t4 = lane & 3;
+    const float scale = ((D == 16) ? 0.25f : 0.17677669529663687f) * 1.4426950408889634f;  // (C//heads)**-0.5 (:187) * log2(e)
+#pragma unroll 1
+    for (int pr = warp; pr < FA_WIN * HEADS; pr += GEMM_CONSUMER_THREADS / 32) {
+        const int w = pr / HEADS, head = pr - w * HEADS, gw = blockIdx.x * FA_WIN + w;
+        if (gw >= nwin) continue;
+        const int r = gw % (nww * nwy), wy = r / nww, wx = r % nww;
+        __half* sq = sqkv + (size_t)w * 3 * WTOK * LD;
+        __half* sk = sq + WTOK * LD;
+        __half* sv = sk + WTOK * LD;
+        AttnCtx<D> cx;
+        cx.sq = sq; cx.sreg = sreg + w * WPAD; cx.bf = bias_frag + (size_t)head * (3 * 6 * 32) + lane;
+        cx.hc = head * D; cx.g = g; cx.t4 = t4; cx.scale = scale;
+        cx.boundary = shift > 0 && (wy == nwy - 1 || wx == nww - 1);   // only these windows mix mask regions
+#pragma unroll
+        for (int nt = 0; nt < NKT; ++nt) cx.kbase[nt] = sk + min(nt * 8 + g, WTOK - 1) * LD + cx.hc + 2 * t4;
+        cx.vbase[0] = sv + (lane & 15) * LD + cx.hc;
+        cx.vbase[1] = sv + (16 + (lane & 15)) * LD + cx.hc;
+        cx.vbase[2] = sv + min(32 + (lane & 7), WTOK - 1) * LD + cx.hc;
+        attn_mtile<D, false>(cx, 0);
+        attn_mtile<D, false>(cx, 1);
+        attn_mtile<D, true>(cx, 2);
+    }
+    consumer_bar_sync();
+    for (int i = tid; i < FA_WIN * WTOK * (C / 8); i += GEMM_CONSUMER_THREADS) {
+        const int r = i / (C / 8), u = i % (C / 8);
+        const int tok = stok[r];
+        if (tok < 0) continue;
+        const int w = r / WTOK, tk = r - w * WTOK;
+        *reinterpret_cast<uint4*>(out + (size_t)tok * C + u * 8) =
+            *reinterpret_cast<const uint4*>(sqkv + ((size_t)w * 3 * WTOK + tk) * LD + u * 8);
+    }
+}
+
+int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const float* bqkv, const float* bias_frag_f, __half* att,
+                    int B, int H, int W, int C, int shift) {
+    NB_CHECK(x && wqkv && bqkv && bias_frag_f && att, "null pointer");
+    NB_CHECK(H % WS == 0 && W % WS == 0, "feature map must be a multiple of the 6x6 window");
+    NB_CHECK(C == 96 || C == 192, "fused window attention supports C=96 (d=16) and C=192 (d=32)");
+    if (WS >= H) shift = 0;  // torchvision :151-155
+    const long long nwin = (long long)B * (H / WS) * (W / WS);
+    NB_CHECK(nwin > 0 && nwin < (1LL << 31), "window count out of range");
+    CUtensorMap wmap;
+    const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(3 * C)};
+    const cuuint64_t strides[1] = {(cuuint64_t)C * 2};
+    const cuuint32_t box[2] = {32, 96};
+    if (encode(&wmap, wqkv, 2, dims, strides, box, 64)) return 1;
+    const double T = (double)B * H * W;
+    ProfScope ps(st, PC_FUSED_ATTN, T * 3.0 * C * C * 2 + T * C * 36 * 4, T * C * 2, T * C * 2);   // qkv GEMM + QK^T/PV; x in, att out
+    const unsigned grid = (unsigned)((nwin + FA_WIN - 1) / FA_WIN);
+    const float4* bf = reinterpret_cast<const float4*>(bias_frag_f);
+    if (C == 96) {
+        if (ensure_dyn_smem((const void*)swin_attn_fused_kernel<96>, FaCfg<96>::SMEM)) return 1;
+        swin_attn_fused_kernel<96><<<grid, FA_THREADS, FaCfg<96>::SMEM, st>>>(wmap, x, bqkv, bf, att, H, W, shift, (int)nwin);
+    } else {
+        if (ensure_dyn_smem((const void*)swin_attn_fused_kernel<192>, FaCfg<192>::SMEM)) return 1;
+        swin_attn_fused_kernel<192><<<grid, FA_THREADS, FaCfg<192>::SMEM, st>>>(wmap, x, bqkv, bf, att, H, W, shift, (int)nwin);
     }
     NB_LAUNCHED();
     return 0;

@@ -1,4 +1,4 @@
-// Tensor-map (TMA descriptor) construction shared by the tcgen05 kernels (gemm.cu).
+// Tensor-map (TMA descriptor) construction shared by the TMA kernels (gemm.cu).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>

@@ -28,6 +28,10 @@ __device__ __forceinline__ float linear_to_srgb(float x) {
     return (x <= 0.0031308f) ? x * 12.92f : 1.055f * powf(x, 1.0f / 2.4f) - 0.055f;
 }
 
+// a*x + b*y with both products and the sum rounded on their own.  Both backward-warp kernels blend through this, so they
+// agree bit for bit whichever product the compiler would otherwise fuse into an FMA.
+__device__ __forceinline__ float mix2_rn(float a, float x, float b, float y) { return __fadd_rn(__fmul_rn(a, x), __fmul_rn(b, y)); }
+
 // iw3/anaglyph.py:51-92 for one pixel
 __device__ __forceinline__ void dubois_px(const float l[3], const float r[3], bool clip_before, float out[3]) {
     const float lm[3][3] = {{0.437f, 0.449f, 0.164f}, {-0.062f, -0.062f, -0.024f}, {-0.048f, -0.050f, -0.017f}};
@@ -97,8 +101,10 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
             if (same) {
                 float is = __fsub_rn(__fmul_rn(dep[(size_t)y * p.w + x], p.shift), p.shift_conv);
                 float lx = linspace_m1_1(x, p.w, p.step_x);
-                gl = lx + (-is) * p.delta_scale;
-                gr = lx + is * p.delta_scale;
+                // each product and sum rounded on its own, as in the row-staged kernel's grid table (no FMA contraction)
+                const float d = __fmul_rn(is, p.delta_scale);
+                gl = __fsub_rn(lx, d);
+                gr = __fadd_rn(lx, d);
             } else {
                 float srcx = __fmul_rn(p.sx, (float)x);
                 int j0 = min((int)srcx, p.w - 1);
@@ -109,11 +115,12 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
                 float is10 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + j0), p.shift), p.shift_conv);
                 float is11 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + j1), p.shift), p.shift_conv);
                 float l0 = linspace_m1_1(j0, p.w, p.step_x), l1 = linspace_m1_1(j1, p.w, p.step_x);
-                float ds = p.delta_scale;
-                gl = ly0 * (lx0 * (l0 - is00 * ds) + lx1 * (l1 - is01 * ds)) +
-                     ly1 * (lx0 * (l0 - is10 * ds) + lx1 * (l1 - is11 * ds));
-                gr = ly0 * (lx0 * (l0 + is00 * ds) + lx1 * (l1 + is01 * ds)) +
-                     ly1 * (lx0 * (l0 + is10 * ds) + lx1 * (l1 + is11 * ds));
+                const float ds = p.delta_scale;
+                const float d00 = __fmul_rn(is00, ds), d01 = __fmul_rn(is01, ds), d10 = __fmul_rn(is10, ds), d11 = __fmul_rn(is11, ds);
+                gl = mix2_rn(ly0, mix2_rn(lx0, __fsub_rn(l0, d00), lx1, __fsub_rn(l1, d01)),
+                             ly1, mix2_rn(lx0, __fsub_rn(l0, d10), lx1, __fsub_rn(l1, d11)));
+                gr = mix2_rn(ly0, mix2_rn(lx0, __fadd_rn(l0, d00), lx1, __fadd_rn(l1, d01)),
+                             ly1, mix2_rn(lx0, __fadd_rn(l0, d10), lx1, __fadd_rn(l1, d11)));
             }
             const float wm1 = (float)(p.W - 1);
 #pragma unroll
@@ -136,7 +143,7 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
                 for (int k = 0; k < 3; ++k) {
                     float va = __ldg(crow + k * plane + xa);
                     float vb = __ldg(crow + k * plane + xb);
-                    o[v][k] = clamp01(va * wa + vb * wb);
+                    o[v][k] = clamp01(mix2_rn(va, wa, vb, wb));
                 }
             }
         }
@@ -255,8 +262,8 @@ __global__ void __launch_bounds__(256) backward_warp_row_kernel(BwParams p, int 
             const float lx1 = srcx - (float)j0, lx0 = 1.f - lx1;
             const float4 t0 = *reinterpret_cast<const float4*>(gt + j0);
             const float4 t1 = *reinterpret_cast<const float4*>(gt + j0 + 1);
-            const float gl = ly0 * (lx0 * t0.x + lx1 * t1.x) + ly1 * (lx0 * t0.z + lx1 * t1.z);
-            const float gr = ly0 * (lx0 * t0.y + lx1 * t1.y) + ly1 * (lx0 * t0.w + lx1 * t1.w);
+            const float gl = mix2_rn(ly0, mix2_rn(lx0, t0.x, lx1, t1.x), ly1, mix2_rn(lx0, t0.z, lx1, t1.z));
+            const float gr = mix2_rn(ly0, mix2_rn(lx0, t0.y, lx1, t1.y), ly1, mix2_rn(lx0, t0.w, lx1, t1.w));
 #pragma unroll
             for (int eye = 0; eye < 2; ++eye) {
                 float* o = eye == 0 ? outl[v] : outr[v];
@@ -273,7 +280,7 @@ __global__ void __launch_bounds__(256) backward_warp_row_kernel(BwParams p, int 
                 const float wb = ix - fx, wa = (fx + 1.f) - ix;
                 const float* sp = srow + (int)fx;
 #pragma unroll
-                for (int k = 0; k < 3; ++k) o[k] = __saturatef(sp[k * S] * wa + sp[k * S + 1] * wb);
+                for (int k = 0; k < 3; ++k) o[k] = __saturatef(mix2_rn(sp[k * S], wa, sp[k * S + 1], wb));
             }
         }
         if (COMPOSE == NB200_COMPOSE_ANAGLYPH_DUBOIS) {

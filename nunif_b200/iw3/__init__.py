@@ -1,9 +1,9 @@
-"""B200-native mirror of the iw3 hot-path callables (reference: iw3/*.py).
+"""H100-native mirror of the iw3 hot-path callables (reference: iw3/*.py).
 
 Same names, argument meaning and error behaviour as the reference functions so
 that ``iw3.utils.apply_divergence`` / ``postprocess_image`` can import these in
 place of the originals (INTEGRATION.md).  Every function requires CUDA tensors
-and dispatches to hand-written sm_100a kernels through the C ABI; there is no
+and dispatches to hand-written sm_90a kernels through the C ABI; there is no
 CPU path.
 """
 from .backward_warp import apply_divergence_grid_sample  # noqa: F401

@@ -7,7 +7,7 @@ from ._common import VIEWS, COMPOSE_NONE, prep
 def apply_divergence_grid_sample(c, depth, divergence, convergence, synthetic_view="both", compose=COMPOSE_NONE):
     """c: B,3,H,W float; depth: B,1,h,w float (any resolution) -> (left_eye, right_eye).
 
-    One fused sm_100a kernel (csrc/warp_backward.cu) replaces make_grid +
+    One fused sm_90a kernel (csrc/warp_backward.cu) replaces make_grid +
     F.interpolate(grid) + 2x F.grid_sample + clamp.  ``compose`` (extension) selects a
     fused SBS (returns B,3,H,2W) or dubois-anaglyph (B,3,H,W) epilogue instead.
     """

@@ -5,7 +5,7 @@
 ``flush_minmax_normalize`` (:176-194) - e.g. ``process_image`` (iw3/utils.py:505-545) calls
 ``get_ema_buffer_size() -> infer() -> minmax_normalize_chw()``.  Differences that are deliberate and loud:
 
-* the network is compiled ahead of time for sm_100a, so ``compile`` / ``compile_context`` have nothing to do;
+* the network is compiled ahead of time for sm_90a, so ``compile`` / ``compile_context`` have nothing to do;
 * one process owns one GPU (DESIGN.md section 6): a list of several GPUs raises instead of building the reference's
   ``DeviceSwitchInference`` thread pool;
 * checkpoints are read from disk only (``force_update`` would need the network and raises).
@@ -36,10 +36,10 @@ def _device_of(gpu):
         device = torch.device(gpu)
     else:
         if int(gpu) < 0:
-            raise RuntimeError("nunif_b200 depth models need a CUDA (sm_100) device; there is no CPU path")
+            raise RuntimeError("nunif_b200 depth models need a CUDA (sm_90) device; there is no CPU path")
         device = torch.device("cuda", int(gpu))
     if device.type != "cuda":
-        raise RuntimeError("nunif_b200 depth models need a CUDA (sm_100) device; there is no CPU path")
+        raise RuntimeError("nunif_b200 depth models need a CUDA (sm_90) device; there is no CPU path")
     return device
 
 

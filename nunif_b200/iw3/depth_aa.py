@@ -1,7 +1,7 @@
 """Mirror of `iw3.depth_aa` (iw3/models/depth_aa.py:30-87): the learned anti-aliasing filter batch_infer applies to the
 Depth-Anything output when ``depth_aa`` is set (iw3/depth_anything_model.py:153-154, :190-194).
 
-The Linears / 1x1 / 3x3 convolutions run on the tcgen05 GEMM, everything else in csrc/depth_aa.cu (nb200_depth_aa)."""
+The Linears / 1x1 / 3x3 convolutions run on the wgmma GEMM, everything else in csrc/depth_aa.cu (nb200_depth_aa)."""
 import ctypes
 import torch
 from .. import _lib
@@ -16,7 +16,7 @@ class DepthAA:
     def __init__(self, state_dict, device="cuda:0"):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_100) device; there is no CPU path")
+            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
         items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in state_dict.items()]
         n = len(items)
         names = (ctypes.c_char_p * n)(*[k.encode() for k, _ in items])

@@ -1,9 +1,9 @@
 """Mirror of iw3/depth_anything_model.py (DepthAnythingModel / batch_infer, lines 113-253) for the
-Depth-Anything-V2 ViT-S network on the B200 engine.
+Depth-Anything-V2 ViT-S network on the H100 engine.
 
 The reference obtains the network from torch.hub ("nagadomi/Depth-Anything_iw3:main", DepthAnything(encoder="v2_vits"),
 depth_anything_model.py:223-230); here the same checkpoint (upstream key names ``pretrained.*`` / ``depth_head.*``) is
-packed into the native container (csrc/depth_model.inl) and run as tcgen05 GEMMs + the kernels in
+packed into the native container (csrc/depth_model.inl) and run as wgmma GEMMs + the kernels in
 csrc/depth_kernels.cu.  ``infer`` keeps the reference's signature and output convention: depth B,1,h,w (or 1,h,w)
 float32 on ``x.device``, larger = nearer.
 """
@@ -29,7 +29,7 @@ class DepthAnythingNet:
         self.encoder = encoder
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_100) device; there is no CPU path")
+            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
         items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in state_dict.items()]
         n = len(items)
         names = (ctypes.c_char_p * n)(*[k.encode() for k, _ in items])
@@ -105,7 +105,7 @@ class DepthAnythingModel(BaseDepthModel):
 
     def __init__(self, model_type="Any_V2_S"):
         if model_type not in ENCODER_OF:
-            raise ValueError(f"the B200 engine implements {list(ENCODER_OF)} (Depth-Anything-V2 relative-depth models)")
+            raise ValueError(f"the H100 engine implements {list(ENCODER_OF)} (Depth-Anything-V2 relative-depth models)")
         super().__init__(model_type)
 
     @classmethod

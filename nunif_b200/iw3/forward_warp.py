@@ -9,14 +9,14 @@ def apply_divergence_forward_warp(c, depth, divergence, convergence, method=None
                                   width_base=True, compose=COMPOSE_NONE):
     """Depth-ordered bilinear forward warp (+ hole fill when method == "forward_fill").
 
-    Row-parallel sm_100a kernel (csrc/warp_forward.cu); semantics follow
+    Row-parallel sm_90a kernel (csrc/warp_forward.cu); semantics follow
     depth_order_bilinear_forward_warp (forward_warp.py:140-243) including the
     100-iteration caps.  ``inconsistent_shift=True`` (a debugging variant of the
     reference, forward_warp.py:34-37) is not on the hot path and is rejected.
     """
     assert synthetic_view in {"both", "right", "left"}      # forward_warp.py:145
     if inconsistent_shift:
-        raise NotImplementedError("inconsistent_shift=True is not supported by the B200 forward warp")
+        raise NotImplementedError("inconsistent_shift=True is not supported by the H100 forward warp")
     c = prep(c, "c")
     depth = prep(depth, "depth")
     B, _, H, W = c.shape

@@ -1,7 +1,7 @@
 """Mirror of iw3's learned stereo warp: the `sbs.row_flow_v3` model (iw3/models/row_flow_v3.py) in delta_output mode and
 its driver apply_divergence_nn_LR / apply_divergence_nn_delta (iw3/backward_warp.py:124-232).
 
-The delta network runs as tcgen05 GEMMs + the kernels in csrc/rowflow_kernels.cu; the warp is the fused grid-sample kernel
+The delta network runs as wgmma GEMMs + the kernels in csrc/rowflow_kernels.cu; the warp is the fused grid-sample kernel
 (csrc/warp_backward.cu, nb200_backward_warp_delta).  steps > 1 (iterative re-warping of the depth, :205-226) and
 preserve_screen_border (:33-47) run the same kernels once per step.
 """
@@ -36,7 +36,7 @@ class MLBW:
     def __init__(self, state_dict, device="cuda:0"):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_100) device; there is no CPU path")
+            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
         self._h = _create(KIND_MLBW, state_dict, self.device)
         self.num_layers = int(_lib.lib().nb200_mlbw_num_layers(self._h))
 
@@ -70,7 +70,7 @@ class RowFlowV3:
     def __init__(self, state_dict, device="cuda:0"):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_100) device; there is no CPU path")
+            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
         self._h = _create(KIND_ROW_FLOW_V3, state_dict, self.device)
 
     def __del__(self):
@@ -193,7 +193,7 @@ def apply_divergence_nn_LR(model, c, depth, divergence, convergence, steps=None,
     """iw3/backward_warp.py:124-160 for the non-symmetric delta models (sbs.row_flow_v3, sbs.mlbw)."""
     assert synthetic_view in {"both", "right", "left"}
     if getattr(model, "symmetric", False):
-        raise NotImplementedError("symmetric side models (row_flow_v2) are not implemented by the B200 engine")
+        raise NotImplementedError("symmetric side models (row_flow_v2) are not implemented by the H100 engine")
     kw = dict(steps=steps, preserve_screen_border=preserve_screen_border, enable_amp=enable_amp)
     if synthetic_view == "both":
         return (apply_divergence_nn(model, c, depth, divergence, convergence, shift=-1, **kw),

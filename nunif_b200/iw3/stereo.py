@@ -38,4 +38,4 @@ def stereo_sbs(c, depth, divergence=2.0, convergence=0.5, method="forward_fill",
             from .anaglyph import apply_anaglyph_redcyan
             return apply_anaglyph_redcyan(l, r, anaglyph)
         return torch.cat([l, r], dim=3)
-    raise ValueError(f"method {method} is not on the B200 hot path")
+    raise ValueError(f"method {method} is not on the H100 hot path")

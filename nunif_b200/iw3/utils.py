@@ -28,7 +28,7 @@ def apply_divergence(depth, im, args, side_model, reset_pts=None):
         depth, im = depth.unsqueeze(0), im.unsqueeze(0)
     state = _arg(args, "state", None) or {}
     if state.get("convergence_model") is not None:
-        raise NotImplementedError("auto-convergence (args.state['convergence_model']) is not implemented by the B200 engine")
+        raise NotImplementedError("auto-convergence (args.state['convergence_model']) is not implemented by the H100 engine")
     if not _arg(args, "disable_amp", False) is False:
         raise NotImplementedError("--disable-amp (fp32 side model) is not implemented: the engine runs the CUDA autocast numerics")
     convergence = args.convergence
@@ -43,12 +43,12 @@ def apply_divergence(depth, im, args, side_model, reset_pts=None):
         eyes = apply_divergence_forward_warp(im, depth, args.divergence, convergence=convergence, method=method,
                                              synthetic_view=args.synthetic_view, width_base=False)
     elif method in {"forward_inpaint", "mlbw_l2_inpaint"}:
-        raise NotImplementedError(f"method {method} (video inpainting side model) is outside the B200 hot path")
+        raise NotImplementedError(f"method {method} (video inpainting side model) is outside the H100 hot path")
     else:
         # the learned warps (row_flow*, mlbw*): apply_divergence_nn_LR with args.side_model (:363-385)
         stereo_width = _arg(args, "stereo_width", None)
         if stereo_width is not None and depth.shape[3] != min(im.shape[3], stereo_width):
-            raise NotImplementedError("--stereo-width depth resampling is not implemented by the B200 engine")
+            raise NotImplementedError("--stereo-width depth resampling is not implemented by the H100 engine")
         if side_model is None:
             raise ValueError(f"method {method} needs side_model")
         eyes = apply_divergence_nn_LR(side_model, im, depth, args.divergence, convergence, _arg(args, "warp_steps", None),

@@ -1,10 +1,10 @@
 """Mirror of iw3/zoedepth_model.py (ZoeDepthModel / batch_infer, lines 89-233) for the ZoeD_N metric depth network on the
-B200 engine.
+H100 engine.
 
 The reference obtains the network from torch.hub ("nagadomi/ZoeDepth_iw3:main", ZoeD_N, config_mode="infer",
 zoedepth_model.py:151-157) and removes its internal resize/normalise (`model.core.prep = lambda x: x`, :169); here the
 same checkpoint (ZoeD_M12_N.pt, upstream key names `core.core.pretrained.*`, `core.core.scratch.*`, `conv2`,
-`seed_bin_regressor`, ...) is packed into the native container (csrc/zoe_model.inl) and run as tcgen05 GEMMs + the
+`seed_bin_regressor`, ...) is packed into the native container (csrc/zoe_model.inl) and run as wgmma GEMMs + the
 kernels in csrc/depth_kernels.cu / zoe_kernels.cu.  ``infer`` keeps the reference's signature and output convention:
 B,1,h,w (or 1,h,w) float32 on ``x.device`` = the NEGATED metric depth of the unpadded frame (larger = nearer).
 
@@ -40,7 +40,7 @@ class ZoeDepthNet:
     def __init__(self, state_dict, device="cuda:0"):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_100) device; there is no CPU path")
+            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
         items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in _strip_checkpoint(state_dict).items()
                  if torch.is_tensor(v)]
         n = len(items)
@@ -111,7 +111,7 @@ class ZoeDepthModel(BaseDepthModel):
 
     def __init__(self, model_type="ZoeD_N"):
         if model_type not in MODEL_FILES:
-            raise ValueError(f"the B200 engine implements {list(MODEL_FILES)}; ZoeD_K / ZoeD_NK / ZoeD_Any_* are not built")
+            raise ValueError(f"the H100 engine implements {list(MODEL_FILES)}; ZoeD_K / ZoeD_NK / ZoeD_Any_* are not built")
         super().__init__(model_type)
 
     @classmethod

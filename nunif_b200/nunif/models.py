@@ -1,5 +1,5 @@
 """Model containers with the reference's I2IBaseModel contract
-(nunif/models/model.py:65-86) backed by the sm_100a engine.
+(nunif/models/model.py:65-86) backed by the sm_90a engine.
 
 A container owns a packed fp16 weight blob on ONE device, created from a
 state_dict with the reference's key names (strict, like load_state_dict).
@@ -31,7 +31,7 @@ class B200I2IModel:
         self.name = name
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_100) device; there is no CPU path")
+            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
         self._downscale = _downscale
         self._parent = _parent  # keeps the shared handle alive (to_2x(shared=True))
         self.training = False

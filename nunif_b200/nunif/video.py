@@ -39,7 +39,7 @@ class FrameBatchPipeline:
         self.batch_size = int(batch_size)
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("FrameBatchPipeline runs on a CUDA (sm_100) device")
+            raise RuntimeError("FrameBatchPipeline runs on a CUDA (sm_90) device")
         self.dtype = torch.uint16 if use_16bit else torch.uint8
         self.bits = 16 if use_16bit else 8
         self.slots = [_Slot() for _ in range(depth)]

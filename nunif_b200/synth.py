@@ -6,7 +6,7 @@ under the *reference's* key names and shapes (waifu2x/models/cunet.py:10-163,
 waifu2x/models/swin_unet.py:119-199, torchvision swin_transformer.py:234-312)
 so the same dict loads into the real reference modules with
 ``load_state_dict(strict=True)`` (done in oracle/gen_golden.py) and into the
-B200 engine's weight packer.
+H100 engine's weight packer.
 
 Gains are chosen so activations stay O(1) through the stack and the final
 output spans [0, 1] (the clamps and the seam blend are then exercised).

@@ -1,4 +1,4 @@
-"""`waifu2x` hub entry for the B200 engine: the same public surface as the reference's
+"""`waifu2x` hub entry for the H100 engine: the same public surface as the reference's
 ``Waifu2xImageModel`` / ``waifu2x()`` factory (waifu2x/hub.py:31-175), built as a thin adapter.
 
 Design (not a transcription): the reference class mixes mode bookkeeping, device plumbing and three input
@@ -8,7 +8,7 @@ front-ends in one class body.  Here
 * ``_decode`` / ``_encode``   are the only places that know about PIL (hub.py:105-120, nunif/utils/pil_io.py:218-253),
 * ``Waifu2xImageModel``   is a small facade: every ``infer*`` funnels into ``_run`` -> ``Waifu2x.convert``.
 
-Engine restrictions are loud, never silent: models live on one sm_100 device (``cpu()`` raises), the forward is the
+Engine restrictions are loud, never silent: models live on one sm_90 device (``cpu()`` raises), the forward is the
 reference's CUDA autocast numerics (``amp=False`` / ``float()`` raise), nothing is downloaded.
 """
 import os

@@ -30,14 +30,14 @@ class Waifu2x():
             gpu = 0
         self.device = torch.device(f"cuda:{gpu}") if isinstance(gpu, int) else torch.device(gpu)
         if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200.waifu2x runs on CUDA (sm_100) only")
+            raise RuntimeError("nunif_b200.waifu2x runs on CUDA (sm_90) only")
         self.gpus = gpus
         self.model_dir = model_dir
         self.is_half = False
 
     def compile(self):
         """waifu2x/utils.py:49-58 wraps the modules in torch.compile; this engine's kernels are compiled ahead of time
-        (nvcc, sm_100a), so there is nothing left to do - same results either way, as in the reference."""
+        (nvcc, sm_90a), so there is nothing left to do - same results either way, as in the reference."""
         return self
 
     def _loaded_models(self):

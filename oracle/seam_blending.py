@@ -118,7 +118,7 @@ def tiled_render(x, model_fn, scale, offset, blend_size, tile_size, batch_size):
 def tiled_render_closed_form(x, model_fn, scale, offset, blend_size, tile_size, batch_size):
     """Order-independent statement of the same blend: sum(w*z)/sum(w).
 
-    This is what the B200 engine computes (DESIGN.md); SURVEY.md section 7
+    This is what the H100 engine computes (DESIGN.md); SURVEY.md section 7
     hard-part 2 measured it within 4.2e-7 of the raster-order reference.
     """
     C, H, W = x.shape

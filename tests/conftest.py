@@ -8,7 +8,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (B200)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (H100)")
 
 
 def pytest_collection_modifyitems(config, items):

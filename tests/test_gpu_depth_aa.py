@@ -1,4 +1,4 @@
-"""GPU: iw3.depth_aa (csrc/depth_aa.cu + tcgen05 GEMMs) against the reference-generated golden (tests/golden/depth_aa.npz,
+"""GPU: iw3.depth_aa (csrc/depth_aa.cu + wgmma GEMMs) against the reference-generated golden (tests/golden/depth_aa.npz,
 oracle/gen_golden.py gen_depth_aa ran the REAL model) and against the oracle at other shapes.  The reference runs this filter in
 fp32 (outside autocast, iw3/depth_anything_model.py:153-154); the engine's GEMMs are fp16 with fp32 accumulation."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 implicit-GEMM against torch fp32 on fp16-rounded operands."""
+"""GPU: the wgmma implicit-GEMM against torch fp32 on fp16-rounded operands."""
 import pytest
 import torch
 import torch.nn.functional as F

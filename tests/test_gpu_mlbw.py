@@ -1,4 +1,4 @@
-"""GPU: sbs.mlbw (csrc/mlbw.cu + tcgen05 GEMMs) in delta_output mode and apply_divergence_nn_delta_weight against the
+"""GPU: sbs.mlbw (csrc/mlbw.cu + wgmma GEMMs) in delta_output mode and apply_divergence_nn_delta_weight against the
 reference-generated golden (tests/golden/mlbw.npz: the REAL model, fp32 on the CPU) and against the oracle for the 4-layer and
 `small` variants.  The engine runs the reference's CUDA numerics (fp16 autocast): bounds as for sbs.row_flow_v3."""
 import pytest
