@@ -75,10 +75,10 @@ struct AttnCtx {
 };
 
 // One 16-row query tile of one head: S = Q K^T, bias/mask, base-2 softmax numerators, O = P V, normalise, stage.
-// LAST: query rows 32..35 only (accumulator rows g+8 are padding and are not evaluated).
-template <int D, bool LAST>
+// LD: row stride (halves) of the q/k/v tiles.  LAST: query rows 32..35 only (accumulator rows g+8 are padding and are not
+// evaluated).
+template <int D, int LD, bool LAST>
 __device__ __forceinline__ void attn_mtile(const AttnCtx<D>& cx, int mt) {
-    constexpr int C = D * HEADS, LD = C + 8;
     constexpr uint32_t ONES = 0x3C003C00u;   // half2(1, 1)
     constexpr int HL = LAST ? 1 : 2;         // accumulator row halves in use
     const int g = cx.g, t4 = cx.t4, hc = cx.hc;
@@ -260,8 +260,8 @@ __global__ void __launch_bounds__(192, D == 16 ? 6 : 4) window_attention_mma_ker
     // 4 CTAs fit per SM; K / V fragments are re-read from shared memory per m-tile (cheap, conflict-free).
     // The last tile holds query rows 32..35 only: its upper half (rows 40..47) is skipped.
 #pragma unroll 1
-    for (int mt = 0; mt < 2; ++mt) attn_mtile<D, false>(cx, mt);
-    attn_mtile<D, true>(cx, 2);
+    for (int mt = 0; mt < 2; ++mt) attn_mtile<D, LD, false>(cx, mt);
+    attn_mtile<D, LD, true>(cx, 2);
     __syncthreads();
     for (int t = rg; t < WTOK; t += RG)
         *reinterpret_cast<uint4*>(out + (size_t)stok[t] * C + vv * 8) = *reinterpret_cast<const uint4*>(sq + t * LD + vv * 8);
@@ -344,40 +344,43 @@ int window_attention(cudaStream_t st, const __half* qkv, const float* bias_frag_
 // ---------------------------------------------------------------------------------------------
 // Fused block head: att = window_attention_core(x . Wqkv^T + bqkv), q/k/v never leave shared memory.
 // One CTA = 3 windows = 108 tokens (+20 zero rows) = the 128 rows of two wgmma warpgroups.
-//   warp 8    : TMA producer of the weight blocks [96 rows][32] (64B swizzle), 3C/96 column chunks x C/32 K-blocks
-//   warps 0-7 : gather the rolled window tokens into a swizzled [128][C] A tile; per 96-column chunk of q|k|v one
-//               wgmma accumulation (M = 64 per warpgroup), bias, fp16 into the per-window q/k/v tiles of the
-//               mma.sync attention core (attn_mtile, the same code as window_attention_mma_kernel); then the 18
-//               (window, head) pairs on the 8 warps, and the un-rolled rows back to HBM.
+// q|k|v is computed head-major in C/32 chunks of 96 columns: chunk c holds columns [32c, 32c+32) of q, of k and of v, i.e.
+// head c (d = 32) or heads 2c, 2c+1 (d = 16), so it is complete input of the attention core for those heads.
+//   warp 8    : TMA producer of the weight blocks: per (chunk c, K-block) the rows 32c, C + 32c and 2C + 32c of Wqkv as three
+//               [32][32] boxes (64B swizzle) stacked into one [96][32] operand, C/32 chunks x C/32 K-blocks
+//   warps 0-7 : gather the rolled window tokens into a swizzled [128][C] A tile (cp.async); per chunk one wgmma
+//               accumulation (M = 64 per warpgroup), bias, fp16 into the chunk's per-window q/k/v tiles; then the chunk's
+//               (window, head, m-tile) items of the mma.sync attention core (attn_mtile, the same code as
+//               window_attention_mma_kernel) on the 8 warps, each warp writing its un-rolled output rows back to HBM.
+// Only one chunk of q/k/v is resident (25 KB instead of 127 KB for all heads at C = 192), so two CTAs share an SM at both C
+// and one CTA's GEMM overlaps the other's attention.
 // ---------------------------------------------------------------------------------------------
-constexpr int FA_ROWS = 128, FA_WIN = 3, FA_THREADS = GEMM_CONSUMER_THREADS + 32, FA_SLOT = 96 * 64;
+constexpr int FA_ROWS = 128, FA_WIN = 3, FA_THREADS = GEMM_CONSUMER_THREADS + 32, FA_SLOT = 96 * 64, FA_STAGES = 4;
+constexpr int FA_LD = 32 + 8;   // chunk tile row: 80 B = 20 words, so fragment loads and ldmatrix rows are conflict-free
+constexpr int FA_CHUNK_BYTES = FA_WIN * 3 * WTOK * FA_LD * 2;
 
 template <int C>
 struct FaCfg {
-    // C = 96: 2 weight stages keep the CTA at ~104 KB so that two CTAs (and their GEMM / attention phases) share an SM
-    static constexpr int STAGES = C == 96 ? 2 : 4, MIN_CTAS = C == 96 ? 2 : 1;
-    static constexpr int LD = C + 8;
     static constexpr int X_BYTES = FA_ROWS * C * 2;
-    static constexpr int QKV_BYTES = FA_WIN * 3 * WTOK * LD * 2;
-    static constexpr int SMEM = X_BYTES + STAGES * FA_SLOT + QKV_BYTES + FA_WIN * (WTOK + WPAD) * 4 + 2 * STAGES * 8 + 1024;
+    static constexpr int SMEM = X_BYTES + FA_STAGES * FA_SLOT + FA_CHUNK_BYTES + FA_WIN * (WTOK + WPAD) * 4 + 2 * FA_STAGES * 8 + 1024;
 };
 
 template <int C>
-__global__ void __launch_bounds__(FA_THREADS, FaCfg<C>::MIN_CTAS) swin_attn_fused_kernel(const __grid_constant__ CUtensorMap wmap,
+__global__ void __launch_bounds__(FA_THREADS, 2) swin_attn_fused_kernel(const __grid_constant__ CUtensorMap wmap,
                                                                         const __half* __restrict__ x, const float* __restrict__ bqkv,
                                                                         const float4* __restrict__ bias_frag, __half* __restrict__ out,
                                                                         int H, int W, int shift, int nwin) {
     using Cfg = FaCfg<C>;
-    constexpr int D = C / HEADS, LD = Cfg::LD, KB = C / 32, NCH = 3 * C / 96;
+    constexpr int D = C / HEADS, KB = C / 32, NCH = C / 32, HPC = 32 / D;   // HPC: heads per chunk
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     uint8_t* sx = smem;
     uint8_t* ring = smem + Cfg::X_BYTES;
-    __half* sqkv = reinterpret_cast<__half*>(ring + Cfg::STAGES * FA_SLOT);   // [window][q|k|v][WTOK][LD]
-    int* stok = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(sqkv) + Cfg::QKV_BYTES);   // [window][WTOK], -1 = none
+    __half* sqkv = reinterpret_cast<__half*>(ring + FA_STAGES * FA_SLOT);   // [window][q|k|v][WTOK][FA_LD], one chunk
+    int* stok = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(sqkv) + FA_CHUNK_BYTES);   // [window][WTOK], -1 = none
     int* sreg = stok + FA_WIN * WTOK;                                                         // [window][WPAD]
     uint64_t* full = reinterpret_cast<uint64_t*>(sreg + FA_WIN * WPAD);
-    uint64_t* empty = full + Cfg::STAGES;
+    uint64_t* empty = full + FA_STAGES;
     const int tid = threadIdx.x, warp = tid >> 5;
     const int nww = W / WS, nwy = H / WS;
     if (tid < FA_WIN * WPAD) {
@@ -403,7 +406,7 @@ __global__ void __launch_bounds__(FA_THREADS, FaCfg<C>::MIN_CTAS) swin_attn_fuse
     }
     if (tid == GEMM_CONSUMER_THREADS) {
         tma_prefetch_desc(&wmap);
-        for (int s = 0; s < Cfg::STAGES; ++s) {
+        for (int s = 0; s < FA_STAGES; ++s) {
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], 2);   // one arrival per consumer warpgroup
         }
@@ -415,101 +418,108 @@ __global__ void __launch_bounds__(FA_THREADS, FaCfg<C>::MIN_CTAS) swin_attn_fuse
         // ===================== weight producer =====================
         if (elect_one()) {
             for (int i = 0; i < NCH * KB; ++i) {
-                const int s = i % Cfg::STAGES;
-                mbar_wait(&empty[s], ((i / Cfg::STAGES) & 1) ^ 1);
+                const int s = i % FA_STAGES, c = i / KB;
+                mbar_wait(&empty[s], ((i / FA_STAGES) & 1) ^ 1);
                 mbar_expect_tx(&full[s], FA_SLOT);
-                tma_load_2d(&wmap, &full[s], ring + s * FA_SLOT, (i % KB) * 32, (i / KB) * 96);
+                // 32-row boxes at 2 KB offsets: the 64B swizzle repeats every 512 B, so the stack is laid out as one 96-row box
+#pragma unroll
+                for (int m = 0; m < 3; ++m)
+                    tma_load_2d(&wmap, &full[s], ring + s * FA_SLOT + m * 32 * 64, (i % KB) * 32, m * C + 32 * c);
             }
         }
         return;
     }
 
     // ===================== gather: row r = window r/36, token r%36; rows >= 108 and missing windows are zero =====================
+    // 16-byte cp.async copies: all of a thread's loads are in flight at once
     for (int i = tid; i < FA_ROWS * (C / 8); i += GEMM_CONSUMER_THREADS) {
         const int r = i / (C / 8), u = i % (C / 8);
-        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-        if (r < FA_WIN * WTOK) {
-            const int tok = stok[r];
-            if (tok >= 0) v = __ldg(reinterpret_cast<const uint4*>(x + (size_t)tok * C) + u);
-        }
-        *reinterpret_cast<uint4*>(sx + (u >> 2) * (FA_ROWS * 64) + stage_off<32>(r, u & 3)) = v;
+        uint8_t* dst = sx + (u >> 2) * (FA_ROWS * 64) + stage_off<32>(r, u & 3);
+        const int tok = r < FA_WIN * WTOK ? stok[r] : -1;
+        if (tok >= 0) cp_async16(dst, x + (size_t)tok * C + u * 8);
+        else *reinterpret_cast<uint4*>(dst) = make_uint4(0u, 0u, 0u, 0u);
     }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
     fence_async_smem();   // generic-proxy writes of the A tile -> visible to wgmma
     consumer_bar_sync();
 
-    // ===================== q | k | v = x Wqkv^T + b, 96 columns at a time =====================
     const int wg = tid >> 7, t = tid & 127;
     const int row0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
     const int cq = 2 * (t & 3);
     const uint32_t a_base = smem_u32(sx) + wg * 64 * 64;
+    const int lane = tid & 31, g = lane >> 2, t4 = lane & 3;
+    const float scale = ((D == 16) ? 0.25f : 0.17677669529663687f) * 1.4426950408889634f;  // (C//heads)**-0.5 (:187) * log2(e)
 #pragma unroll 1
     for (int c = 0; c < NCH; ++c) {
+        // ===================== chunk c of q | k | v = x Wqkv^T + b =====================
         float acc[48];
 #pragma unroll
         for (int j = 0; j < 48; ++j) acc[j] = 0.f;
 #pragma unroll 1
         for (int kb = 0; kb < KB; ++kb) {
-            const int it = c * KB + kb, s = it % Cfg::STAGES;
-            mbar_wait(&full[s], (it / Cfg::STAGES) & 1);
+            const int it = c * KB + kb, s = it % FA_STAGES;
+            mbar_wait(&full[s], (it / FA_STAGES) & 1);
             const uint32_t a = a_base + kb * (FA_ROWS * 64), bb = smem_u32(ring + s * FA_SLOT);
             wgmma_fence();
             wgmma_f16<96>(acc, make_kmajor_desc<64>(a), make_kmajor_desc<64>(bb), 1u);
             wgmma_f16<96>(acc, make_kmajor_desc<64>(a + 32), make_kmajor_desc<64>(bb + 32), 1u);
             wgmma_commit();
-            wgmma_wait<0>();
-            if (t == 0) mbar_arrive(&empty[s]);
+            // keep one group in flight: the stage read by the previous group is released once that group retired
+            wgmma_wait<1>();
+            if (kb > 0 && t == 0) mbar_arrive(&empty[(it - 1) % FA_STAGES]);
         }
+        wgmma_wait<0>();
+        if (t == 0) mbar_arrive(&empty[(c * KB + KB - 1) % FA_STAGES]);
         wgmma_fence_operands(acc);
+        consumer_bar_sync();   // every warp is done with the previous chunk's q/k/v
 #pragma unroll
         for (int j = 0; j < 12; ++j) {
-            const int n = 96 * c + 8 * j + cq;           // q | k | v column (reference row order of Wqkv)
-            const int m = n / C, col = n - m * C;
-            const float2 bq = __ldg(reinterpret_cast<const float2*>(bqkv + n));
+            const int m = j >> 2, col = 8 * (j & 3) + cq;   // q|k|v, column within the chunk
+            const float2 bq = __ldg(reinterpret_cast<const float2*>(bqkv + m * C + 32 * c + col));
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 const int r = row0 + 8 * i;
                 if (r < FA_WIN * WTOK) {
                     const int w = r / WTOK, tk = r - w * WTOK;
-                    *reinterpret_cast<__half2*>(sqkv + ((size_t)(w * 3 + m) * WTOK + tk) * LD + col) =
+                    *reinterpret_cast<__half2*>(sqkv + ((w * 3 + m) * WTOK + tk) * FA_LD + col) =
                         __floats2half2_rn(acc[4 * j + 2 * i] + bq.x, acc[4 * j + 2 * i + 1] + bq.y);
                 }
             }
         }
-    }
-    consumer_bar_sync();
+        consumer_bar_sync();
 
-    // ===================== attention: (window, head) pairs on the 8 consumer warps =====================
-    const int lane = tid & 31, g = lane >> 2, t4 = lane & 3;
-    const float scale = ((D == 16) ? 0.25f : 0.17677669529663687f) * 1.4426950408889634f;  // (C//heads)**-0.5 (:187) * log2(e)
+        // ===================== attention: the chunk's (window, head, m-tile) items on the 8 consumer warps =====================
+        // m-tile-major order, so that the items left over for a last round are the cheap 4-row tiles
 #pragma unroll 1
-    for (int pr = warp; pr < FA_WIN * HEADS; pr += GEMM_CONSUMER_THREADS / 32) {
-        const int w = pr / HEADS, head = pr - w * HEADS, gw = blockIdx.x * FA_WIN + w;
-        if (gw >= nwin) continue;
-        const int r = gw % (nww * nwy), wy = r / nww, wx = r % nww;
-        __half* sq = sqkv + (size_t)w * 3 * WTOK * LD;
-        __half* sk = sq + WTOK * LD;
-        __half* sv = sk + WTOK * LD;
-        AttnCtx<D> cx;
-        cx.sq = sq; cx.sreg = sreg + w * WPAD; cx.bf = bias_frag + (size_t)head * (3 * 6 * 32) + lane;
-        cx.hc = head * D; cx.g = g; cx.t4 = t4; cx.scale = scale;
-        cx.boundary = shift > 0 && (wy == nwy - 1 || wx == nww - 1);   // only these windows mix mask regions
+        for (int item = warp; item < 3 * FA_WIN * HPC; item += GEMM_CONSUMER_THREADS / 32) {
+            const int mt = item / (FA_WIN * HPC), pr = item - mt * (FA_WIN * HPC), w = pr / HPC, hh = pr - w * HPC;
+            const int gw = blockIdx.x * FA_WIN + w;
+            if (gw >= nwin) continue;
+            const int r = gw % (nww * nwy), wy = r / nww, wx = r % nww, head = c * HPC + hh;
+            __half* sq = sqkv + w * 3 * WTOK * FA_LD;
+            __half* sk = sq + WTOK * FA_LD;
+            __half* sv = sk + WTOK * FA_LD;
+            AttnCtx<D> cx;
+            cx.sq = sq; cx.sreg = sreg + w * WPAD; cx.bf = bias_frag + (size_t)head * (3 * 6 * 32) + lane;
+            cx.hc = hh * D; cx.g = g; cx.t4 = t4; cx.scale = scale;
+            cx.boundary = shift > 0 && (wy == nwy - 1 || wx == nww - 1);   // only these windows mix mask regions
 #pragma unroll
-        for (int nt = 0; nt < NKT; ++nt) cx.kbase[nt] = sk + min(nt * 8 + g, WTOK - 1) * LD + cx.hc + 2 * t4;
-        cx.vbase[0] = sv + (lane & 15) * LD + cx.hc;
-        cx.vbase[1] = sv + (16 + (lane & 15)) * LD + cx.hc;
-        cx.vbase[2] = sv + min(32 + (lane & 7), WTOK - 1) * LD + cx.hc;
-        attn_mtile<D, false>(cx, 0);
-        attn_mtile<D, false>(cx, 1);
-        attn_mtile<D, true>(cx, 2);
-    }
-    consumer_bar_sync();
-    for (int i = tid; i < FA_WIN * WTOK * (C / 8); i += GEMM_CONSUMER_THREADS) {
-        const int r = i / (C / 8), u = i % (C / 8);
-        const int tok = stok[r];
-        if (tok < 0) continue;
-        const int w = r / WTOK, tk = r - w * WTOK;
-        *reinterpret_cast<uint4*>(out + (size_t)tok * C + u * 8) =
-            *reinterpret_cast<const uint4*>(sqkv + ((size_t)w * 3 * WTOK + tk) * LD + u * 8);
+            for (int nt = 0; nt < NKT; ++nt) cx.kbase[nt] = sk + min(nt * 8 + g, WTOK - 1) * FA_LD + cx.hc + 2 * t4;
+            cx.vbase[0] = sv + (lane & 15) * FA_LD + cx.hc;
+            cx.vbase[1] = sv + (16 + (lane & 15)) * FA_LD + cx.hc;
+            cx.vbase[2] = sv + min(32 + (lane & 7), WTOK - 1) * FA_LD + cx.hc;
+            if (mt < 2) attn_mtile<D, FA_LD, false>(cx, mt);
+            else attn_mtile<D, FA_LD, true>(cx, 2);
+            // the m-tile's output rows (staged over its own q rows by this warp) -> HBM, D columns = D/8 16-byte pieces per row
+            __syncwarp();
+            const int nrow = mt < 2 ? 16 : WTOK - 32;
+            for (int e = lane; e < nrow * (D / 8); e += 32) {
+                const int tk = 16 * mt + e / (D / 8), u = e % (D / 8);
+                *reinterpret_cast<uint4*>(out + (size_t)stok[w * WTOK + tk] * C + head * D + u * 8) =
+                    *reinterpret_cast<const uint4*>(sq + tk * FA_LD + cx.hc + u * 8);
+            }
+        }
     }
 }
 
@@ -524,7 +534,7 @@ int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const 
     CUtensorMap wmap;
     const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(3 * C)};
     const cuuint64_t strides[1] = {(cuuint64_t)C * 2};
-    const cuuint32_t box[2] = {32, 96};
+    const cuuint32_t box[2] = {32, 32};   // [32 rows][32]: one q, k or v block of a chunk
     if (encode(&wmap, wqkv, 2, dims, strides, box, 64)) return 1;
     const double T = (double)B * H * W;
     ProfScope ps(st, PC_FUSED_ATTN, T * 3.0 * C * C * 2 + T * C * 36 * 4, T * C * 2, T * C * 2);   // qkv GEMM + QK^T/PV; x in, att out
