@@ -91,7 +91,9 @@ enum {
     /* ZoeD_N metric depth: third-party net the reference loads through torch.hub "nagadomi/ZoeDepth_iw3" (iw3/zoedepth_model.py:151-157);
      * state_dict keys of ZoeD_M12_N.pt (`core.core.pretrained.*`, `core.core.scratch.*`, `conv2`, `seed_bin_regressor`, ...).
      * The widths are read off the tensor sizes (BEiT-L/16 for the released checkpoint). */
-    NB200_MODEL_ZOEDEPTH_N = 12
+    NB200_MODEL_ZOEDEPTH_N = 12,
+    NB200_MODEL_UPCONV_7 = 13,             /* waifu2x.upconv_7 (waifu2x/models/upconv_7.py:6-38): scale 2, offset 14 */
+    NB200_MODEL_VGG_7 = 14                 /* waifu2x.vgg_7    (waifu2x/models/vgg_7.py:6-36): scale 1, offset 7 */
 };
 
 /* Create a model from named fp32 host tensors using the reference's state_dict

@@ -1,11 +1,12 @@
 // Model containers: weight packing from the reference's state_dict keys and the
-// forward passes of SwinUNet (swin_unet.py:119-199) and CUNet/UpCUNet (cunet.py:10-203)
-// expressed as sequences of the sm_90a kernels.  Also the whole-image tiled render.
+// forward passes of SwinUNet (swin_unet.py:119-199), CUNet/UpCUNet (cunet.py:10-203) and UpConv7/VGG7
+// (upconv_7.py, vgg_7.py) expressed as sequences of the sm_90a kernels.  Also the whole-image tiled render.
 #include "common.cuh"
 #include "gemm.h"
 #include "gemm_wgmma.cuh"
 #include "swin_kernels.h"
 #include "cunet_kernels.h"
+#include "legacy_kernels.h"
 #include "depth_kernels.h"
 #include "rowflow_kernels.h"
 #include "depth_aa_kernels.h"
@@ -200,6 +201,7 @@ struct SwinW {
 };
 
 struct CUNetW;  // cunet_model.inl
+struct LegacyW; // legacy_model.inl
 struct DaW;     // depth_model.inl
 struct RfW;     // rowflow_model.inl
 struct AaW;     // depth_aa_model.inl
@@ -217,6 +219,7 @@ struct nb200_model {
     size_t blob_bytes = 0;
     SwinW sw;
     std::shared_ptr<CUNetW> cu;
+    std::shared_ptr<LegacyW> lg;
     std::shared_ptr<DaW> da;
     std::shared_ptr<RfW> rf;
     std::shared_ptr<AaW> aa;
@@ -465,6 +468,7 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
 }  // namespace nb200
 
 #include "cunet_model.inl"
+#include "legacy_model.inl"
 // debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth forward is copied to `g_tap_buf`
 static int g_tap_id = -1;
 static void* g_tap_buf = nullptr;
@@ -488,7 +492,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* names, const float* const* data,
                                   const int64_t* numel, int no_clip, nb200_model** out) {
     NB_CHECK(out && names && data && numel, "null pointer");
-    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_ZOEDEPTH_N, "unknown model kind");
+    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_VGG_7, "unknown model kind");
     int dev = 0;
     NB_CUDA(cudaGetDevice(&dev));
     if (nb200_check_device(dev)) return 1;
@@ -520,6 +524,8 @@ extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* na
         case NB200_MODEL_MLBW: m->ml = pack_mlbw(pk); m->scale = 1; m->offset = 32; m->blend = 4; break;               // mlbw.py:41
         case NB200_MODEL_DEPTH_AA: m->aa = pack_depth_aa(pk); m->scale = 1; break;                                     // depth_aa.py:34
         case NB200_MODEL_ROW_FLOW_V3: m->rf = pack_row_flow(pk); m->scale = 1; m->offset = 32; m->blend = 4; break;   // row_flow_v3.py:37
+        case NB200_MODEL_UPCONV_7: m->lg = pack_legacy(pk, true); m->scale = 2; m->offset = 14; m->blend = 0; break;  // upconv_7.py:11
+        case NB200_MODEL_VGG_7: m->lg = pack_legacy(pk, false); m->scale = 1; m->offset = 7; m->blend = 0; break;     // vgg_7.py:11
     }
     if (pk.err.empty())
         for (auto& kv : pk.src)
@@ -583,8 +589,9 @@ extern "C" int nb200_model_forward(nb200_model* m, const void* x, int n, int til
     int scale, offset, blend, S;
     if (model_out_geometry(m, tile_size, downscale, &scale, &offset, &blend, &S)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
-    NB_CHECK(m->kind <= NB200_MODEL_SWIN_UNET_4X, "not an image-to-image model");
+    NB_CHECK(m->kind <= NB200_MODEL_SWIN_UNET_4X || m->lg, "not an image-to-image model");
     auto eager = [&]() {
+        if (m->lg) return legacy_forward(m, st, (const __half*)x, n, tile_size, (__half*)z);
         if (m->kind >= NB200_MODEL_SWIN_UNET_1X) return swin_forward(m, st, (const __half*)x, n, tile_size, downscale, z);
         return cunet_forward(m, st, (const __half*)x, n, tile_size, (__half*)z);
     };

@@ -11,6 +11,7 @@ from .. import _lib
 KINDS = {
     "waifu2x.upcunet": 1, "waifu2x.cunet": 2,
     "waifu2x.swin_unet_1x": 3, "waifu2x.swin_unet_2x": 4, "waifu2x.swin_unet_4x": 5,
+    "waifu2x.upconv_7": 13, "waifu2x.vgg_7": 14,
 }
 
 
@@ -20,6 +21,18 @@ def _cunet_validator(size):            # waifu2x/models/cunet.py:124-125
 
 def _swin_validator(size):             # waifu2x/models/swin_unet.py:202-205
     return size > 16 and (size - 16) % 12 == 0 and (size - 16) % 16 == 0
+
+
+def _any_size_validator(size):         # upconv_7 / vgg_7 register no validator (nunif/models/model.py:51-62)
+    return True
+
+
+def _validator_for(name):
+    if "cunet" in name:
+        return _cunet_validator
+    if name in ("waifu2x.upconv_7", "waifu2x.vgg_7"):
+        return _any_size_validator
+    return _swin_validator
 
 
 class B200I2IModel:
@@ -38,7 +51,7 @@ class B200I2IModel:
         self.i2i_in_channels = 3
         self.i2i_default_tile_size = 256                              # model.py:69
         self.i2i_default_batch_size = 4
-        self._validator = _cunet_validator if "cunet" in name else _swin_validator
+        self._validator = _validator_for(name)
         lib = _lib.lib()
         if _handle is not None:
             self._h = _handle

@@ -103,6 +103,38 @@ def cunet_state_dict(seed=0, in_channels=3, out_channels=3):
 
 
 # ----------------------------------------------------------------------------
+# UpConv7 / VGG7 (waifu2x/models/upconv_7.py, vgg_7.py): nn.Sequential `net.{0,2,...,12}`
+# ----------------------------------------------------------------------------
+
+def _plain_stack(sd, g, widths):
+    for i in range(len(widths) - 1):
+        _conv(sd, g, f"net.{2 * i}", widths[i + 1], widths[i], 3, 3)
+
+
+def upconv7_state_dict(seed=0):
+    """Keys of ``waifu2x.upconv_7`` (upconv_7.py:12-26); the output ConvTranspose2d(256, 3, 4, 2, 3) is scaled so the tile
+    spans [0, 1] with both clamps hit."""
+    g = torch.Generator().manual_seed(50_000 + int(seed))
+    sd = {}
+    _plain_stack(sd, g, [3, 16, 32, 64, 128, 128, 256])
+    # weight (in, out, 4, 4); each output sees 2x2 taps x 256 channels
+    sd["net.12.weight"] = _normal(g, (256, 3, 4, 4), 1.2 * math.sqrt(1.0 / 1024))
+    sd["net.12.bias"] = torch.full((3,), 0.5) + _normal(g, (3,), 0.02)
+    return sd
+
+
+def vgg7_state_dict(seed=0):
+    """Keys of ``waifu2x.vgg_7`` (vgg_7.py:12-25); the output Conv2d(128, 3, 3) is scaled so the tile spans [0, 1] with both
+    clamps hit."""
+    g = torch.Generator().manual_seed(60_000 + int(seed))
+    sd = {}
+    _plain_stack(sd, g, [3, 32, 32, 64, 64, 128, 128])
+    sd["net.12.weight"] = _normal(g, (3, 128, 3, 3), 0.9 * math.sqrt(1.0 / 1152))
+    sd["net.12.bias"] = torch.full((3,), 0.35) + _normal(g, (3,), 0.02)   # the hidden activations' mean lifts the output by ~0.1
+    return sd
+
+
+# ----------------------------------------------------------------------------
 # SwinUNet family (waifu2x/models/swin_unet.py)
 # ----------------------------------------------------------------------------
 

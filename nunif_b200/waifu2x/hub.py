@@ -21,8 +21,8 @@ from .utils import Waifu2x
 MODEL_DIR = os.environ.get("NUNIF_B200_MODEL_DIR",
                            path.join(os.environ.get("NUNIF_HOME", path.expanduser("~/.nunif")), "waifu2x", "pretrained_models"))
 
-_ARCH_STYLES = (("swin_unet", ("art", "art_scan", "photo")), ("cunet", ("art",)))
-NO_4X_MODELS = {"cunet/art"}
+_ARCH_STYLES = (("swin_unet", ("art", "art_scan", "photo")), ("cunet", ("art",)), ("upconv_7", ("art", "photo")))
+NO_4X_MODELS = {"cunet/art", "upconv_7/art", "upconv_7/photo"}
 METHODS = ["noise", "scale", "noise_scale", "scale2x", "noise_scale2x", "scale4x", "noise_scale4x"]
 
 
