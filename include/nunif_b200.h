@@ -93,7 +93,8 @@ enum {
      * The widths are read off the tensor sizes (BEiT-L/16 for the released checkpoint). */
     NB200_MODEL_ZOEDEPTH_N = 12,
     NB200_MODEL_UPCONV_7 = 13,             /* waifu2x.upconv_7 (waifu2x/models/upconv_7.py:6-38): scale 2, offset 14 */
-    NB200_MODEL_VGG_7 = 14                 /* waifu2x.vgg_7    (waifu2x/models/vgg_7.py:6-36): scale 1, offset 7 */
+    NB200_MODEL_VGG_7 = 14,                /* waifu2x.vgg_7    (waifu2x/models/vgg_7.py:6-36): scale 1, offset 7 */
+    NB200_MODEL_LIGHT_INPAINT_V1 = 15      /* inpaint.light_inpaint_v1, iw3's image-mode hole inpainting (iw3/models/light_inpaint_v1.py) */
 };
 
 /* Create a model from named fp32 host tensors using the reference's state_dict
@@ -162,6 +163,24 @@ int nb200_row_flow_delta(nb200_model* m, const float* x, int B, int h, int w, fl
  * the L layers); L = nb200_mlbw_num_layers (2 or 4, read off the state_dict).  hole_mask models are not supported. */
 int nb200_mlbw_delta(nb200_model* m, const float* x, int B, int h, int w, float* delta, float* layer_weight, void* stream);
 int nb200_mlbw_num_layers(const nb200_model* m);
+
+/* iw3 forward_inpaint, image mode (iw3/forward_inpaint.py:18-40,69-103).  All tensors planar fp32 in image coordinates.
+ * nb200_inpaint_mask: the mask chain of forward_right / forward_left (:18-40): binarize => mask > 0; closing => mask_closing
+ *   (iw3/dilation.py:41-64,145-152); then dilate_outer(., outer_iter, base_width) and dilate_inner(., inner_iter, base_width)
+ *   (dilation.py:67-98; base_width <= 0 means None).  mirror = 1 gives the result forward_left computes on the flipped mask,
+ *   flipped back.  mask, out [B][1][H][W]; any stage may be switched off, so each reference function is available alone.
+ * nb200_inpaint_blur: clamp(blur15(mask) + mask, 0, 1), the mask half of LightInpaintV1.preprocess (light_inpaint_v1.py:88-100).
+ * nb200_light_inpaint: LightInpaintV1.infer(x, mask) (light_inpaint_v1.py:102-154) of a model of kind
+ *   NB200_MODEL_LIGHT_INPAINT_V1: x [B][3][H][W] (the warped eye), mask [B][1][H][W] (from nb200_inpaint_mask) -> out, same
+ *   shape as x.  mirror = 1 runs the network on x.flip(-1), mask.flip(-1) and flips the result (forward_left). */
+int nb200_inpaint_mask(const float* mask, int B, int H, int W, int binarize, int closing, int outer_iter, int inner_iter,
+                       int base_width, int mirror, float* out, void* stream);
+/* forward_inpaint.py:74-81: F.interpolate(x, (new_h, new_w), bilinear, antialias=True, align_corners=False) of x [B][3][H][W]
+ * (the max_width resize; no clamp). */
+int nb200_resize_bilinear_aa(const float* x, int B, int H, int W, int new_h, int new_w, float* out, void* stream);
+int nb200_inpaint_blur(const float* mask, int B, int H, int W, float* out, void* stream);
+int nb200_light_inpaint(nb200_model* m, const float* x, const float* mask, int B, int H, int W, int mirror, float* out,
+                        void* stream);
 
 /* backward_warp(c, grid, delta, delta_scale) of the learned warps (iw3/backward_warp.py:67-83,213-226):
  * c [B][3][H][W], delta [B][1][h][w] fp32 -> out [B][3][H][W] = clamp(grid_sample(c, grid + delta*delta_scale)). */

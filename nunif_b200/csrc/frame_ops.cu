@@ -51,6 +51,7 @@ struct DaPrepParams {
     float supy, supx;     // filter support: scale if scale >= 1 else 1
     float invy, invx;     // 1/scale if scale >= 1 else 1
     float mean[3], stdv[3];
+    int plain;            // 1: the resize alone (no clamp, no normalisation)
 };
 
 // ATen UpSampleKernel (_upsample_bilinear2d_aa): centre = scale*(i+0.5); taps [xmin, xmin+xsize);
@@ -86,8 +87,10 @@ __global__ void __launch_bounds__(128) da_preprocess_kernel(DaPrepParams p) {
             }
             acc += wy * h;
         }
-        acc = clamp01(acc);                                                    // depth_anything_model.py:104 / zoedepth_model.py:75
-        acc = __fdiv_rn(__fsub_rn(acc, p.mean[c]), p.stdv[c]);                 // :107-109 / :78-80
+        if (!p.plain) {
+            acc = clamp01(acc);                                                // depth_anything_model.py:104 / zoedepth_model.py:75
+            acc = __fdiv_rn(__fsub_rn(acc, p.mean[c]), p.stdv[c]);             // :107-109 / :78-80
+        }
         p.out[(((size_t)b * 3 + c) * OH + py) * OW + px] = acc;
     }
 }
@@ -147,8 +150,9 @@ extern "C" int nb200_da_preprocess_size(int H, int W, int lower_bound, int max_a
 }
 
 static int launch_prep(const float* x, int B, int H, int W, int frame_h, int frame_w, int pad_h, int pad_w, const float* mean,
-                       const float* stdv, float* out, void* stream) {
+                       const float* stdv, float* out, void* stream, int plain = 0) {
     DaPrepParams p;
+    p.plain = plain;
     p.x = x; p.out = out; p.B = B; p.H = H; p.W = W; p.oh = frame_h; p.ow = frame_w; p.pad_h = pad_h; p.pad_w = pad_w;
     p.sy = (float)H / (float)frame_h;   // area_pixel_compute_scale, align_corners=False, no scale_factor given
     p.sx = (float)W / (float)frame_w;
@@ -170,6 +174,14 @@ extern "C" int nb200_da_preprocess(const float* x, int B, int H, int W, int new_
     NB_CHECK(B > 0 && H > 0 && W > 0 && new_h > 0 && new_w > 0, "bad shape");
     const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};
     return launch_prep(x, B, H, W, new_h, new_w, 0, 0, mean, stdv, out, stream);
+}
+
+// F.interpolate(x, (new_h, new_w), mode="bilinear", antialias=True, align_corners=False) alone (iw3/forward_inpaint.py:74-81)
+extern "C" int nb200_resize_bilinear_aa(const float* x, int B, int H, int W, int new_h, int new_w, float* out, void* stream) {
+    NB_CHECK(x && out, "null pointer");
+    NB_CHECK(B > 0 && H > 0 && W > 0 && new_h > 0 && new_w > 0, "bad shape");
+    const float zero[3] = {0.f, 0.f, 0.f}, one[3] = {1.f, 1.f, 1.f};
+    return launch_prep(x, B, H, W, new_h, new_w, 0, 0, zero, one, out, stream, 1);
 }
 
 // iw3/zoedepth_model.py:30-71 (integers; Python float == C double, round() == round-half-even)

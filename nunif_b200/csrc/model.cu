@@ -12,6 +12,7 @@
 #include "depth_aa_kernels.h"
 #include "mlbw_kernels.h"
 #include "zoe_kernels.h"
+#include "inpaint_kernels.h"
 #include "../../include/nunif_b200.h"
 #include <map>
 #include <vector>
@@ -20,6 +21,7 @@
 #include <cmath>
 #include <memory>
 #include <tuple>
+#include <algorithm>
 
 namespace nb200 {
 
@@ -207,6 +209,7 @@ struct RfW;     // rowflow_model.inl
 struct AaW;     // depth_aa_model.inl
 struct MlW;     // mlbw_model.inl
 struct ZoeW;    // zoe_model.inl
+struct InpW;    // inpaint_model.inl
 
 }  // namespace nb200
 
@@ -225,6 +228,7 @@ struct nb200_model {
     std::shared_ptr<AaW> aa;
     std::shared_ptr<MlW> ml;
     std::shared_ptr<ZoeW> zoe;
+    std::shared_ptr<InpW> inp;
     uint8_t* ws = nullptr;
     size_t ws_bytes = 0;
     cudaStream_t copy_stream = nullptr;   // D2H side stream of nb200_tiled_render_host
@@ -485,6 +489,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 #include "depth_aa_model.inl"
 #include "mlbw_model.inl"
 #include "zoe_model.inl"
+#include "inpaint_model.inl"
 
 // ---------------------------------------------------------------------------------------------
 // C ABI
@@ -492,7 +497,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* names, const float* const* data,
                                   const int64_t* numel, int no_clip, nb200_model** out) {
     NB_CHECK(out && names && data && numel, "null pointer");
-    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_VGG_7, "unknown model kind");
+    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_LIGHT_INPAINT_V1, "unknown model kind");
     int dev = 0;
     NB_CUDA(cudaGetDevice(&dev));
     if (nb200_check_device(dev)) return 1;
@@ -526,6 +531,7 @@ extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* na
         case NB200_MODEL_ROW_FLOW_V3: m->rf = pack_row_flow(pk); m->scale = 1; m->offset = 32; m->blend = 4; break;   // row_flow_v3.py:37
         case NB200_MODEL_UPCONV_7: m->lg = pack_legacy(pk, true); m->scale = 2; m->offset = 14; m->blend = 0; break;  // upconv_7.py:11
         case NB200_MODEL_VGG_7: m->lg = pack_legacy(pk, false); m->scale = 1; m->offset = 7; m->blend = 0; break;     // vgg_7.py:11
+        case NB200_MODEL_LIGHT_INPAINT_V1: m->inp = pack_light_inpaint(pk); m->scale = 1; m->offset = 16; m->blend = 8; break;  // light_inpaint_v1.py:56
     }
     if (pk.err.empty())
         for (auto& kv : pk.src)
@@ -789,4 +795,45 @@ extern "C" int nb200_row_flow_delta(nb200_model* m, const float* x, int B, int h
     NB_CHECK(m->kind == NB200_MODEL_ROW_FLOW_V3 && m->rf, "model is not sbs.row_flow_v3");
     NB_CHECK(B > 0 && h > 0 && w > 0, "bad shape");
     return row_flow_forward(m, (cudaStream_t)stream, x, B, h, w, delta);
+}
+
+// iw3/dilation.py:67-98: n = max(round(W / base_width * n_iter), 1) (Python's round: half to even), 0 when n_iter <= 0
+static int dilation_run(int n_iter, int base_width, int W) {
+    if (n_iter <= 0) return 0;
+    if (base_width <= 0) return n_iter;
+    const double n = std::nearbyint((double)W / base_width * n_iter);
+    return n < 1 ? 1 : (int)n;
+}
+
+extern "C" int nb200_inpaint_mask(const float* mask, int B, int H, int W, int binarize, int closing, int outer_iter, int inner_iter,
+                                  int base_width, int mirror, float* out, void* stream) {
+    NB_CHECK(mask && out, "null pointer");
+    NB_CHECK(B > 0 && H > 0 && W > 0, "empty mask");
+    const int no = dilation_run(outer_iter, base_width, W), ni = dilation_run(inner_iter, base_width, W);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* tmp = nullptr;
+    if (closing) NB_CUDA(cudaMallocAsync((void**)&tmp, (size_t)B * H * W * 4, st));
+    // in image coordinates the mirrored mask's right-hand runs (dilate_outer) grow to the left
+    const int rc = inpaint_mask(st, mask, B, H, W, binarize, closing, mirror ? ni : no, mirror ? no : ni, tmp, out);
+    if (tmp) cudaFreeAsync(tmp, st);
+    return rc;
+}
+
+extern "C" int nb200_inpaint_blur(const float* mask, int B, int H, int W, float* out, void* stream) {
+    NB_CHECK(mask && out, "null pointer");
+    NB_CHECK(B > 0 && H > 0 && W > 0, "empty mask");
+    cudaStream_t st = (cudaStream_t)stream;
+    float* tmp = nullptr;
+    NB_CUDA(cudaMallocAsync((void**)&tmp, (size_t)B * H * W * 4, st));
+    const int rc = inpaint_blur(st, mask, B, H, W, 0, tmp, out);
+    cudaFreeAsync(tmp, st);
+    return rc;
+}
+
+extern "C" int nb200_light_inpaint(nb200_model* m, const float* x, const float* mask, int B, int H, int W, int mirror, float* out,
+                                   void* stream) {
+    NB_CHECK(m && x && mask && out, "null pointer");
+    NB_CHECK(m->kind == NB200_MODEL_LIGHT_INPAINT_V1 && m->inp, "model is not inpaint.light_inpaint_v1");
+    NB_CHECK(B > 0 && H > 0 && W > 0, "empty input");
+    return light_inpaint_forward(m, (cudaStream_t)stream, x, mask, B, H, W, mirror, out);
 }

@@ -8,7 +8,7 @@ CPU path.
 """
 from .backward_warp import apply_divergence_grid_sample  # noqa: F401
 from .forward_warp import apply_divergence_forward_warp  # noqa: F401
-from .dilation import dilate_edge, edge_dilation_parse, edge_dilation_is_enabled  # noqa: F401
+from .dilation import dilate_edge, edge_dilation_parse, edge_dilation_is_enabled, mask_closing, dilate_outer, dilate_inner  # noqa: F401
 from .depth_scaler import minmax_normalize, depth_mapper, EMAMinMaxScaler  # noqa: F401
 from .base_depth_model import BaseDepthModel  # noqa: F401
 from .anaglyph import apply_anaglyph_redcyan  # noqa: F401
@@ -21,4 +21,5 @@ from .zoedepth_model import ZoeDepthModel, ZoeDepthNet  # noqa: F401
 from .row_flow import RowFlowV3, MLBW, apply_divergence_nn_LR, apply_divergence_nn_delta, apply_divergence_nn_delta_weight  # noqa: F401
 from .depth_aa import DepthAA  # noqa: F401
 from .postprocess import postprocess_image, postprocess_padding, resize_bicubic_aa, equirectangular_projection  # noqa: F401
+from .forward_inpaint import ForwardInpaint, LightInpaintV1  # noqa: F401
 from .utils import apply_divergence, process_image  # noqa: F401

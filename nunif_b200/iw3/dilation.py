@@ -1,4 +1,4 @@
-"""Mirror of iw3/dilation.py:5-27,115-142."""
+"""Mirror of iw3/dilation.py:5-27,67-98,115-152."""
 import torch
 from .. import _lib
 from ._common import prep
@@ -43,3 +43,28 @@ def dilate_edge(x, n):
         _lib.check(lib.nb200_dilate_edge(_lib.ptr(x), B, h, w, int(x_iter), int(y_iter), _lib.ptr(out),
                                          _lib.ptr(ws), _lib.stream_ptr(x.device)))
     return out
+
+
+def _mask_op(mask, **kw):
+    from .forward_inpaint import inpaint_mask
+    return inpaint_mask(mask, **kw)
+
+
+def mask_closing(mask, kernel_size=3, n_iter=2):
+    """dilation.py:145-152 (3x3, 2 iterations): closing of a B,1,h,w mask, OR the input, as float."""
+    assert kernel_size == 3 and n_iter == 2, "the engine implements mask_closing's defaults"
+    return _mask_op(mask.float(), binarize=False, closing=True)
+
+
+def dilate_outer(mask, n_iter, base_width=None):
+    """dilation.py:67-82: runs grow n pixels to the right, n = max(round(W / base_width * n_iter), 1)."""
+    if n_iter <= 0:
+        return mask
+    return _mask_op(mask.float(), binarize=False, closing=False, outer_dilation=n_iter, base_width=base_width).to(mask.dtype)
+
+
+def dilate_inner(mask, n_iter, base_width=None):
+    """dilation.py:85-98: runs grow n pixels to the left."""
+    if n_iter <= 0:
+        return mask
+    return _mask_op(mask.float(), binarize=False, closing=False, inner_dilation=n_iter, base_width=base_width).to(mask.dtype)

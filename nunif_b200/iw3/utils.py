@@ -4,7 +4,7 @@ layers, which stay in the reference's host code).
 
 ``args`` is the reference's argparse namespace; the fields read here are the ones the reference reads on this path:
 ``method, mapper, convergence, divergence, synthetic_view, warp_steps, preserve_screen_border, stereo_width, disable_amp,
-state["convergence_model"]``.  Anything the engine does not implement raises ``NotImplementedError`` - never a silent
+mask_inner_dilation, mask_outer_dilation, inpaint_max_width, state["convergence_model"]``.  Anything the engine does not implement raises ``NotImplementedError`` - never a silent
 fallback."""
 import torch
 
@@ -42,8 +42,15 @@ def apply_divergence(depth, im, args, side_model, reset_pts=None):
     elif _WARP.get(method) == "forward":
         eyes = apply_divergence_forward_warp(im, depth, args.divergence, convergence=convergence, method=method,
                                              synthetic_view=args.synthetic_view, width_base=False)
-    elif method in {"forward_inpaint", "mlbw_l2_inpaint"}:
-        raise NotImplementedError(f"method {method} (video inpainting side model) is outside the H100 hot path")
+    elif method == "forward_inpaint":
+        # side_model.infer per frame (:333-367); image mode returns no delayed frames (flush() -> (None, None))
+        if side_model is None:
+            raise ValueError("method forward_inpaint needs side_model (nunif_b200.iw3.ForwardInpaint)")
+        eyes = side_model.infer(im, depth, args.divergence, convergence, synthetic_view=args.synthetic_view,
+                                inner_dilation=_arg(args, "mask_inner_dilation", 0), outer_dilation=_arg(args, "mask_outer_dilation", 0),
+                                max_width=_arg(args, "inpaint_max_width", None), enable_amp=True)
+    elif method == "mlbw_l2_inpaint":
+        raise NotImplementedError("method mlbw_l2_inpaint (mask_mlbw_l2 + video inpainting) is not implemented by the H100 engine")
     else:
         # the learned warps (row_flow*, mlbw*): apply_divergence_nn_LR with args.side_model (:363-385)
         stereo_width = _arg(args, "stereo_width", None)

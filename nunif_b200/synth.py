@@ -477,3 +477,40 @@ def zoedepth_state_dict(seed=0, cfg=None):
     conv("conditional_log_binomial.mlp.0", (33 + 128) // 2, 33 + 128, 1, gain=1.4)
     conv("conditional_log_binomial.mlp.2", 4, (33 + 128) // 2, 1, gain=2.0, bias=0.5)
     return sd
+
+
+# ----------------------------------------------------------------------------
+# iw3 inpainting (iw3/models/light_inpaint_v1.py)
+# ----------------------------------------------------------------------------
+
+def _gmlp_block(sd, g, prefix, C, N):
+    """One GMLPBlock (light_inpaint_v1.py:37-49, nunif/modules/attention.py:621-660).  proj_spatial gets about +-1/sqrt(N) and a
+    varied bias instead of the reference's init (+-1e-3/C, bias 1), which would make the token mixing invisible in the output."""
+    p = prefix + ".gmlp.gmlp"
+    _linear(sd, g, p + ".proj_in", 4 * C, C, gain=1.0, bias_std=0.2)
+    sd[p + ".proj_spatial.weight"] = (torch.rand((N, N, 1), generator=g) * 2 - 1) * (1.0 / math.sqrt(N))
+    sd[p + ".proj_spatial.bias"] = 0.5 + torch.rand((N,), generator=g)
+    _linear(sd, g, p + ".proj_out", C, 2 * C, gain=0.5, bias_std=0.05)
+    sd[prefix + ".norm1.weight"] = 1.0 + _normal(g, (C,), 0.1)
+    sd[prefix + ".norm2.weight"] = 1.0 + _normal(g, (2 * C,), 0.1)
+    _conv(sd, g, prefix + ".glu_conv.w1", C, C, 1, 1, gain=1.0, bias_std=0.1)
+    _conv(sd, g, prefix + ".glu_conv.w2", C, C // 2, 3, 3, gain=0.3, bias_std=0.02)
+
+
+def light_inpaint_v1_state_dict(seed=0):
+    """`inpaint.light_inpaint_v1` (81 tensors).  The output head is scaled so that the network's output spans [0, 1] around
+    0.5 and the hole pixels, which take the network output, show every stage; `mask_bias` is far from zero."""
+    g = _gen(seed)
+    sd = {}
+    C = 96
+    sd["mask_bias"] = _normal(g, (1, C, 1, 1), 0.5)
+    _conv(sd, g, "patch.0", C, 48, 1, 1, gain=1.0, bias_std=0.05)
+    _gmlp_block(sd, g, "enc1", C, 256)
+    _conv(sd, g, "down", 2 * C, C, 2, 2, gain=0.5, bias_std=0.02)
+    for i in range(4):
+        _gmlp_block(sd, g, f"enc2.{i}", 2 * C, 64)
+    _conv(sd, g, "up", 4 * C, 2 * C, 1, 1, gain=0.5, bias_std=0.02)
+    _gmlp_block(sd, g, "dec1", C, 256)
+    _conv(sd, g, "to_image.1", 48, C, 3, 3, gain=0.05, bias_std=0.0)
+    sd["to_image.1.bias"] = 0.5 + _normal(g, (48,), 0.05)
+    return sd
