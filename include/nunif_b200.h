@@ -349,7 +349,8 @@ int nb200_equirectangular(const float* c, int C, int H, int W, float* out, void*
  * bench.py for the live roofline figure.  report writes a JSON object
  * {"gemm": {"launches": n, "ms": t, "work": flops_or_bytes}, ...} and synchronises the device. */
 int nb200_tune_set(int key, int value);   /* kernel-selection knobs (csrc/gemm.cu g_tune), for tests and A/B runs */
-int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermediate `id` of nb200_zoedepth_forward to dev_buf */
+int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermediate `id` of nb200_zoedepth_forward (ids 0..14)
+                                                               or nb200_light_inpaint (ids 100..173, DESIGN.md §5) to dev_buf */
 int nb200_profile_enable(int on);
 int nb200_profile_report(char* buf, size_t cap);
 int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launch: class,ms,work,read_bytes,write_bytes */

@@ -473,7 +473,8 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
 
 #include "cunet_model.inl"
 #include "legacy_model.inl"
-// debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth forward is copied to `g_tap_buf`
+// debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth or light_inpaint_v1 forward is copied to `g_tap_buf`
+// (ZoeDepth ids 0..14 in zoe_model.inl; light_inpaint_v1 ids 100..173, table in DESIGN.md §5)
 static int g_tap_id = -1;
 static void* g_tap_buf = nullptr;
 static size_t g_tap_cap = 0;
@@ -740,7 +741,8 @@ extern "C" int nb200_tiled_render_host(nb200_model* m, const float* x_host, int 
     return rc;   // scratch_guard frees xd / od behind the last copy (stream-ordered)
 }
 
-// debug: copy intermediate `id` of the following nb200_zoedepth_forward calls into dev_buf (capacity bytes); id < 0 disables
+// debug: copy intermediate `id` of the following nb200_zoedepth_forward / nb200_light_inpaint calls into dev_buf (capacity bytes);
+// id < 0 disables
 extern "C" int nb200_debug_tap(int id, void* dev_buf, size_t capacity) {
     g_tap_id = id; g_tap_buf = dev_buf; g_tap_cap = capacity;
     return 0;
