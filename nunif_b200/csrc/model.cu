@@ -202,6 +202,20 @@ struct SwinW {
     std::vector<SwinBlockW> s1, s2, s3, s4, s5;
 };
 
+// Bump allocator over a model's workspace: every take() starts on a 256-byte boundary.  With a null base it hands out
+// null pointers and only advances `off`, which is how a forward's plan sizes its workspace (nb200_model::carve).
+struct Arena {
+    uint8_t* base = nullptr;
+    size_t off = 0;
+    template <typename T>
+    T* take(size_t count) {
+        off = (off + 255) & ~(size_t)255;
+        T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+        off += count * sizeof(T);
+        return p;
+    }
+};
+
 struct CUNetW;  // cunet_model.inl
 struct LegacyW; // legacy_model.inl
 struct DaW;     // depth_model.inl
@@ -281,6 +295,17 @@ struct nb200_model {
         ws_bytes = bytes;
         return 0;
     }
+    // A forward lists its workspace buffers once, as plan(Arena&): the first run over a null base sizes the workspace
+    // (plus a 4 KB tail guard), the second hands out the pointers into it.
+    template <typename F>
+    int carve(F plan) {
+        Arena size;
+        plan(size);
+        if (ensure_ws(size.off + 4096)) return 1;
+        Arena a{ws};
+        plan(a);
+        return 0;
+    }
 };
 
 namespace nb200 {
@@ -352,18 +377,6 @@ static void pack_swin(Packer& pk, SwinW& w, int r) {
 // ---------------------------------------------------------------------------------------------
 // forward helpers
 // ---------------------------------------------------------------------------------------------
-struct Arena {
-    uint8_t* base;
-    size_t off = 0, cap;
-    template <typename T>
-    T* take(size_t count) {
-        off = (off + 255) & ~(size_t)255;
-        T* p = reinterpret_cast<T*>(base + off);
-        off += count * sizeof(T);
-        return p;
-    }
-};
-
 // split > 0: the N outputs are written as N/split dense [M][split] planes (OUT_SPLIT); a_planes > 1: A is given as planes
 static int linear_flat(cudaStream_t st, const nb200_model* m, const Lin& l, const __half* A, long long M, int lda, __half* out,
                        int ldo, int act, const __half* res = nullptr, int ldr = 0, int split = 0, int a_planes = 1) {
@@ -385,40 +398,24 @@ static int swin_block(cudaStream_t st, const nb200_model* m, const SwinBlockW& w
                           m->at<__half>(w.fc2.w), m->at<float>(w.fc2.b));
 }
 
-static size_t swin_ws_bytes(const SwinW& w, int n, int T) {
-    const size_t Hc = T - 16, t1 = (size_t)n * Hc * Hc, C = w.C;
-    const size_t C5 = w.r == 4 ? 2 * C : C;
-    size_t b = 0;
-    auto add = [&](size_t elems) { b += ((elems * 2 + 255) & ~(size_t)255) + 256; };
-    add((size_t)n * (T - 2) * (T - 2) * 64);  // S1
-    add(t1 * C);                              // X1
-    add(t1 * C5);                             // ATT
-    add(t1 / 4 * 2 * C);                      // X2
-    add(t1 / 16 * 2 * C);                     // X3
-    add(t1 / 4 * 2 * C);                      // X4
-    add(t1 * 2 * C);                          // P2
-    add(t1 * C5);                             // X5
-    add(t1 * w.cs);                           // Y
-    return b + 4096;
-}
-
 static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n, int T, int down, void* z) {
     const SwinW& w = m->sw;
     NB_CHECK(T > 16 && (T - 16) % 12 == 0 && (T - 16) % 16 == 0, "invalid tile size for swin_unet (swin_unet.py:202-205)");
     const int C = w.C, Hc = T - 16, H2 = Hc / 2, H3 = Hc / 4, S1w = T - 2;
     const int C5 = w.r == 4 ? 2 * C : C;
-    if (m->ensure_ws(swin_ws_bytes(w, n, T))) return 1;
-    Arena a{m->ws, 0, m->ws_bytes};
     const size_t t1 = (size_t)n * Hc * Hc;
-    __half* S1 = a.take<__half>((size_t)n * S1w * S1w * 64);
-    __half* X1 = a.take<__half>(t1 * C);
-    __half* ATT = a.take<__half>(t1 * C5);
-    __half* X2 = a.take<__half>(t1 / 4 * 2 * C);
-    __half* X3 = a.take<__half>(t1 / 16 * 2 * C);
-    __half* X4 = a.take<__half>(t1 / 4 * 2 * C);
-    __half* P2 = a.take<__half>(t1 * 2 * C);
-    __half* X5 = a.take<__half>(t1 * C5);
-    __half* Y = a.take<__half>(t1 * w.cs);
+    __half *S1, *X1, *ATT, *X2, *X3, *X4, *P2, *X5, *Y;
+    if (m->carve([&](Arena& a) {
+            S1 = a.take<__half>((size_t)n * S1w * S1w * 64);
+            X1 = a.take<__half>(t1 * C);
+            ATT = a.take<__half>(t1 * C5);
+            X2 = a.take<__half>(t1 / 4 * 2 * C);
+            X3 = a.take<__half>(t1 / 16 * 2 * C);
+            X4 = a.take<__half>(t1 / 4 * 2 * C);
+            P2 = a.take<__half>(t1 * 2 * C);
+            X5 = a.take<__half>(t1 * C5);
+            Y = a.take<__half>(t1 * w.cs);
+        })) return 1;
 
     // patch stem (swin_unet.py:133-137) + crop 6 (:182) folded into the second conv's addressing
     if (stem_conv3x3(st, x, m->at<float>(w.stem.w), m->at<float>(w.stem.b), S1, n, T, T, 64, 64)) return 1;
