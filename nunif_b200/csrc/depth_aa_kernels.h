@@ -10,13 +10,6 @@ int aa_minmax(cudaStream_t st, const float* x, long long n, float* mm);
 // x fp32 [B][1][H][W] -> tokens fp16 [B][Hh][Wh][32]
 int aa_prep(cudaStream_t st, const float* x, const float* mm, int B, int H, int W, int ph1, int pw1, int Hh, int Wh, const float* w_in,
             const float* b_in, __half* out);
-// WindowMHA2d core (nunif/modules/attention.py:118-161): 8x8 windows, 2 heads of 16, additive (64 x 64) bias; shift != 0: the token
-// grid is zero padded by 4 on every side BEFORE the qkv projection, i.e. padded tokens carry q | k | v = the projection bias.
-// qkv fp16 [M][96] (q | k | v), qkv_bias fp32 [96], out fp16 [M][32]
-int aa_window_attention(cudaStream_t st, const __half* qkv, const float* qkv_bias, const float* bias, __half* out, int B, int Hh, int Wh,
-                        int shift);
-// replication pad 1 of a [B][H][W][C] fp16 tensor (C % 8 == 0)
-int aa_reppad(cudaStream_t st, const __half* x, int B, int H, int W, int C, __half* out);
 // proj_out (1x1 conv 32 -> 4) + pixel_shuffle(2) + crop + residual (+ clamp, or de-normalisation by mm): -> fp32 [B][1][H][W]
 int aa_out(cudaStream_t st, const __half* tok, const float* x, const float* mm, int B, int H, int W, int ph1, int pw1, int Hh, int Wh,
            const float* w_out, const float* b_out, int clamp, float* out);

@@ -1,13 +1,11 @@
-// Kernels of `sbs.mlbw` (iw3/models/mlbw.py:36-127), the multi-layer learned stereo warp (methods mlbw_l2 / mlbw_l4 [s]): everything
-// except its Linears / 1x1 / 3x3 convs, which run on the wgmma GEMM.  Like row_flow_v3 the network works on a (1, 8)
-// pixel-unshuffled token grid; it predicts L horizontal flow layers and L blending weights per pixel.
+// Kernels of `sbs.mlbw` (iw3/models/mlbw.py:36-127), the multi-layer learned stereo warp (methods mlbw_l2 / mlbw_l4 [s]): its input
+// and output stages.  Like row_flow_v3 the network works on a (1, 8) pixel-unshuffled token grid, through window-attention
+// blocks (window_mha.cu and the wgmma GEMM); it predicts L horizontal flow layers and L blending weights per pixel.
 #include "mlbw_kernels.h"
 
 namespace nb200 {
 
 namespace {
-
-constexpr int WSZ = 4, NT = 16, HD = 32;
 
 __global__ void __launch_bounds__(256) mlbw_prep_kernel(const float* __restrict__ x, __half* __restrict__ out, int B, int H, int W, int ph1,
                                                          int pw1, int Hp, int Wt, int C1, const float* __restrict__ w_in,
@@ -49,106 +47,6 @@ __global__ void __launch_bounds__(256) mlbw_prep_kernel(const float* __restrict_
         o[s] = __floats2half2_rn(a0, a1);
     }
     *reinterpret_cast<uint4*>(out + (((size_t)b * Hp + y) * Wt + xt) * (8 * C1) + c * 8) = *reinterpret_cast<const uint4*>(o);
-}
-
-// One thread per (window, head, query); K and V of the window staged in shared memory (dynamic: WPB x 16 x C x 2 halfs).
-template <int HEADS>
-__global__ void __launch_bounds__(128) mlbw_window_attention_kernel(const __half* __restrict__ qkv, const float* __restrict__ qkv_bias,
-                                                                     const float* __restrict__ bias, __half* __restrict__ out, int Hp, int Wt,
-                                                                     int pad_y, int pad_x, int nwx, int nwy, long long nwin) {
-    constexpr int C = HD * HEADS, TPW = NT * HEADS, WPB = 128 / TPW, VPT = C / 8;     // 16-byte vectors per token per matrix
-    extern __shared__ __align__(16) uint8_t smem_raw[];
-    __half* sK = reinterpret_cast<__half*>(smem_raw);                  // [WPB][NT][C]
-    __half* sV = sK + WPB * NT * C;
-    __shared__ float sBias[NT * NT];
-    if (threadIdx.x == 0) NB_PDL_TRIGGER();
-    for (int i = threadIdx.x; i < NT * NT; i += blockDim.x) sBias[i] = bias[i];
-    const int wl = threadIdx.x / TPW, r = threadIdx.x % TPW;
-    const long long win = (long long)blockIdx.x * WPB + wl;
-    const bool active = win < nwin;
-    int y0 = 0, x0 = 0, b = 0;
-    if (active) {
-        const int wx = (int)(win % nwx), wy = (int)((win / nwx) % nwy);
-        b = (int)(win / ((long long)nwx * nwy));
-        y0 = wy * WSZ - pad_y;
-        x0 = wx * WSZ - pad_x;
-        for (int i = r; i < NT * 2 * VPT; i += TPW) {
-            const int j = i / (2 * VPT), v = i % (2 * VPT);
-            const int y = y0 + j / WSZ, xx = x0 + j % WSZ;
-            uint4 val;
-            if (y >= 0 && y < Hp && xx >= 0 && xx < Wt) {
-                val = __ldg(reinterpret_cast<const uint4*>(qkv + (((size_t)b * Hp + y) * Wt + xx) * (3 * C) + C) + v);
-            } else {                                                   // a token of the zero padding: k | v = projection bias
-                __align__(16) __half2 h[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) h[k] = __floats2half2_rn(qkv_bias[C + v * 8 + 2 * k], qkv_bias[C + v * 8 + 2 * k + 1]);
-                val = *reinterpret_cast<const uint4*>(h);
-            }
-            if (v < VPT) *reinterpret_cast<uint4*>(sK + ((size_t)wl * NT + j) * C + v * 8) = val;
-            else *reinterpret_cast<uint4*>(sV + ((size_t)wl * NT + j) * C + (v - VPT) * 8) = val;
-        }
-    }
-    __syncthreads();
-    if (!active) return;
-    const int head = r / NT, qi = r % NT;
-    const int qy = y0 + qi / WSZ, qx = x0 + qi % WSZ;
-    if (qy < 0 || qy >= Hp || qx < 0 || qx >= Wt) return;              // cropped away after the attention
-    const size_t tokq = ((size_t)b * Hp + qy) * Wt + qx;
-    float q[HD];
-    {
-        const uint4* qp = reinterpret_cast<const uint4*>(qkv + tokq * (3 * C) + head * HD);
-#pragma unroll
-        for (int v = 0; v < HD / 8; ++v) {
-            const uint4 raw = __ldg(qp + v);
-            const __half2* hh = reinterpret_cast<const __half2*>(&raw);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const float2 f = __half22float2(hh[k]);
-                q[v * 8 + 2 * k] = f.x;
-                q[v * 8 + 2 * k + 1] = f.y;
-            }
-        }
-    }
-    float s[NT], mx = -1e30f;
-#pragma unroll
-    for (int j = 0; j < NT; ++j) {
-        const __half2* kp = reinterpret_cast<const __half2*>(sK + ((size_t)wl * NT + j) * C + head * HD);
-        float acc = 0.f;
-#pragma unroll
-        for (int k = 0; k < HD / 2; ++k) {
-            const float2 f = __half22float2(kp[k]);
-            acc = fmaf(q[2 * k], f.x, acc);
-            acc = fmaf(q[2 * k + 1], f.y, acc);
-        }
-        s[j] = acc * 0.17677669529663687f + sBias[qi * NT + j];       // 1/sqrt(32); additive attn_mask
-        mx = fmaxf(mx, s[j]);
-    }
-    float sum = 0.f;
-#pragma unroll
-    for (int j = 0; j < NT; ++j) { s[j] = __expf(s[j] - mx); sum += s[j]; }
-    const float inv = 1.f / sum;
-    float o[HD];
-#pragma unroll
-    for (int k = 0; k < HD; ++k) o[k] = 0.f;
-#pragma unroll
-    for (int j = 0; j < NT; ++j) {
-        const __half2* vp = reinterpret_cast<const __half2*>(sV + ((size_t)wl * NT + j) * C + head * HD);
-        const float pj = s[j] * inv;
-#pragma unroll
-        for (int k = 0; k < HD / 2; ++k) {
-            const float2 f = __half22float2(vp[k]);
-            o[2 * k] = fmaf(pj, f.x, o[2 * k]);
-            o[2 * k + 1] = fmaf(pj, f.y, o[2 * k + 1]);
-        }
-    }
-    __half* op = out + tokq * C + head * HD;
-#pragma unroll
-    for (int v = 0; v < HD / 8; ++v) {
-        __align__(16) __half2 hv[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) hv[k] = __floats2half2_rn(o[v * 8 + 2 * k], o[v * 8 + 2 * k + 1]);
-        *reinterpret_cast<uint4*>(op + v * 8) = *reinterpret_cast<const uint4*>(hv);
-    }
 }
 
 template <int L>
@@ -199,22 +97,6 @@ int mlbw_prep(cudaStream_t st, const float* x, int B, int H, int W, int ph1, int
               const float* b_in, __half* out) {
     const long long total = (long long)B * Hp * Wt * C1;
     mlbw_prep_kernel<<<(unsigned)cdiv64(total, 256), 256, (size_t)(C1 * 28) * 4, st>>>(x, out, B, H, W, ph1, pw1, Hp, Wt, C1, w_in, b_in);
-    NB_LAUNCHED();
-    return 0;
-}
-
-int mlbw_window_attention(cudaStream_t st, const __half* qkv, const float* qkv_bias, const float* bias, __half* out, int B, int Hp, int Wt,
-                          int heads, int pad_y, int pad_x) {
-    NB_CHECK(Hp % WSZ == 0 && Wt % WSZ == 0, "token grid must be a multiple of the 4x4 window");
-    NB_CHECK(heads == 2 || heads == 4, "sbs.mlbw has 2 or 4 layers (= attention heads)");
-    const int nwx = (Wt + 2 * pad_x) / WSZ, nwy = (Hp + 2 * pad_y) / WSZ;
-    const long long nwin = (long long)B * nwx * nwy;
-    const int wpb = 128 / (NT * heads);
-    const size_t smem = (size_t)wpb * NT * HD * heads * 2 * 2;
-    if (heads == 2)
-        mlbw_window_attention_kernel<2><<<(unsigned)cdiv64(nwin, wpb), 128, smem, st>>>(qkv, qkv_bias, bias, out, Hp, Wt, pad_y, pad_x, nwx, nwy, nwin);
-    else
-        mlbw_window_attention_kernel<4><<<(unsigned)cdiv64(nwin, wpb), 128, smem, st>>>(qkv, qkv_bias, bias, out, Hp, Wt, pad_y, pad_x, nwx, nwy, nwin);
     NB_LAUNCHED();
     return 0;
 }

@@ -8,10 +8,6 @@ namespace nb200 {
 // x fp32 [B][3][H][W] -> tokens fp16 [B][Hp][Wt][8 * C1] (channel = c * 8 + sw)
 int mlbw_prep(cudaStream_t st, const float* x, int B, int H, int W, int ph1, int pw1, int Hp, int Wt, int C1, const float* w_in,
               const float* b_in, __half* out);
-// WindowMHA2d core with 4x4 windows, heads of 32, additive (16 x 16) bias; pad_y / pad_x = 2 where the block is shifted in that
-// direction (zero padding BEFORE the qkv projection: padded tokens carry the projection bias).  qkv fp16 [M][3C], out fp16 [M][C]
-int mlbw_window_attention(cudaStream_t st, const __half* qkv, const float* qkv_bias, const float* bias, __half* out, int B, int Hp, int Wt,
-                          int heads, int pad_y, int pad_x);
 // pixel_shuffle (1, 8) of (t + t0) + lv1_out (ReplicationPad (4,4,0,0) + Conv2d(C1, 2L, (1,9))) + crop + chunk + softmax over the layers:
 // -> delta fp32 [B][L][H][W], layer_weight fp32 [B][L][H][W]
 int mlbw_out(cudaStream_t st, const __half* t, const __half* t0, int B, int H, int W, int ph1, int pw1, int Hp, int Wt, int C1, int L,

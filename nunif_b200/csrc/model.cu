@@ -13,6 +13,7 @@
 #include "mlbw_kernels.h"
 #include "zoe_kernels.h"
 #include "inpaint_kernels.h"
+#include "window_mha.h"
 #include "../../include/nunif_b200.h"
 #include <map>
 #include <vector>
@@ -483,6 +484,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 }
 
 #include "depth_model.inl"
+#include "wa_block.inl"
 #include "rowflow_model.inl"
 #include "depth_aa_model.inl"
 #include "mlbw_model.inl"

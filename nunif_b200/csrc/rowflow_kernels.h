@@ -7,11 +7,6 @@ namespace nb200 {
 // x fp32 [B][3][h][w] -> tokens fp16 [B][Hp][Wt][32]: replicate-pad to (Hp, Wt*8), pixel_unshuffle (1, 8) (channel = c*8 + sw),
 // channels 24..31 zero
 int rf_prep(cudaStream_t st, const float* x, int B, int h, int w, int Hp, int Wt, __half* out);
-// windowed 2-head attention with an additive (N x N) bias over ws x ws windows of the [B][Hp][Wt] token grid;
-// qkv fp16 [M][192] (q | k | v), out fp16 [M][64]
-int rf_window_attention(cudaStream_t st, const __half* qkv, const float* bias, __half* out, int B, int Hp, int Wt, int ws);
-// replication pad 1: [B][H][W][64] -> [B][H+2][W+2][64]
-int rf_reppad(cudaStream_t st, const __half* x, int B, int H, int W, __half* out);
 // pixel_shuffle (1, 8) + crop to (h, w) + replication pad 1 + conv3x3 (8 -> 1): tokens [B][Hp][Wt][64] -> delta fp32 [B][1][h][w]
 int rf_last_conv(cudaStream_t st, const __half* x, int B, int Hp, int Wt, int h, int w, const float* wt72, float bias, float* delta);
 

@@ -1,9 +1,6 @@
 // Non-GEMM kernels of the SwinUNet path (NHWC fp16 activations).
 //   stem_conv3x3_kernel     first 3x3 valid conv from the (3->8 padded) tile batch, LeakyReLU(0.1)
 //                           (swin_unet.py:133-134, cunet.py:14-15 conv.0); K=27 is too thin for tensor cores
-//   window_attention_kernel fused shifted-window attention core: roll + 6x6 partition + QK^T*scale +
-//                           relative-position bias + shift mask + softmax + PV + un-roll, all by index
-//                           arithmetic (torchvision swin_transformer.py:166-221 between the qkv and proj Linears)
 //   to_image_kernel         pixel_shuffle + clamp (+ bicubic-antialias /2,/4 + clamp) -> planar fp16 z
 //                           (swin_unet.py:108-115, :366-379)
 #include "common.cuh"
@@ -172,139 +169,6 @@ int stem_conv3x3(cudaStream_t st, const __half* x, const float* wt, const float*
     NB_LAUNCHED();
     return 0;
 }
-
-// ---------------------------------------------------------------------------------------------
-// window attention (6x6 windows, HEADS=6).  One CTA per window, one thread per (head, query).
-// qkv: [B][H][W][3C] fp16 (q | k | v, each head-major like torchvision's reshape :179-180)
-// out: [B][H][W][C] fp16 (pre-projection)
-// ---------------------------------------------------------------------------------------------
-constexpr int WS = 6, WTOK = 36, HEADS = 6;
-
-#if 0  // round-1 CUDA-core version, superseded by the tensor-core kernel in swin_attention_mma.cu
-template <int D>  // head dim: 16 (C=96) or 32 (C=192)
-__global__ void __launch_bounds__(224) window_attention_kernel(const __half* __restrict__ qkv, const float* __restrict__ bias_table,
-                                                               __half* __restrict__ out, int H, int W, int shift) {
-    constexpr int C = D * HEADS;
-    __shared__ __align__(16) __half sk[WTOK * C];
-    __shared__ __align__(16) __half sv[WTOK * C];
-    __shared__ float stab[121 * HEADS];
-    __shared__ int stok[WTOK];    // token -> flat pixel index (b*H + y)*W + x in the un-rolled map
-    __shared__ int sreg[WTOK];    // shift-mask region id (:193-203)
-    const int nww = W / WS;
-    const int wx = blockIdx.x % nww, wy = blockIdx.x / nww, b = blockIdx.y;
-    const int tid = threadIdx.x;
-    if (tid < WTOK) {
-        const int ry = wy * WS + tid / WS, rx = wx * WS + tid % WS;        // rolled coordinates
-        const int y = (ry + shift) % H, x = (rx + shift) % W;              // torch.roll(-shift) :166-167
-        stok[tid] = (b * H + y) * W + x;
-        int hr = 0, wr = 0;
-        if (shift > 0) {
-            hr = ry < H - WS ? 0 : (ry < H - shift ? 1 : 2);
-            wr = rx < W - WS ? 0 : (rx < W - shift ? 1 : 2);
-        }
-        sreg[tid] = hr * 3 + wr;
-    }
-    for (int i = tid; i < 121 * HEADS; i += blockDim.x) stab[i] = bias_table[i];
-    __syncthreads();
-    // stage K and V of the 36 tokens (16-byte vectors, coalesced per token row)
-    constexpr int VPT = C / 8;  // uint4 per token per matrix
-    for (int i = tid; i < WTOK * VPT; i += blockDim.x) {
-        const int t = i / VPT, v = i - t * VPT;
-        const uint4* src = reinterpret_cast<const uint4*>(qkv + (size_t)stok[t] * (3 * C));
-        reinterpret_cast<uint4*>(sk)[t * VPT + v] = __ldg(src + VPT + v);
-        reinterpret_cast<uint4*>(sv)[t * VPT + v] = __ldg(src + 2 * VPT + v);
-    }
-    __syncthreads();
-    if (tid >= WTOK * HEADS) return;
-    const int head = tid / WTOK, q = tid - head * WTOK;
-    const float scale = (D == 16) ? 0.25f : 0.17677669529663687f;  // (C // heads) ** -0.5 (:187)
-    float qv[D];
-    {
-        const __half* qp = qkv + (size_t)stok[q] * (3 * C) + head * D;
-#pragma unroll
-        for (int j = 0; j < D; j += 8) {
-            const uint4 v = __ldg(reinterpret_cast<const uint4*>(qp + j));
-            const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const float2 f = __half22float2(h[k]);
-                qv[j + 2 * k] = f.x * scale;
-                qv[j + 2 * k + 1] = f.y * scale;
-            }
-        }
-    }
-    const int qy = q / WS, qx = q - qy * WS, qreg = sreg[q];
-    float s[WTOK];
-    float mx = -1e30f;
-#pragma unroll
-    for (int k = 0; k < WTOK; ++k) {
-        const __half* kp = sk + k * C + head * D;
-        float acc = 0.f;
-#pragma unroll
-        for (int j = 0; j < D; j += 8) {
-            const uint4 v = *reinterpret_cast<const uint4*>(kp + j);
-            const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h[e]);
-                acc += qv[j + 2 * e] * f.x + qv[j + 2 * e + 1] * f.y;
-            }
-        }
-        const int ky = k / WS, kx = k - ky * WS;
-        acc += stab[((qy - ky + WS - 1) * (2 * WS - 1) + (qx - kx + WS - 1)) * HEADS + head];  // :49-59,:190
-        if (sreg[k] != qreg) acc += -100.0f;                                                    // :204-209
-        s[k] = acc;
-        mx = fmaxf(mx, acc);
-    }
-    float sum = 0.f;
-#pragma unroll
-    for (int k = 0; k < WTOK; ++k) {
-        s[k] = __expf(s[k] - mx);
-        sum += s[k];
-    }
-    const float inv = 1.f / sum;
-    float o[D];
-#pragma unroll
-    for (int j = 0; j < D; ++j) o[j] = 0.f;
-#pragma unroll
-    for (int k = 0; k < WTOK; ++k) {
-        const float pk = s[k] * inv;
-        const __half* vp = sv + k * C + head * D;
-#pragma unroll
-        for (int j = 0; j < D; j += 8) {
-            const uint4 v = *reinterpret_cast<const uint4*>(vp + j);
-            const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float2 f = __half22float2(h[e]);
-                o[j + 2 * e] += pk * f.x;
-                o[j + 2 * e + 1] += pk * f.y;
-            }
-        }
-    }
-    __half* op = out + (size_t)stok[q] * C + head * D;
-#pragma unroll
-    for (int j = 0; j < D; j += 8) {
-        __align__(16) __half2 hv[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) hv[e] = __floats2half2_rn(o[j + 2 * e], o[j + 2 * e + 1]);
-        *reinterpret_cast<uint4*>(op + j) = *reinterpret_cast<const uint4*>(hv);
-    }
-}
-
-int window_attention(cudaStream_t st, const __half* qkv, const float* bias_table, __half* out, int B, int H, int W, int C,
-                     int shift) {
-    NB_CHECK(H % WS == 0 && W % WS == 0, "feature map must be a multiple of the 6x6 window");
-    NB_CHECK(C == 96 || C == 192, "window attention supports C=96 (d=16) and C=192 (d=32)");
-    if (WS >= H) shift = 0;  // torchvision :151-155
-    dim3 grid((H / WS) * (W / WS), B);
-    ProfScope ps(st, PC_ATTN, (double)B * H * W * C * 4 * 2);  // bytes: read q,k,v + write out
-    if (C == 96) window_attention_kernel<16><<<grid, 224, 0, st>>>(qkv, bias_table, out, H, W, shift);
-    else window_attention_kernel<32><<<grid, 224, 0, st>>>(qkv, bias_table, out, H, W, shift);
-    NB_LAUNCHED();
-    return 0;
-}
-#endif
 
 // ---------------------------------------------------------------------------------------------
 // ToImage tail: y [n][Hs][Ws][cs] fp16 with channel = c*r*r + dy*r + dx (F.pixel_shuffle) ->

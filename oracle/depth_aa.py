@@ -1,35 +1,14 @@
 """ORACLE (test infrastructure only - never imported by nunif_b200/): CPU/torch restatement of `iw3.depth_aa`
 (iw3/models/depth_aa.py:11-87), the learned depth anti-aliasing filter applied after Depth-Anything when
-`depth_aa=True` (iw3/depth_anything_model.py:153-154), incl. the shifted WindowMHA2d
-(nunif/modules/attention.py:118-161: zero padding by half a window, window attention, crop).
+`depth_aa=True` (iw3/depth_anything_model.py:153-154).  Its three window-attention blocks (the first and the last
+shifted) are oracle/wa_block.py's.
 
 SURVEY.md 8f rank 4 "next" row: the engine raises NotImplementedError for depth_aa today; this pins the algorithm
 against the real reference model (tests/golden/depth_aa.npz, oracle/gen_golden.py depth_aa) for the round that ports it.
 """
 import torch
 import torch.nn.functional as F
-from .row_flow import window_bias
-
-
-def window_mha2d(sd, p, x, ws, heads, shift, bias):
-    """WindowMHA2d.forward with a square window and shift in both directions or none."""
-    pad = ws // 2 if shift else 0
-    if pad:
-        x = F.pad(x, (pad, pad, pad, pad), mode="constant", value=0)
-    B, C, H, W = x.shape
-    oh, ow = H // ws, W // ws
-    t = x.reshape(B, C, oh, ws, ow, ws).permute(0, 2, 4, 3, 5, 1).reshape(B * oh * ow, ws * ws, C)
-    qkv = F.linear(t, sd[p + "mha.qkv_proj.weight"], sd[p + "mha.qkv_proj.bias"])
-    q, k, v = qkv.split(C, dim=-1)
-    d = C // heads
-    q, k, v = [a.reshape(-1, ws * ws, heads, d).permute(0, 2, 1, 3) for a in (q, k, v)]
-    a = F.scaled_dot_product_attention(q, k, v, attn_mask=bias.to(q.dtype))
-    a = a.permute(0, 2, 1, 3).reshape(-1, ws * ws, C)
-    a = F.linear(a, sd[p + "mha.head_proj.weight"], sd[p + "mha.head_proj.bias"])
-    a = a.reshape(B, oh, ow, ws, ws, C).permute(0, 5, 1, 3, 2, 4).reshape(B, C, H, W)
-    if pad:
-        a = a[:, :, pad:-pad, pad:-pad]
-    return a
+from .wa_block import wa_block
 
 
 def depth_aa_forward(sd, x, clamp=True):
@@ -43,11 +22,7 @@ def depth_aa_forward(sd, x, clamp=True):
     x = F.pixel_unshuffle(x, 2)
     x = F.conv2d(x, sd["proj_in.weight"], sd["proj_in.bias"])
     for i, shift in enumerate((True, False, True)):
-        p = f"blocks.{i}."
-        x = x + window_mha2d(sd, p + "mha.", x, 8, 2, shift, window_bias(sd, p + "bias.", 8))
-        m = F.gelu(F.conv2d(x, sd[p + "conv_mlp.0.weight"], sd[p + "conv_mlp.0.bias"]))
-        m = F.pad(m, (1, 1, 1, 1), mode="replicate")
-        x = x + F.leaky_relu(F.conv2d(m, sd[p + "conv_mlp.3.weight"], sd[p + "conv_mlp.3.bias"]), 0.1)
+        x = wa_block(sd, f"blocks.{i}.", x, 8, 2, shift, act=True)
     x = F.conv2d(x, sd["proj_out.weight"], sd["proj_out.bias"])
     x = F.pixel_shuffle(x, 2)
     x = x[:, :, ph1:x.shape[2] - ph2, pw1:x.shape[3] - pw2]

@@ -8,32 +8,11 @@ sbs.mlbw today; this pins the algorithm against the real reference model (tests/
 """
 import torch
 import torch.nn.functional as F
-from .row_flow import window_bias, make_input
+from .row_flow import make_input
+from .wa_block import wa_block
 
 PACK = 8
 MOD = 4
-
-
-def _window_mha(sd, p, x, ws, heads, shift, bias):
-    """WindowMHA2d (nunif/modules/attention.py:118-161): zero padding by ws/2 in the shifted directions, attention, crop.
-    shift = bool (both directions) or (shift_h, shift_w)."""
-    sh, sw = shift if isinstance(shift, tuple) else (shift, shift)
-    ph, pw = (ws // 2 if sh else 0), (ws // 2 if sw else 0)
-    pad = ph or pw
-    if pad:
-        x = F.pad(x, (pw, pw, ph, ph), mode="constant", value=0)
-    B, C, H, W = x.shape
-    oh, ow = H // ws, W // ws
-    t = x.reshape(B, C, oh, ws, ow, ws).permute(0, 2, 4, 3, 5, 1).reshape(B * oh * ow, ws * ws, C)
-    qkv = F.linear(t, sd[p + "mha.qkv_proj.weight"], sd[p + "mha.qkv_proj.bias"])
-    q, k, v = qkv.split(C, dim=-1)
-    d = C // heads
-    q, k, v = [a.reshape(-1, ws * ws, heads, d).permute(0, 2, 1, 3) for a in (q, k, v)]
-    a = F.scaled_dot_product_attention(q, k, v, attn_mask=bias.to(q.dtype))
-    a = a.permute(0, 2, 1, 3).reshape(-1, ws * ws, C)
-    a = F.linear(a, sd[p + "mha.head_proj.weight"], sd[p + "mha.head_proj.bias"])
-    a = a.reshape(B, oh, ow, ws, ws, C).permute(0, 5, 1, 3, 2, 4).reshape(B, C, H, W)
-    return a[:, :, ph:a.shape[2] - ph, pw:a.shape[3] - pw] if pad else a
 
 
 def mlbw_delta(sd, x, num_layers=2, small=False):
@@ -47,10 +26,7 @@ def mlbw_delta(sd, x, num_layers=2, small=False):
     B, C1, Hp, Wp = x1.shape
     t = x1.reshape(B, C1, Hp, 1, Wp // PACK, PACK).permute(0, 1, 3, 5, 2, 4).reshape(B, C1 * PACK, Hp, Wp // PACK)
     for i, shift in enumerate(((False, True), False) if small else (True, False, True, False)):       # mlbw.py:53-64
-        p = f"lv2.{i}."
-        t = t + _window_mha(sd, p + "mha.", t, 4, num_layers, shift, window_bias(sd, p + "bias.", 4))
-        m = F.gelu(F.conv2d(t, sd[p + "conv_mlp.0.weight"], sd[p + "conv_mlp.0.bias"]))
-        t = t + F.conv2d(F.pad(m, (1, 1, 1, 1), mode="replicate"), sd[p + "conv_mlp.3.weight"], sd[p + "conv_mlp.3.bias"])
+        t = wa_block(sd, f"lv2.{i}.", t, 4, num_layers, shift, act=False)
     C = t.shape[1]
     t = t.reshape(B, C // PACK, 1, PACK, Hp, Wp // PACK).permute(0, 1, 4, 2, 5, 3).reshape(B, C // PACK, Hp, Wp)
     y = F.conv2d(F.pad(t + x1, (4, 4, 0, 0), mode="replicate"), sd["lv1_out.1.weight"], sd["lv1_out.1.bias"])

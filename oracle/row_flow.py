@@ -8,38 +8,11 @@ Pinned against the real reference model (create_model("sbs.row_flow_v3") with a 
 """
 import torch
 import torch.nn.functional as F
+from .wa_block import wa_block
 
 OFFSET = 32
 MOD = 12
 PACK = 8
-
-
-def window_bias(sd, p, ws):
-    """WindowScoreBias.forward (nunif/modules/attention.py:408-420): (N, N) additive attention bias."""
-    N = ws * ws
-    b = F.linear(F.gelu(F.linear(sd[p + "delta"], sd[p + "to_bias.0.weight"], sd[p + "to_bias.0.bias"])),
-                 sd[p + "to_bias.2.weight"], sd[p + "to_bias.2.bias"])
-    return b[sd[p + "index"]].reshape(N, N)
-
-
-def _wa_block(sd, p, x, ws):
-    """WABlock.forward (row_flow_v3.py:26-29); x: B,C,H,W."""
-    B, C, H, W = x.shape
-    oh, ow = H // ws, W // ws
-    t = x.reshape(B, C, oh, ws, ow, ws).permute(0, 2, 4, 3, 5, 1).reshape(B * oh * ow, ws * ws, C)     # bchw_to_bnc
-    qkv = F.linear(t, sd[p + "mha.mha.qkv_proj.weight"], sd[p + "mha.mha.qkv_proj.bias"])
-    q, k, v = qkv.split(C, dim=-1)
-    heads, d = 2, C // 2
-    q, k, v = [a.reshape(-1, ws * ws, heads, d).permute(0, 2, 1, 3) for a in (q, k, v)]
-    a = F.scaled_dot_product_attention(q, k, v, attn_mask=window_bias(sd, p + "bias.", ws).to(q.dtype))
-    a = a.permute(0, 2, 1, 3).reshape(-1, ws * ws, C)
-    a = F.linear(a, sd[p + "mha.mha.head_proj.weight"], sd[p + "mha.mha.head_proj.bias"])
-    a = a.reshape(B, oh, ow, ws, ws, C).permute(0, 5, 1, 3, 2, 4).reshape(B, C, H, W)                    # bnc_to_bchw
-    x = x + a
-    m = F.gelu(F.conv2d(x, sd[p + "conv_mlp.0.weight"], sd[p + "conv_mlp.0.bias"]))
-    m = F.pad(m, (1, 1, 1, 1), mode="replicate")
-    m = F.leaky_relu(F.conv2d(m, sd[p + "conv_mlp.3.weight"], sd[p + "conv_mlp.3.bias"]), 0.1)
-    return x + m
 
 
 def row_flow_delta(sd, x):
@@ -51,8 +24,8 @@ def row_flow_delta(sd, x):
     B, C, Hp, Wp = x.shape
     x = x.reshape(B, C, Hp, 1, Wp // PACK, PACK).permute(0, 1, 3, 5, 2, 4).reshape(B, C * PACK, Hp, Wp // PACK)   # pixel_unshuffle (1, 8)
     x = F.conv2d(x, sd["blocks.0.weight"], sd["blocks.0.bias"])
-    x = _wa_block(sd, "blocks.1.", x, 4)
-    x = _wa_block(sd, "blocks.2.", x, 3)
+    x = wa_block(sd, "blocks.1.", x, 4, 2, False, act=True)
+    x = wa_block(sd, "blocks.2.", x, 3, 2, False, act=True)
     C = x.shape[1]
     x = x.reshape(B, C // PACK, 1, PACK, Hp, Wp // PACK).permute(0, 1, 4, 2, 5, 3).reshape(B, C // PACK, Hp, Wp)  # pixel_shuffle (1, 8)
     x = x[:, :, :H, :W]

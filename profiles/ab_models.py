@@ -11,10 +11,11 @@ The comparison build is made from a git revision into the git-ignored profiles/_
 Both builds get the same seeded weights (nunif_b200.synth) and inputs through each model's C ABI entry, at production sizes:
 swin_unet 1x / 2x / 4x (and 4x's to_2x) and UpCUNet / CUNet / UpConv7 / VGG7 on 256^2 tiles in batches of 16, Depth-Anything-V2
 S / B / L at the iw3_1080p network input (4 x 392x686), ZoeD_N at 384x512 and 384x704 (batch 2), and row_flow_v3, mlbw
-(2 and 4 layers), depth_aa (all three modes) and light_inpaint_v1 (with and without the mirror) on 1080p frames.  Every output
-must be bit-identical, and so must ZoeD_N's debug taps 0..14 and light_inpaint_v1's taps 100..173; Depth-Anything must leave
-an armed ZoeD_N tap buffer untouched.  Then the DA-S and ZoeD_N (384x512) forwards are timed: REPS CUDA-event windows per
-build, the order of the two builds alternating.  The device name and its power limit are printed with the timings.
+(2 and 4 layers, and 2 layers `small`: two blocks shifted along x only), depth_aa (all three modes) and light_inpaint_v1 (with
+and without the mirror) on 1080p frames.  Every output must be bit-identical, and so must ZoeD_N's debug taps 0..14 and
+light_inpaint_v1's taps 100..173; Depth-Anything must leave an armed ZoeD_N tap buffer untouched.  Then the cases in TIMED
+are timed: REPS CUDA-event windows per build, the order of the two builds alternating (a depth_aa call runs its three modes).
+The device name and its power limit are printed with the timings.
 """
 import argparse
 import ctypes
@@ -32,6 +33,7 @@ FRAME = (1080, 1920)
 REPS = 7
 WINDOW_MS = 150.0
 TAP_BYTES = 256 << 20
+TIMED = ("depth_anything_v2_vits", "zoedepth_n_384x512", "row_flow_v3", "mlbw_2", "mlbw_4", "depth_aa")
 INPAINT_TAPS = [100, 101] + [110 + 10 * k + s for k in range(6) for s in range(8)] + [170, 171, 172, 173]
 
 
@@ -144,6 +146,9 @@ def cases():
             check(lib, lib.nb200_mlbw_delta(h, p(t["x"]), B, H, W, p(d), p(lw), stream()))
             return [d, lw]
         out.append((f"mlbw_{L}", 11, lambda L=L: synth.mlbw_state_dict(0, L), lambda dev: {"x": stereo_input(dev, B, 3)}, mlbw))
+        if L == 2:   # `small` is read off the missing lv2.2 / lv2.3: shifted blocks pad along x only (pad_y = 0, pad_x = 2)
+            small = lambda: {k: v for k, v in synth.mlbw_state_dict(0, 2).items() if not k.startswith(("lv2.2.", "lv2.3."))}
+            out.append(("mlbw_2_small", 11, small, lambda dev: {"x": stereo_input(dev, B, 3)}, mlbw))
 
     def depth_aa(lib, h, t):
         res = []
@@ -259,7 +264,7 @@ def main():
                     row["zoe_taps_answered"] = [i for i in range(15)
                                                 if bool(tapped(libs["new"], i, taps["new"], lambda: call(libs["new"], h["new"], t))[0].any())]
                     row["equal"] = row["equal"] and not row["zoe_taps_answered"]
-                if name in ("depth_anything_v2_vits", "zoedepth_n_384x512"):
+                if name in TIMED:
                     timings[name] = time_ab({k: (lambda k=k: call(libs[k], h[k], t)) for k in libs})
                     tr = timings[name]
                     row["timing"] = tr
