@@ -413,6 +413,8 @@ __global__ void __launch_bounds__(FA_THREADS, 2) swin_attn_fused_kernel(const __
         fence_barrier_init();
     }
     __syncthreads();
+    // the block tail (swin_block.cu, a PDL launch) may start its prologue and weight loads once every CTA of this grid is resident
+    if (tid == 0) NB_PDL_TRIGGER();
 
     if (warp == GEMM_CONSUMER_THREADS / 32) {
         // ===================== weight producer =====================

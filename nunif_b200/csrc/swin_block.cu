@@ -1,13 +1,21 @@
 // Fused tail of one SwinTransformerBlock (torchvision swin_transformer.py:228 proj, :453-455; MLP = Linear-GELU-Linear,
 // ratio 2, Identity norms: waifu2x/models/swin_unet.py:16-17,31):
 //   x1 = x + att . Wp^T + bp   (att == nullptr: x1 = x);   x <- x1 + gelu(x1 . W1^T + b1) . W2^T + b2
-// x1 and the 2C hidden tensor never reach HBM.  One CTA = 128 tokens = two wgmma warpgroups of 64 rows.
-//   warp 8    : TMA: the x (and att) tile once, then the weight blocks [rows][32] (64B swizzle) through a ring, in the
-//               order the consumers use them: Wp (C/32 blocks), then per 64-wide hidden chunk W1 (C/32) and W2 (2)
-//   warps 0-7 : proj into registers, x1 written in place over the x tile (A operand of fc1, residual of fc2); per hidden
-//               chunk fc1 into registers, bias + GELU, packed to fp16 A fragments in registers and fed straight to the fc2
-//               wgmma (A from registers), whose C-wide accumulator lives in registers for the whole tile; the output is
-//               written in place over the x tile and stored with TMA.
+// x1 and the 2C hidden tensor never reach HBM.  One CTA = 128 tokens = two wgmma warpgroups of 64 rows + a producer warpgroup.
+//   warp 8    : TMA: the weights through a ring of [128 C]-byte stages, in the order the consumers use them: Wp two K-blocks
+//               per stage ([C][64]), then per 64-wide hidden chunk h one stage of W1 rows ([64][C]) and one of W2 columns
+//               ([C][64]), with W1(h + 1) ahead of W2(h).  The stages that fit the ring are
+//               issued before griddepcontrol.wait (the weights do not depend on the previous kernel), the att tile (one
+//               barrier per 32-column K-block) and the x tile (one barrier) after it.
+//   warps 0-7 : proj into registers as the att K-blocks land, x1 written in place over the x tile (A operand of fc1, residual
+//               of fc2); per hidden chunk fc1 into registers, bias + GELU, packed to fp16 A fragments in registers and fed
+//               straight to the fc2 wgmma (A from registers), whose C-wide accumulator lives in registers for the whole tile;
+//               the output is written in place over the x tile and stored with TMA.
+// Each ring stage is one wgmma commit group and is released when that group has retired, so the tensor pipe is never drained
+// inside a GEMM.  fc1 of chunk h + 1 goes into a second hidden accumulator before the GELU of chunk h, so that it runs with
+// tensor work in flight.  That takes ~210 registers per consumer thread (fc2's accumulator alone is C/2): with 288 threads
+// three warps share an SM sub-partition's 64 KB register file, which caps a thread at 168, so the producer is a whole
+// warpgroup (warps 8-11, one of them working) that gives its registers to the consumers with setmaxnreg.
 // The two entry points of include/nunif_b200.h that expose the fused block kernels (head: swin_attention_mma.cu).
 #include "gemm_wgmma.cuh"
 #include "swin_kernels.h"
@@ -15,13 +23,15 @@
 
 namespace nb200 {
 
-constexpr int FM_ROWS = 128, FM_STAGES = 6, FM_THREADS = GEMM_CONSUMER_THREADS + 32;
+constexpr int FM_ROWS = 128, FM_STAGES = 5, FM_THREADS = GEMM_CONSUMER_THREADS + 128;
+constexpr int FM_PRODUCER_REGS = 40, FM_CONSUMER_REGS = 232;   // 2 x 232 + 40 per sub-partition: 504 x 32 <= 16384
 
 template <int C>
 struct FmCfg {
+    static constexpr int KB = C / 32;
     static constexpr int TILE = FM_ROWS * C * 2;   // one [128][C] activation tile (C/32 boxes of [128][32])
-    static constexpr int SLOT = C * 64;            // largest weight block: [C rows][32]
-    static constexpr int SMEM = 2 * TILE + FM_STAGES * SLOT + (2 * FM_STAGES + 1) * 8 + 1024;
+    static constexpr int STAGE = 128 * C;          // [64][C] of W1, [C][64] of W2 or of Wp
+    static constexpr int SMEM = 2 * TILE + FM_STAGES * STAGE + (2 * FM_STAGES + KB + 1) * 8 + 1024;
 };
 
 struct FmMaps {
@@ -31,97 +41,157 @@ struct FmMaps {
 template <int K>
 __device__ __forceinline__ float (&half96(float (&acc)[K], int h))[48] { return *reinterpret_cast<float(*)[48]>(&acc[48 * h]); }
 
-template <int C>
+// mbar_wait without the diagnostic printf of its timeout: a function call inside a wgmma pipeline (between a wgmma and the
+// wait_group that retires it) makes ptxas serialise every wgmma of the kernel.  Still bounded: a protocol bug traps.
+__device__ __forceinline__ void fm_wait(uint64_t* bar, uint32_t parity) {
+    const uint32_t addr = smem_u32(bar);
+    uint32_t done = 0;
+#pragma unroll 1
+    for (uint32_t it = 0; it < (1u << 18) && !done; ++it)
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(done) : "r"(addr), "r"(parity), "r"(20000u) : "memory");
+    if (!done) __trap();
+}
+
+// wgmma.wait_group 0 or 1, with a count that is a constant after unrolling
+__device__ __forceinline__ void wgmma_wait_n(int n) {
+    if (n == 0) wgmma_wait<0>();
+    else wgmma_wait<1>();
+}
+
+// PROJ (att != nullptr) is a template parameter: wgmmas under a run-time branch make ptxas serialise all of them.
+template <int C, bool PROJ>
 __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __grid_constant__ FmMaps maps, const float* __restrict__ bp,
-                                                                       const float* __restrict__ b1, const float* __restrict__ b2,
-                                                                       int has_proj) {
+                                                                     const float* __restrict__ b1, const float* __restrict__ b2) {
     using Cfg = FmCfg<C>;
-    constexpr int KB = C / 32, NH = 2 * C / 64, NHALF = C / 96;
+    constexpr int KB = Cfg::KB, NP = (KB + 1) / 2, NH = 2 * C / 64, NHALF = C / 96;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
     uint8_t* sx = smem;
     uint8_t* satt = smem + Cfg::TILE;
     uint8_t* ring = smem + 2 * Cfg::TILE;
-    uint64_t* full = reinterpret_cast<uint64_t*>(ring + FM_STAGES * Cfg::SLOT);
+    uint64_t* full = reinterpret_cast<uint64_t*>(ring + FM_STAGES * Cfg::STAGE);
     uint64_t* empty = full + FM_STAGES;
-    uint64_t* xbar = empty + FM_STAGES;
+    uint64_t* abar = empty + FM_STAGES;   // [KB]: att K-block kb
+    uint64_t* xbar = abar + KB;
     const int tid = threadIdx.x, warp = tid >> 5;
     const int row_base = blockIdx.x * FM_ROWS;
     if (tid == GEMM_CONSUMER_THREADS) {
         tma_prefetch_desc(&maps.x);
         tma_prefetch_desc(&maps.w1);
         tma_prefetch_desc(&maps.w2);
+        if (PROJ) {
+            tma_prefetch_desc(&maps.att);
+            tma_prefetch_desc(&maps.wp);
+        }
         for (int s = 0; s < FM_STAGES; ++s) {
             mbar_init(&full[s], 1);
             mbar_init(&empty[s], 2);   // one arrival per consumer warpgroup
         }
+        for (int kb = 0; kb < KB; ++kb) mbar_init(&abar[kb], 1);
         mbar_init(xbar, 1);
         fence_barrier_init();
     }
     __syncthreads();
 
-    if (warp == GEMM_CONSUMER_THREADS / 32) {
+    if (warp >= GEMM_CONSUMER_THREADS / 32) {
         // ===================== TMA producer =====================
-        if (elect_one()) {
-            mbar_expect_tx(xbar, (has_proj ? 2 : 1) * Cfg::TILE);
-            for (int kb = 0; kb < KB; ++kb) {
-                tma_load_2d(&maps.x, xbar, sx + kb * (FM_ROWS * 64), kb * 32, row_base);
-                if (has_proj) tma_load_2d(&maps.att, xbar, satt + kb * (FM_ROWS * 64), kb * 32, row_base);
-            }
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(FM_PRODUCER_REGS));
+        if (warp == GEMM_CONSUMER_THREADS / 32 && elect_one()) {
+            bool acts = false;
+            // programmatic dependent launch: everything before this overlapped the previous kernel of the stream (the head,
+            // which writes att); once it returns, that kernel's outputs are complete and visible
+            auto load_acts = [&]() {
+                asm volatile("griddepcontrol.wait;" ::: "memory");
+                if (PROJ)
+                    for (int kb = 0; kb < KB; ++kb) {
+                        mbar_expect_tx(&abar[kb], FM_ROWS * 64);
+                        tma_load_2d(&maps.att, &abar[kb], satt + kb * (FM_ROWS * 64), kb * 32, row_base);
+                    }
+                mbar_expect_tx(xbar, Cfg::TILE);
+                for (int kb = 0; kb < KB; ++kb) tma_load_2d(&maps.x, xbar, sx + kb * (FM_ROWS * 64), kb * 32, row_base);
+                acts = true;
+            };
             int it = 0;
-            auto push = [&](const CUtensorMap* m, int k, int n, int rows) {
+            // one ring stage: nbox boxes of `rows` x 32 columns, box b at column k0 + 32 b, row n0
+            auto push = [&](const CUtensorMap* m, int k0, int n0, int rows, int nbox) {
+                if (it == FM_STAGES) load_acts();   // the first FM_STAGES stages need no free slot, so cannot wait on consumers
                 const int s = it % FM_STAGES;
-                mbar_wait(&empty[s], ((it / FM_STAGES) & 1) ^ 1);
-                mbar_expect_tx(&full[s], rows * 64);
-                tma_load_2d(m, &full[s], ring + s * Cfg::SLOT, k, n);
+                fm_wait(&empty[s], ((it / FM_STAGES) & 1) ^ 1);
+                mbar_expect_tx(&full[s], nbox * rows * 64);
+                for (int b = 0; b < nbox; ++b) tma_load_2d(m, &full[s], ring + s * Cfg::STAGE + b * rows * 64, k0 + 32 * b, n0);
                 ++it;
             };
-            if (has_proj)
-                for (int kb = 0; kb < KB; ++kb) push(&maps.wp, kb * 32, 0, C);
+            if (PROJ)
+                for (int j = 0; j < NP; ++j) push(&maps.wp, 64 * j, 0, C, min(2, KB - 2 * j));
+            push(&maps.w1, 0, 0, 64, KB);
             for (int hc = 0; hc < NH; ++hc) {
-                for (int kb = 0; kb < KB; ++kb) push(&maps.w1, kb * 32, hc * 64, 64);
-                for (int kb = 0; kb < 2; ++kb) push(&maps.w2, hc * 64 + kb * 32, 0, C);
+                if (hc + 1 < NH) push(&maps.w1, 0, (hc + 1) * 64, 64, KB);
+                push(&maps.w2, hc * 64, 0, C, 2);
             }
+            if (!acts) load_acts();
         }
         return;
     }
 
     // ===================== consumers (warps 0..7) =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(FM_CONSUMER_REGS));
     const int wg = tid >> 7, t = tid & 127;
     const int row0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);   // accumulator rows row0 and row0 + 8
     const int cq = 2 * (t & 3);
     const uint32_t x_base = smem_u32(sx) + wg * 64 * 64, att_base = smem_u32(satt) + wg * 64 * 64;
-    int it = 0;
+    // every stage taken is one commit group; the `pending` groups before stage `it` are not released yet.  pending is a
+    // constant at every point of the unrolled code, so the release loops unroll and no branch sits between the wgmmas.
+    int it = 0, pending = 0;
     auto take = [&]() -> uint32_t {
         const int s = it % FM_STAGES;
-        mbar_wait(&full[s], (it / FM_STAGES) & 1);
-        return smem_u32(ring + s * Cfg::SLOT);
+        fm_wait(&full[s], (it / FM_STAGES) & 1);
+        return smem_u32(ring + s * Cfg::STAGE);
     };
-    auto release = [&]() {
-        if (t == 0) mbar_arrive(&empty[it % FM_STAGES]);
+    auto commit = [&]() {
+        wgmma_commit();
         ++it;
+        ++pending;
     };
-    mbar_wait(xbar, 0);
+    // wait until at most n groups are in flight and release the stages of the retired ones
+    auto retire = [&](int n) {
+        wgmma_wait_n(n);
+#pragma unroll
+        for (int k = 0; k < FM_STAGES; ++k)
+            if (k < pending - n && t == 0) mbar_arrive(&empty[(it - pending + k) % FM_STAGES]);
+        pending = min(pending, n);
+    };
 
-    if (has_proj) {
+    if (PROJ) {
         // x1 = x + att Wp^T + bp  (x :453)
         float acc[C / 2];
 #pragma unroll
         for (int j = 0; j < C / 2; ++j) acc[j] = 0.f;
-#pragma unroll 1
-        for (int kb = 0; kb < KB; ++kb) {
-            const uint32_t bb = take(), a = att_base + kb * (FM_ROWS * 64);
+        wgmma_fence_operands(acc);   // the zeros are in the accumulator registers before the first wgmma_fence
+#pragma unroll
+        for (int j = 0; j < NP; ++j) {
+            const uint32_t bb = take();
+#pragma unroll
+            for (int kb = 2 * j; kb < 2 * j + 2 && kb < KB; ++kb) fm_wait(&abar[kb], 0);
             wgmma_fence();
 #pragma unroll
-            for (int s = 0; s < 2; ++s)
+            for (int kb = 2 * j; kb < 2 * j + 2 && kb < KB; ++kb) {
+                const uint32_t a = att_base + kb * (FM_ROWS * 64), b = bb + (kb - 2 * j) * (C * 64);
 #pragma unroll
-                for (int h = 0; h < NHALF; ++h)
-                    wgmma_f16<96>(half96(acc, h), make_kmajor_desc<64>(a + 32 * s), make_kmajor_desc<64>(bb + h * 96 * 64 + 32 * s), 1u);
-            wgmma_commit();
-            wgmma_wait<0>();
-            release();
+                for (int s = 0; s < 2; ++s)
+#pragma unroll
+                    for (int h = 0; h < NHALF; ++h)
+                        wgmma_f16<96>(half96(acc, h), make_kmajor_desc<64>(a + 32 * s), make_kmajor_desc<64>(b + h * 96 * 64 + 32 * s), 1u);
+            }
+            commit();
+            retire(1);
         }
+        retire(0);
         wgmma_fence_operands(acc);
+        fm_wait(xbar, 0);
 #pragma unroll
         for (int j = 0; j < C / 8; ++j) {
             const int col = 8 * j + cq;
@@ -135,53 +205,63 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
         }
         fence_async_smem();   // x1 (generic-proxy writes) -> A operand of this warpgroup's fc1 wgmma
         asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+    } else {
+        fm_wait(xbar, 0);
     }
 
     float oacc[C / 2];
 #pragma unroll
     for (int j = 0; j < C / 2; ++j) oacc[j] = 0.f;
-#pragma unroll 1
-    for (int hc = 0; hc < NH; ++hc) {
-        // hidden chunk: gelu(x1 W1[64 hc : 64 hc + 64]^T + b1) (:444), rounded to fp16 as the reference stores it
-        float hacc[32];
+    wgmma_fence_operands(oacc);
+    float hacc[2][32];
+    uint32_t af[4][4];   // k16 block kk of a chunk: {row g | g+8} x {cols 2t, 2t+8} as in the m16n8k16 A fragment
+    // hidden chunk hc before GELU: x1 W1[64 hc : 64 hc + 64]^T, one stage of C/32 K-blocks
+    auto fc1 = [&](float (&h)[32]) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) hacc[j] = 0.f;
-#pragma unroll 1
+        for (int j = 0; j < 32; ++j) h[j] = 0.f;
+        wgmma_fence_operands(h);
+        const uint32_t bb = take();
+        wgmma_fence();
+#pragma unroll
         for (int kb = 0; kb < KB; ++kb) {
-            const uint32_t bb = take(), a = x_base + kb * (FM_ROWS * 64);
-            wgmma_fence();
-            wgmma_f16<64>(hacc, make_kmajor_desc<64>(a), make_kmajor_desc<64>(bb), 1u);
-            wgmma_f16<64>(hacc, make_kmajor_desc<64>(a + 32), make_kmajor_desc<64>(bb + 32), 1u);
-            wgmma_commit();
-            wgmma_wait<0>();
-            release();
+            const uint32_t a = x_base + kb * (FM_ROWS * 64), b = bb + kb * (64 * 64);
+            wgmma_f16<64>(h, make_kmajor_desc<64>(a), make_kmajor_desc<64>(b), 1u);
+            wgmma_f16<64>(h, make_kmajor_desc<64>(a + 32), make_kmajor_desc<64>(b + 32), 1u);
         }
-        wgmma_fence_operands(hacc);
-        uint32_t af[4][4];   // k16 block kk of the chunk: {row g | g+8} x {cols 2t, 2t+8} as in the m16n8k16 A fragment
+        commit();
+    };
+    fc1(hacc[0]);
+#pragma unroll
+    for (int hc = 0; hc < NH; ++hc) {
+        const int buf = hc & 1;
+        if (hc + 1 < NH) fc1(hacc[buf ^ 1]);
+        // fc1(hc) and fc2(hc - 1), the last reader of af, retired; fc1(hc + 1), committed after them, stays in flight during
+        // the GELU
+        retire(hc + 1 < NH ? 1 : 0);
+        wgmma_fence_operands(hacc[buf]);
+        // gelu(. + b1) (:444), rounded to fp16 as the reference stores it
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const int j = 2 * kk + (q >> 1), i = q & 1;
                 const float2 bq = __ldg(reinterpret_cast<const float2*>(b1 + 64 * hc + 8 * j + cq));
-                const __half2 h = __floats2half2_rn(gelu_erf(hacc[4 * j + 2 * i] + bq.x), gelu_erf(hacc[4 * j + 2 * i + 1] + bq.y));
+                const __half2 h = __floats2half2_rn(gelu_erf(hacc[buf][4 * j + 2 * i] + bq.x), gelu_erf(hacc[buf][4 * j + 2 * i + 1] + bq.y));
                 af[kk][q] = *reinterpret_cast<const uint32_t*>(&h);
             }
         // out += hidden_chunk W2[:, 64 hc : 64 hc + 64]^T
-#pragma unroll 1
-        for (int kb = 0; kb < 2; ++kb) {
-            const uint32_t bb = take();
-            wgmma_fence();
+        const uint32_t bb = take();
+        wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < 2; ++kb)
 #pragma unroll
             for (int s = 0; s < 2; ++s)
 #pragma unroll
                 for (int h = 0; h < NHALF; ++h)
-                    wgmma_f16_rs96(half96(oacc, h), af[2 * kb + s], make_kmajor_desc<64>(bb + h * 96 * 64 + 32 * s), 1u);
-            wgmma_commit();
-            wgmma_wait<0>();
-            release();
-        }
+                    wgmma_f16_rs96(half96(oacc, h), af[2 * kb + s], make_kmajor_desc<64>(bb + kb * (C * 64) + h * 96 * 64 + 32 * s), 1u);
+        commit();
     }
+    retire(0);
     wgmma_fence_operands(oacc);
     // x <- x1 + mlp(x1) (:454), in place over the x1 tile, then one TMA store per 32-column box
 #pragma unroll
@@ -211,6 +291,22 @@ static int map2d(CUtensorMap* m, const void* base, int cols, long long rows, int
     return encode(m, base, 2, dims, strides, box, 64);
 }
 
+template <int C, bool PROJ>
+static int launch_mlp(cudaStream_t st, unsigned grid, const FmMaps& maps, const float* bp, const float* b1, const float* b2) {
+    if (ensure_dyn_smem((const void*)swin_mlp_fused_kernel<C, PROJ>, FmCfg<C>::SMEM)) return 1;
+    // programmatic dependent launch (as gemm.cu): the producer's set-up and first weight stages overlap the head's last wave
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(FM_THREADS); cfg.dynamicSmemBytes = FmCfg<C>::SMEM;
+    cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    NB_CUDA(cudaLaunchKernelEx(&cfg, swin_mlp_fused_kernel<C, PROJ>, maps, bp, b1, b2));
+    NB_LAUNCHED();
+    return 0;
+}
+
 int swin_mlp_fused(cudaStream_t st, __half* x, const __half* att, long long T, int C, const __half* wp, const float* bp,
                    const __half* w1, const float* b1, const __half* w2, const float* b2) {
     NB_CHECK(x && w1 && b1 && w2 && b2 && (!att || (wp && bp)), "null pointer");
@@ -224,15 +320,8 @@ int swin_mlp_fused(cudaStream_t st, __half* x, const __half* att, long long T, i
     const double Td = (double)T;
     ProfScope ps(st, PC_FUSED_MLP, Td * C * C * 2 * ((att ? 1 : 0) + 4), Td * C * 2 * (att ? 2 : 1), Td * C * 2);
     const unsigned grid = (unsigned)((T + FM_ROWS - 1) / FM_ROWS);
-    if (C == 96) {
-        if (ensure_dyn_smem((const void*)swin_mlp_fused_kernel<96>, FmCfg<96>::SMEM)) return 1;
-        swin_mlp_fused_kernel<96><<<grid, FM_THREADS, FmCfg<96>::SMEM, st>>>(maps, bp, b1, b2, att ? 1 : 0);
-    } else {
-        if (ensure_dyn_smem((const void*)swin_mlp_fused_kernel<192>, FmCfg<192>::SMEM)) return 1;
-        swin_mlp_fused_kernel<192><<<grid, FM_THREADS, FmCfg<192>::SMEM, st>>>(maps, bp, b1, b2, att ? 1 : 0);
-    }
-    NB_LAUNCHED();
-    return 0;
+    if (C == 96) return att ? launch_mlp<96, true>(st, grid, maps, bp, b1, b2) : launch_mlp<96, false>(st, grid, maps, bp, b1, b2);
+    return att ? launch_mlp<192, true>(st, grid, maps, bp, b1, b2) : launch_mlp<192, false>(st, grid, maps, bp, b1, b2);
 }
 
 }  // namespace nb200
