@@ -160,9 +160,23 @@ int nb200_row_flow_delta(nb200_model* m, const float* x, int B, int h, int w, fl
 
 /* sbs.mlbw in delta_output mode (iw3/models/mlbw.py:96-127,237-245): x [B][3][h][w] fp32 (depth, divergence feature,
  * convergence feature) -> delta [B][L][h][w] (x component of each flow layer) and layer_weight [B][L][h][w] (softmax over
- * the L layers); L = nb200_mlbw_num_layers (2 or 4, read off the state_dict).  hole_mask models are not supported. */
+ * the L layers); L = nb200_mlbw_num_layers (2 or 4, read off the state_dict).  A hole_mask model (sbs.mask_mlbw_l2,
+ * nb200_mlbw_has_hole_mask = 1) fails here: it runs through nb200_mlbw_delta_hole. */
 int nb200_mlbw_delta(nb200_model* m, const float* x, int B, int h, int w, float* delta, float* layer_weight, void* stream);
 int nb200_mlbw_num_layers(const nb200_model* m);
+/* 1 for a hole_mask model (lv1_out.1.bias with 2 * 2 + 1 = 5 elements, iw3/models/mlbw.py:70-74), else 0. */
+int nb200_mlbw_has_hole_mask(const nb200_model* m);
+/* _forward_delta_only of a hole_mask model (mlbw.py:232-240): delta and layer_weight as nb200_mlbw_delta, plus
+ * hole_logits [B][1][h][w] fp32 (the fp16 conv output of channel 2L, .float()). */
+int nb200_mlbw_delta_hole(nb200_model* m, const float* x, int B, int h, int w, float* delta, float* layer_weight,
+                          float* hole_logits, void* stream);
+/* postprocess_hole_mask(logits, (H, W), threshold) (iw3/backward_warp.py:382-393) up to the threshold: closing(logits, n_iter=1)
+ * (iw3/dilation.py:41-64), the align_corners=True bilinear resize to H x W when the size differs, sigmoid(.) > threshold.
+ * logits [B][1][h][w] -> out [B][1][H][W] binary fp32.  mirror = 1 gives the mask forward_left computes on the flipped logits
+ * (iw3/mlbw_inpaint.py:28-34), flipped back.  threshold = NaN writes the resized closed logits instead of the mask (a view
+ * of the first two steps, for tests).  The dilate_inner / dilate_outer steps are nb200_inpaint_mask(binarize=1, closing=0,
+ * outer, inner, base_width = w, mirror). */
+int nb200_hole_mask(const float* logits, int B, int h, int w, int H, int W, float threshold, int mirror, float* out, void* stream);
 
 /* iw3 forward_inpaint, image mode (iw3/forward_inpaint.py:18-40,69-103).  All tensors planar fp32 in image coordinates.
  * nb200_inpaint_mask: the mask chain of forward_right / forward_left (:18-40): binarize => mask > 0; closing => mask_closing

@@ -59,6 +59,9 @@ SIGNATURES = {
     "nb200_depth_aa": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_mlbw_delta": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "nb200_mlbw_num_layers": (c_int, [c_void_p]),
+    "nb200_mlbw_has_hole_mask": (c_int, [c_void_p]),
+    "nb200_mlbw_delta_hole": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_hole_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p]),
     "nb200_row_flow_delta": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_inpaint_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_inpaint_blur": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),

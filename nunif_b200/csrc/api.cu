@@ -21,7 +21,7 @@ static std::vector<ProfRec> g_prof_recs;
 static std::vector<cudaEvent_t> g_prof_pool;
 static const char* kCatNames[PC_COUNT] = {"gemm", "window_attention", "stem_conv", "to_image", "tile_unfold", "tile_blend",
                                           "se_block", "tail_conv", "forward_warp", "backward_warp", "dilate_edge",
-                                          "minmax_map", "other", "fused_mlp", "fused_attn"};
+                                          "minmax_map", "other", "fused_mlp", "fused_attn", "hole_mask"};
 
 static cudaEvent_t prof_event() {
     if (!g_prof_pool.empty()) { cudaEvent_t e = g_prof_pool.back(); g_prof_pool.pop_back(); return e; }

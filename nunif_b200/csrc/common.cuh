@@ -42,7 +42,7 @@ inline int fail(const std::string& msg) {
 
 // ---- optional in-library kernel timing (bench.py roofline): CUDA events around each launch
 enum ProfCat : int { PC_GEMM = 0, PC_ATTN, PC_STEM, PC_TOIMG, PC_UNFOLD, PC_BLEND, PC_SE, PC_TAIL, PC_WARP_FW, PC_WARP_BW,
-                     PC_DILATE, PC_MINMAX, PC_OTHER, PC_FUSED_MLP, PC_FUSED_ATTN, PC_COUNT };
+                     PC_DILATE, PC_MINMAX, PC_OTHER, PC_FUSED_MLP, PC_FUSED_ATTN, PC_HOLE_MASK, PC_COUNT };
 extern std::atomic<int> g_prof_enabled;
 void prof_begin(cudaStream_t st, int cat, double work, double rbytes, double wbytes);
 void prof_end(cudaStream_t st);

@@ -777,10 +777,30 @@ extern "C" int nb200_depth_anything_forward(nb200_model* m, const float* x, int 
 extern "C" int nb200_mlbw_delta(nb200_model* m, const float* x, int B, int h, int w, float* delta, float* layer_weight, void* stream) {
     NB_CHECK(m && x && delta && layer_weight, "null pointer");
     NB_CHECK(m->kind == NB200_MODEL_MLBW && m->ml, "model is not sbs.mlbw");
+    NB_CHECK(!m->ml->hole, "this sbs.mlbw has a hole_mask head (sbs.mask_mlbw_l2): use nb200_mlbw_delta_hole");
     NB_CHECK(B > 0 && h > 0 && w > 0, "empty input");
-    return mlbw_forward(m, (cudaStream_t)stream, x, B, h, w, delta, layer_weight);
+    return mlbw_forward(m, (cudaStream_t)stream, x, B, h, w, delta, layer_weight, nullptr);
 }
 extern "C" int nb200_mlbw_num_layers(const nb200_model* m) { return (m && m->kind == NB200_MODEL_MLBW && m->ml) ? m->ml->L : 0; }
+extern "C" int nb200_mlbw_has_hole_mask(const nb200_model* m) { return (m && m->kind == NB200_MODEL_MLBW && m->ml && m->ml->hole) ? 1 : 0; }
+
+// MLBW._forward_delta_only of a hole_mask model (mlbw.py:232-240): delta, layer_weight and the hole logits
+extern "C" int nb200_mlbw_delta_hole(nb200_model* m, const float* x, int B, int h, int w, float* delta, float* layer_weight,
+                                     float* hole_logits, void* stream) {
+    NB_CHECK(m && x && delta && layer_weight && hole_logits, "null pointer");
+    NB_CHECK(m->kind == NB200_MODEL_MLBW && m->ml, "model is not sbs.mlbw");
+    NB_CHECK(m->ml->hole, "this sbs.mlbw has no hole_mask head: use nb200_mlbw_delta");
+    NB_CHECK(B > 0 && h > 0 && w > 0, "empty input");
+    return mlbw_forward(m, (cudaStream_t)stream, x, B, h, w, delta, layer_weight, hole_logits);
+}
+
+// postprocess_hole_mask (iw3/backward_warp.py:382-393), steps 1-3: closing, align-corners resize, sigmoid > threshold
+extern "C" int nb200_hole_mask(const float* logits, int B, int h, int w, int H, int W, float threshold, int mirror, float* out,
+                               void* stream) {
+    NB_CHECK(logits && out, "null pointer");
+    NB_CHECK(B > 0 && h > 0 && w > 0 && H > 0 && W > 0, "empty mask");
+    return hole_mask((cudaStream_t)stream, logits, B, h, w, H, W, threshold, mirror ? 1 : 0, out);
+}
 
 // DepthAA.forward / DepthAA.infer (iw3/models/depth_aa.py:46-87)
 extern "C" int nb200_depth_aa(nb200_model* m, const float* x, int B, int H, int W, int mode, float* out, void* stream) {

@@ -8,6 +8,7 @@ preserve_screen_border (:33-47) run the same kernels once per step.
 import ctypes
 import torch
 from .. import _lib
+from . import _common
 
 KIND_ROW_FLOW_V3 = 7     # NB200_MODEL_ROW_FLOW_V3
 KIND_MLBW = 11           # NB200_MODEL_MLBW
@@ -26,12 +27,12 @@ def _create(kind, state_dict, device):
 
 
 class MLBW:
-    """Packed `sbs.mlbw` (iw3/models/mlbw.py; methods mlbw_l2 / mlbw_l4 and their `s` variants, hole_mask=False) in delta_output
-    mode: ``model(x)`` with x = B,3,h,w returns ``(delta B,L,h,w, layer_weight B,L,h,w)`` (:237-245 without the y interleave)."""
+    """Packed `sbs.mlbw` (iw3/models/mlbw.py; methods mlbw_l2 / mlbw_l4 and their `s` variants, and mask_mlbw_l2 with
+    hole_mask=True) in delta_output mode: ``model(x)`` with x = B,3,h,w returns ``(delta B,L,h,w, layer_weight B,L,h,w)``, and for
+    a hole_mask model also the hole logits B,1,h,w (_forward_delta_only, :232-240, without the y interleave)."""
     name = "sbs.mlbw"
     symmetric = False
     delta_output = True
-    hole_mask = False
 
     def __init__(self, state_dict, device="cuda:0"):
         self.device = torch.device(device)
@@ -39,6 +40,7 @@ class MLBW:
             raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
         self._h = _create(KIND_MLBW, state_dict, self.device)
         self.num_layers = int(_lib.lib().nb200_mlbw_num_layers(self._h))
+        self.hole_mask = bool(_lib.lib().nb200_mlbw_has_hole_mask(self._h))
 
     def __del__(self):
         try:
@@ -55,6 +57,12 @@ class MLBW:
         xf = x.float().contiguous()
         delta = torch.empty((B, self.num_layers, h, w), dtype=torch.float32, device=x.device)
         lw = torch.empty_like(delta)
+        if self.hole_mask:
+            logits = torch.empty((B, 1, h, w), dtype=torch.float32, device=x.device)
+            with torch.cuda.device(x.device):
+                _lib.check(_lib.lib().nb200_mlbw_delta_hole(self._h, _lib.ptr(xf), B, h, w, _lib.ptr(delta), _lib.ptr(lw), _lib.ptr(logits),
+                                                            _lib.stream_ptr(x.device)))
+            return delta, lw, logits
         with torch.cuda.device(x.device):
             _lib.check(_lib.lib().nb200_mlbw_delta(self._h, _lib.ptr(xf), B, h, w, _lib.ptr(delta), _lib.ptr(lw), _lib.stream_ptr(x.device)))
         return delta, lw
@@ -155,9 +163,38 @@ def apply_divergence_nn_delta(model, c, depth, divergence, convergence, steps, s
     return torch.flip(z, (3,)) if shift > 0 else z
 
 
-def apply_divergence_nn_delta_weight(model, c, depth, divergence, convergence, steps, shift, preserve_screen_border=False, enable_amp=True):
-    """iw3/backward_warp.py:262-329 for sbs.mlbw without a hole mask: every flow layer warps the frame, the warps are blended with
-    the (antialias-bilinear resized) layer weights.  ``steps`` is ignored by the reference for this model."""
+MASK_MLBW_THRESHOLD = 0.15   # iw3/mlbw_inpaint.py:18, and the hole fill of backward_warp.py:334-338
+
+
+def postprocess_hole_mask(mask_logits, target_size, threshold, inner_dilation=0, outer_dilation=0, mirror=False):
+    """iw3/backward_warp.py:382-393: closing of the hole logits (3x3, one iteration), the align-corners bilinear resize to
+    target_size, sigmoid > threshold, dilate_inner and dilate_outer with base_width = the logits' width -> a B,1,H,W float mask of
+    0 / 1.  ``mirror=True`` gives what forward_left computes on the flipped logits (iw3/mlbw_inpaint.py:28-34), flipped back.
+
+    Two launches: nb200_hole_mask (closing, resize, threshold), then the row-run dilation of nb200_inpaint_mask.  The reference
+    dilates inner before outer; OR-shifts to the left and to the right commute (an OR over [x - outer, x + inner] of the row, zero
+    outside it, either way), so the one-pass run dilation gives the same mask."""
+    from .forward_inpaint import inpaint_mask
+    mask_logits = _common.prep(mask_logits, "mask_logits")
+    assert mask_logits.ndim == 4 and mask_logits.shape[1] == 1
+    B, _, h, w = mask_logits.shape
+    H, W = (int(v) for v in target_size)
+    mask = torch.empty((B, 1, H, W), dtype=torch.float32, device=mask_logits.device)
+    with torch.cuda.device(mask_logits.device):
+        _lib.check(_lib.lib().nb200_hole_mask(_lib.ptr(mask_logits), B, h, w, H, W, float(threshold), int(bool(mirror)), _lib.ptr(mask),
+                                              _lib.stream_ptr(mask_logits.device)))
+    if inner_dilation <= 0 and outer_dilation <= 0:
+        return mask
+    return inpaint_mask(mask, inner_dilation=inner_dilation, outer_dilation=outer_dilation, base_width=w, mirror=mirror,
+                        binarize=True, closing=False)
+
+
+def apply_divergence_nn_delta_weight(model, c, depth, divergence, convergence, steps, shift, preserve_screen_border=False, enable_amp=True,
+                                     return_mask=False):
+    """iw3/backward_warp.py:262-341 for sbs.mlbw: every flow layer warps the frame, the warps are blended with the
+    (antialias-bilinear resized) layer weights.  ``steps`` is ignored by the reference for this model.  A hole_mask model
+    (mask_mlbw_l2) also predicts hole logits at depth resolution: ``return_mask=True`` returns ``(z, logits)`` (flipped back with
+    the frame for shift > 0), otherwise the holes are blacked out, z * (1 - postprocess_hole_mask(logits, (H, W), 0.15))."""
     if not enable_amp:
         raise NotImplementedError("nunif_b200 implements the reference's CUDA autocast (fp16) forward only")
     _lib.require_cuda(c, "c")
@@ -166,7 +203,9 @@ def apply_divergence_nn_delta_weight(model, c, depth, divergence, convergence, s
     if shift > 0:
         c, depth = torch.flip(c, (3,)), torch.flip(depth, (3,))
     B, _, H, W = depth.shape
-    delta, lw = model(make_input(depth, divergence, convergence, preserve_screen_border))
+    out = model(make_input(depth, divergence, convergence, preserve_screen_border))
+    delta, lw = out[:2]
+    logits = out[2] if getattr(model, "hole_mask", False) else None
     if c.shape[2:] != lw.shape[2:]:                                                            # :296-298
         L = lw.shape[1]
         lw_full = torch.empty((B, L, c.shape[2], c.shape[3]), dtype=torch.float32, device=c.device)
@@ -179,7 +218,15 @@ def apply_divergence_nn_delta_weight(model, c, depth, divergence, convergence, s
     for i in range(model.num_layers):                                                          # :304-309
         z += _warp_delta(c, delta[:, i:i + 1].contiguous(), delta_scale) * lw[:, i:i + 1]
     z = z.clamp_(0, 1)
-    return torch.flip(z, (3,)) if shift > 0 else z
+    if shift > 0:
+        z = torch.flip(z, (3,))
+        if logits is not None:
+            logits = torch.flip(logits, (3,))
+    if return_mask:
+        return z, logits
+    if logits is not None:                                                                     # :332-339
+        z = z * (1 - postprocess_hole_mask(logits, c.shape[-2:], MASK_MLBW_THRESHOLD))
+    return z
 
 
 def apply_divergence_nn(model, c, depth, divergence, convergence, steps, shift, preserve_screen_border=False, enable_amp=True):

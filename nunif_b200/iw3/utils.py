@@ -50,7 +50,14 @@ def apply_divergence(depth, im, args, side_model, reset_pts=None):
                                 inner_dilation=_arg(args, "mask_inner_dilation", 0), outer_dilation=_arg(args, "mask_outer_dilation", 0),
                                 max_width=_arg(args, "inpaint_max_width", None), enable_amp=True)
     elif method == "mlbw_l2_inpaint":
-        raise NotImplementedError("method mlbw_l2_inpaint (mask_mlbw_l2 + video inpainting) is not implemented by the H100 engine")
+        # the same per-frame side_model.infer as forward_inpaint (:333-367), with preserve_screen_border passed through
+        if side_model is None:
+            raise NotImplementedError("method mlbw_l2_inpaint needs side_model: the H100 engine does not build the reference's "
+                                      "MLBWInpaint implicitly (pass nunif_b200.iw3.MLBWInpaint)")
+        eyes = side_model.infer(im, depth, args.divergence, convergence, preserve_screen_border=_arg(args, "preserve_screen_border", False),
+                                synthetic_view=args.synthetic_view, inner_dilation=_arg(args, "mask_inner_dilation", 0),
+                                outer_dilation=_arg(args, "mask_outer_dilation", 0), max_width=_arg(args, "inpaint_max_width", None),
+                                enable_amp=True)
     else:
         # the learned warps (row_flow*, mlbw*): apply_divergence_nn_LR with args.side_model (:363-385)
         stereo_width = _arg(args, "stereo_width", None)

@@ -398,6 +398,23 @@ def mlbw_state_dict(seed=0, num_layers=2):
     return sd
 
 
+MASK_MLBW_HOLE_BIAS = -2.1
+
+
+def mask_mlbw_state_dict(seed=0):
+    """Seeded weights of `sbs.mask_mlbw_l2` (MLBW(num_layers=2, base_dim=32, hole_mask=True), iw3/models/mlbw.py:70-74): the
+    weights of mlbw_state_dict(seed, 2) plus a fifth lv1_out output, the hole logit, drawn from a generator of its own so that
+    mlbw_state_dict's streams stay as they are.  Its bias puts a few percent of the pixels of a typical frame over the 0.15
+    threshold of iw3/mlbw_inpaint.py:18 (oracle/gen_golden_mask_mlbw.py checks 3-30 % on the golden inputs)."""
+    sd = mlbw_state_dict(seed, 2)
+    g = torch.Generator().manual_seed(41_000 + seed)
+    c1 = 8
+    w = torch.randn(1, c1, 1, 9, generator=g) * (1.5 / (9 * c1) ** 0.5)
+    sd["lv1_out.1.weight"] = torch.cat([sd["lv1_out.1.weight"], w])
+    sd["lv1_out.1.bias"] = torch.cat([sd["lv1_out.1.bias"], torch.tensor([MASK_MLBW_HOLE_BIAS])])
+    return sd
+
+
 ZOED_N = dict(dim=1024, depth=24, heads=16, hooks=(5, 11, 17, 23), oc=(256, 512, 1024, 1024), feat=256, old_grid=24)
 ZOED_MINI = dict(dim=256, depth=4, heads=4, hooks=(0, 1, 2, 3), oc=(64, 128, 256, 256), feat=128, old_grid=6)
 
