@@ -94,7 +94,8 @@ enum {
     NB200_MODEL_ZOEDEPTH_N = 12,
     NB200_MODEL_UPCONV_7 = 13,             /* waifu2x.upconv_7 (waifu2x/models/upconv_7.py:6-38): scale 2, offset 14 */
     NB200_MODEL_VGG_7 = 14,                /* waifu2x.vgg_7    (waifu2x/models/vgg_7.py:6-36): scale 1, offset 7 */
-    NB200_MODEL_LIGHT_INPAINT_V1 = 15      /* inpaint.light_inpaint_v1, iw3's image-mode hole inpainting (iw3/models/light_inpaint_v1.py) */
+    NB200_MODEL_LIGHT_INPAINT_V1 = 15,     /* inpaint.light_inpaint_v1, iw3's image-mode hole inpainting (iw3/models/light_inpaint_v1.py) */
+    NB200_MODEL_ROW_FLOW_V2 = 16           /* sbs.row_flow_v2, the learned row-flow warp of `--method row_flow_v2` (iw3/models/row_flow_v2.py) */
 };
 
 /* Create a model from named fp32 host tensors using the reference's state_dict
@@ -157,6 +158,10 @@ int nb200_depth_aa(nb200_model* m, const float* x, int B, int H, int W, int mode
  * divergence feature, convergence feature (make_input_tensor, iw3/backward_warp.py:18-63) -> delta [B][1][h][w]
  * fp32 (the x component; the y component is zero). */
 int nb200_row_flow_delta(nb200_model* m, const float* x, int B, int h, int w, float* delta, void* stream);
+/* sbs.row_flow_v2 in delta_output mode (iw3/models/row_flow_v2.py:43-47,80-86): same x as nb200_row_flow_delta -> delta
+ * [B][1][h][w] fp32 holding the fp16 values of the reference's autocast output (the x component).  Replaces the pre_pad,
+ * the convolutions and the crop of _forward_delta_only with one kernel. */
+int nb200_row_flow_v2_delta(nb200_model* m, const float* x, int B, int h, int w, float* delta, void* stream);
 
 /* sbs.mlbw in delta_output mode (iw3/models/mlbw.py:96-127,237-245): x [B][3][h][w] fp32 (depth, divergence feature,
  * convergence feature) -> delta [B][L][h][w] (x component of each flow layer) and layer_weight [B][L][h][w] (softmax over
@@ -200,6 +205,16 @@ int nb200_light_inpaint(nb200_model* m, const float* x, const float* mask, int B
  * c [B][3][H][W], delta [B][1][h][w] fp32 -> out [B][3][H][W] = clamp(grid_sample(c, grid + delta*delta_scale)). */
 int nb200_backward_warp_delta(const float* c, const float* delta, int B, int H, int W, int h, int w,
                               double delta_scale, float* out, void* stream);
+/* The same warp for an fp16 delta (sbs.row_flow_v2, whose _forward_delta_only returns the autocast fp16 tensor,
+ * row_flow_v2.py:80-86): `delta * delta_scale` is then an fp16 tensor op, i.e. delta_scale is rounded to fp16 and so is the
+ * product, and only `grid +` runs in fp32 (backward_warp.py:68).  delta holds fp16 values. */
+int nb200_backward_warp_delta_f16(const float* c, const float* delta, int B, int H, int W, int h, int w,
+                                  double delta_scale, float* out, void* stream);
+/* apply_divergence_nn_symmetric's warps (iw3/backward_warp.py:344-379, sbs.row_flow_v3 with symmetric = True) in one launch:
+ * left = backward_warp(c, grid, delta, delta_scale), right = backward_warp(c, grid, -delta, delta_scale).  warp_left /
+ * warp_right = 0 writes a copy of c for that eye instead (synthetic_view "right" / "left"). */
+int nb200_backward_warp_delta_sym(const float* c, const float* delta, int B, int H, int W, int h, int w, double delta_scale,
+                                  int warp_left, int warp_right, float* left, float* right, void* stream);
 
 /* AlphaBorderPadding.forward (nunif/utils/alpha.py:32-57): rgb [3][H][W], alpha [1][H][W] fp32 ->
  * out [3][H][W]: transparent pixels are filled from their opaque neighbours, `offset` rounds

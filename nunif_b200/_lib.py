@@ -63,11 +63,15 @@ SIGNATURES = {
     "nb200_mlbw_delta_hole": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "nb200_hole_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p]),
     "nb200_row_flow_delta": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "nb200_row_flow_v2_delta": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_inpaint_mask": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_inpaint_blur": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_resize_bilinear_aa": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_light_inpaint": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_backward_warp_delta": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_void_p, c_void_p]),
+    "nb200_backward_warp_delta_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_void_p, c_void_p]),
+    "nb200_backward_warp_delta_sym": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_int, c_int, c_void_p,
+                                              c_void_p, c_void_p]),
     "nb200_alpha_border_padding_workspace": (c_size_t, [c_int, c_int]),
     "nb200_alpha_border_padding": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "nb200_tta_transform": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

@@ -225,6 +225,7 @@ struct AaW;     // depth_aa_model.inl
 struct MlW;     // mlbw_model.inl
 struct ZoeW;    // zoe_model.inl
 struct InpW;    // inpaint_model.inl
+struct Rf2W;    // rowflow_v2_model.inl
 
 }  // namespace nb200
 
@@ -244,6 +245,7 @@ struct nb200_model {
     std::shared_ptr<MlW> ml;
     std::shared_ptr<ZoeW> zoe;
     std::shared_ptr<InpW> inp;
+    std::shared_ptr<Rf2W> rf2;
     uint8_t* ws = nullptr;
     size_t ws_bytes = 0;
     cudaStream_t copy_stream = nullptr;   // D2H side stream of nb200_tiled_render_host
@@ -486,6 +488,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 #include "depth_model.inl"
 #include "wa_block.inl"
 #include "rowflow_model.inl"
+#include "rowflow_v2_model.inl"
 #include "depth_aa_model.inl"
 #include "mlbw_model.inl"
 #include "zoe_model.inl"
@@ -497,7 +500,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* names, const float* const* data,
                                   const int64_t* numel, int no_clip, nb200_model** out) {
     NB_CHECK(out && names && data && numel, "null pointer");
-    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_LIGHT_INPAINT_V1, "unknown model kind");
+    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_ROW_FLOW_V2, "unknown model kind");
     int dev = 0;
     NB_CUDA(cudaGetDevice(&dev));
     if (nb200_check_device(dev)) return 1;
@@ -532,6 +535,7 @@ extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* na
         case NB200_MODEL_UPCONV_7: m->lg = pack_legacy(pk, true); m->scale = 2; m->offset = 14; m->blend = 0; break;  // upconv_7.py:11
         case NB200_MODEL_VGG_7: m->lg = pack_legacy(pk, false); m->scale = 1; m->offset = 7; m->blend = 0; break;     // vgg_7.py:11
         case NB200_MODEL_LIGHT_INPAINT_V1: m->inp = pack_light_inpaint(pk); m->scale = 1; m->offset = 16; m->blend = 8; break;  // light_inpaint_v1.py:56
+        case NB200_MODEL_ROW_FLOW_V2: m->rf2 = pack_row_flow_v2(pk); m->scale = 1; m->offset = 28; m->blend = 4; break;   // row_flow_v2.py:14
     }
     if (pk.err.empty())
         for (auto& kv : pk.src)
@@ -816,6 +820,14 @@ extern "C" int nb200_row_flow_delta(nb200_model* m, const float* x, int B, int h
     NB_CHECK(m->kind == NB200_MODEL_ROW_FLOW_V3 && m->rf, "model is not sbs.row_flow_v3");
     NB_CHECK(B > 0 && h > 0 && w > 0, "bad shape");
     return row_flow_forward(m, (cudaStream_t)stream, x, B, h, w, delta);
+}
+
+// RowFlowV2.forward with delta_output=True (iw3/models/row_flow_v2.py:80-86) - the x component of the returned delta
+extern "C" int nb200_row_flow_v2_delta(nb200_model* m, const float* x, int B, int h, int w, float* delta, void* stream) {
+    NB_CHECK(m && x && delta, "null pointer");
+    NB_CHECK(m->kind == NB200_MODEL_ROW_FLOW_V2 && m->rf2, "model is not sbs.row_flow_v2");
+    NB_CHECK(B > 0 && h > 0 && w > 0, "bad shape");
+    return rf2_forward((cudaStream_t)stream, m->blob + m->rf2->params, x, B, h, w, delta);
 }
 
 // iw3/dilation.py:67-98: n = max(round(W / base_width * n_iter), 1) (Python's round: half to even), 0 when n_iter <= 0

@@ -197,7 +197,9 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
 struct __align__(16) GridTab { float l0, r0, l1, r1; };
 constexpr int COMPOSE_RIGHT_ONLY = 3;   // internal: only the "+shift" view, written to p.left (nb200_backward_warp_delta)
 
-template <int COMPOSE>
+// F16_PRODUCT: delta * delta_scale is rounded to fp16 (an fp16 delta, nb200_backward_warp_delta_f16; p.delta_scale is then
+// fp16-valued as well).
+template <int COMPOSE, bool F16_PRODUCT = false>
 __global__ void __launch_bounds__(256) backward_warp_row_kernel(BwParams p, int S, int vec_ok) {
     extern __shared__ __align__(16) unsigned char bw_smem[];
     GridTab* gt = reinterpret_cast<GridTab*>(bw_smem);          // [w + 1]
@@ -235,7 +237,11 @@ __global__ void __launch_bounds__(256) backward_warp_row_kernel(BwParams p, int 
         const float lx = linspace_m1_1(jj, p.w, p.step_x);
         const float is0 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i0 * p.w + jj), p.shift), p.shift_conv);
         const float is1 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + jj), p.shift), p.shift_conv);
-        const float d0 = __fmul_rn(is0, p.delta_scale), d1 = __fmul_rn(is1, p.delta_scale);
+        float d0 = __fmul_rn(is0, p.delta_scale), d1 = __fmul_rn(is1, p.delta_scale);
+        if (F16_PRODUCT) {
+            d0 = __half2float(__float2half_rn(d0));
+            d1 = __half2float(__float2half_rn(d1));
+        }
         GridTab t;
         t.l0 = __fsub_rn(lx, d0); t.r0 = __fadd_rn(lx, d0);
         t.l1 = __fsub_rn(lx, d1); t.r1 = __fadd_rn(lx, d1);
@@ -323,10 +329,10 @@ __global__ void __launch_bounds__(256) backward_warp_row_kernel(BwParams p, int 
 
 extern int g_tune[16];  // gemm.cu; [3] != 0 forces the gather-from-global kernel (tests)
 
-template <int COMPOSE>
+template <int COMPOSE, bool F16_PRODUCT = false>
 static int launch_bw_row(const BwParams& p, size_t smem, int S, int vec_ok, cudaStream_t st) {
-    if (ensure_dyn_smem((const void*)backward_warp_row_kernel<COMPOSE>, smem)) return 1;
-    backward_warp_row_kernel<COMPOSE><<<dim3(p.H, p.B), 256, smem, st>>>(p, S, vec_ok);
+    if (ensure_dyn_smem((const void*)backward_warp_row_kernel<COMPOSE, F16_PRODUCT>, smem)) return 1;
+    backward_warp_row_kernel<COMPOSE, F16_PRODUCT><<<dim3(p.H, p.B), 256, smem, st>>>(p, S, vec_ok);
     return 0;
 }
 
@@ -418,26 +424,66 @@ extern "C" int nb200_anaglyph_dubois(const float* l, const float* r, int B, int 
 // apply_divergence_nn_delta :213-226): grid x = mesh_x + delta * delta_scale at the delta resolution, bilinearly resized to
 // the image (align_corners=True), grid_sample(bilinear, border) and clamp.  Same kernel as the depth-driven warp with
 // index_shift := delta (shift = 1, convergence term = 0) and only the "+" view evaluated.
-extern "C" int nb200_backward_warp_delta(const float* c, const float* delta, int B, int H, int W, int h, int w, double delta_scale,
-                                         float* out, void* stream) {
+static int backward_warp_delta(const float* c, const float* delta, int B, int H, int W, int h, int w, double delta_scale, bool f16,
+                               float* out, cudaStream_t st) {
     NB_CHECK(c && delta && out, "null pointer");
     NB_CHECK(B > 0 && H > 0 && W > 0 && h > 0 && w > 0, "bad shape");
     BwParams p;
     p.c = c; p.depth = delta; p.left = out; p.right = nullptr;
     p.B = B; p.H = H; p.W = W; p.h = h; p.w = w;
     p.shift = 1.0f; p.shift_conv = 0.0f;
-    p.delta_scale = (float)delta_scale;
+    // an fp16 tensor times the 0-dim fp32 CUDA tensor delta_scale: ATen's mul loads both operands as fp16
+    // (opmath_symmetric_gpu_kernel_with_scalars -> BinaryFunctor<Half, Half, Half>, ATen/native/cuda/Loops.cuh)
+    p.delta_scale = f16 ? __half2float(__float2half_rn((float)delta_scale)) : (float)delta_scale;
     p.sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
     p.sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
     p.step_x = w > 1 ? 2.0f / (float)(w - 1) : 0.f;
     p.warp_left = 0; p.warp_right = 1;
-    cudaStream_t st = (cudaStream_t)stream;
     const int S = (W + 1 + 3) & ~3;
     const size_t smem = sizeof(GridTab) * (size_t)(w + 1) + sizeof(float) * 3 * (size_t)S;
     NB_CHECK(smem <= 200 * 1024 && B <= 65535, "image row too wide for the row-staged warp");
     const bool aligned = (((uintptr_t)c | (uintptr_t)out) & 15) == 0;
     ProfScope ps(st, PC_WARP_BW, (double)B * H * W * 4 * 6 + (double)B * h * w * 4);
-    if (launch_bw_row<COMPOSE_RIGHT_ONLY>(p, smem, S, (W % 4 == 0) && aligned, st)) return 1;
+    const int vec_ok = (W % 4 == 0) && aligned;
+    if (f16 ? launch_bw_row<COMPOSE_RIGHT_ONLY, true>(p, smem, S, vec_ok, st) : launch_bw_row<COMPOSE_RIGHT_ONLY>(p, smem, S, vec_ok, st))
+        return 1;
+    NB_LAUNCHED();
+    return 0;
+}
+
+extern "C" int nb200_backward_warp_delta(const float* c, const float* delta, int B, int H, int W, int h, int w, double delta_scale,
+                                         float* out, void* stream) {
+    return backward_warp_delta(c, delta, B, H, W, h, w, delta_scale, false, out, (cudaStream_t)stream);
+}
+
+extern "C" int nb200_backward_warp_delta_f16(const float* c, const float* delta, int B, int H, int W, int h, int w, double delta_scale,
+                                             float* out, void* stream) {
+    return backward_warp_delta(c, delta, B, H, W, h, w, delta_scale, true, out, (cudaStream_t)stream);
+}
+
+// apply_divergence_nn_symmetric (iw3/backward_warp.py:344-379): both eyes from one delta.  With index_shift := -delta
+// (shift = -1, convergence term 0) the kernel's "-" view is mesh + delta * scale (left) and its "+" view mesh - delta * scale
+// (right); negation is exact, so both grids equal the reference's grid + (+-delta) * delta_scale bit for bit.
+extern "C" int nb200_backward_warp_delta_sym(const float* c, const float* delta, int B, int H, int W, int h, int w, double delta_scale,
+                                             int warp_left, int warp_right, float* left, float* right, void* stream) {
+    NB_CHECK(c && delta && left && right, "null pointer");
+    NB_CHECK(B > 0 && H > 0 && W > 0 && h > 0 && w > 0, "bad shape");
+    BwParams p;
+    p.c = c; p.depth = delta; p.left = left; p.right = right;
+    p.B = B; p.H = H; p.W = W; p.h = h; p.w = w;
+    p.shift = -1.0f; p.shift_conv = 0.0f;
+    p.delta_scale = (float)delta_scale;
+    p.sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
+    p.sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
+    p.step_x = w > 1 ? 2.0f / (float)(w - 1) : 0.f;
+    p.warp_left = warp_left != 0; p.warp_right = warp_right != 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int S = (W + 1 + 3) & ~3;
+    const size_t smem = sizeof(GridTab) * (size_t)(w + 1) + sizeof(float) * 3 * (size_t)S;
+    NB_CHECK(smem <= 200 * 1024 && B <= 65535, "image row too wide for the row-staged warp");
+    const bool aligned = (((uintptr_t)c | (uintptr_t)left | (uintptr_t)right) & 15) == 0;
+    ProfScope ps(st, PC_WARP_BW, (double)B * H * W * 4 * 9 + (double)B * h * w * 4);
+    if (launch_bw_row<NB200_COMPOSE_NONE>(p, smem, S, (W % 4 == 0) && aligned, st)) return 1;
     NB_LAUNCHED();
     return 0;
 }

@@ -19,6 +19,7 @@ from .depth_anything_model import DepthAnythingModel, DepthAnythingNet, batch_in
 from . import zoedepth_preprocess  # noqa: F401
 from .zoedepth_model import ZoeDepthModel, ZoeDepthNet  # noqa: F401
 from .row_flow import RowFlowV3, MLBW, apply_divergence_nn_LR, apply_divergence_nn_delta, apply_divergence_nn_delta_weight  # noqa: F401
+from .row_flow import RowFlowV2, apply_divergence_nn_symmetric, load_row_flow_model  # noqa: F401
 from .row_flow import postprocess_hole_mask  # noqa: F401
 from .depth_aa import DepthAA  # noqa: F401
 from .postprocess import postprocess_image, postprocess_padding, resize_bicubic_aa, equirectangular_projection  # noqa: F401

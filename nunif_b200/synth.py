@@ -327,6 +327,25 @@ def row_flow_v3_state_dict(seed=0):
     return sd
 
 
+def row_flow_v2_state_dict(seed=0):
+    """Seeded weights with the key names of `sbs.row_flow_v2` (iw3/models/row_flow_v2.py:13-37).  He-style gains with small
+    positive biases keep the ReLUs alive; the two heads give deltas of a few pixels for unit-range depth."""
+    g = torch.Generator().manual_seed(21_000 + seed)
+
+    def rn(*shape, std=1.0):
+        return torch.randn(*shape, generator=g) * std
+
+    return {
+        "feature.0.weight": rn(16, 3, 1, 3, std=(2.0 / 9) ** 0.5), "feature.0.bias": 0.05 + rn(16, std=0.05),
+        "non_overlap.weight": rn(1, 16, 1, 1, std=0.5), "non_overlap.bias": rn(1, std=0.1),
+        "overlap_residual.0.weight": rn(16, 16, 1, 9, std=(2.0 / 144) ** 0.5), "overlap_residual.0.bias": 0.05 + rn(16, std=0.05),
+        "overlap_residual.2.weight": rn(32, 16, 1, 9, std=(2.0 / 144) ** 0.5), "overlap_residual.2.bias": 0.05 + rn(32, std=0.05),
+        "overlap_residual.4.weight": rn(32, 32, 1, 9, std=(2.0 / 288) ** 0.5), "overlap_residual.4.bias": 0.05 + rn(32, std=0.05),
+        "overlap_residual.6.weight": rn(1, 32, 3, 3, std=1.0 / 288 ** 0.5), "overlap_residual.6.bias": rn(1, std=0.1),
+        "delta_scale": torch.tensor(1.0 / 127.0),
+    }
+
+
 def _window_bias_buffers(ws):
     """`index` / `delta` buffers of WindowScoreBias (nunif/modules/attention.py:347-372) for a square window."""
     N = ws * ws
