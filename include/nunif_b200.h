@@ -95,7 +95,8 @@ enum {
     NB200_MODEL_UPCONV_7 = 13,             /* waifu2x.upconv_7 (waifu2x/models/upconv_7.py:6-38): scale 2, offset 14 */
     NB200_MODEL_VGG_7 = 14,                /* waifu2x.vgg_7    (waifu2x/models/vgg_7.py:6-36): scale 1, offset 7 */
     NB200_MODEL_LIGHT_INPAINT_V1 = 15,     /* inpaint.light_inpaint_v1, iw3's image-mode hole inpainting (iw3/models/light_inpaint_v1.py) */
-    NB200_MODEL_ROW_FLOW_V2 = 16           /* sbs.row_flow_v2, the learned row-flow warp of `--method row_flow_v2` (iw3/models/row_flow_v2.py) */
+    NB200_MODEL_ROW_FLOW_V2 = 16,          /* sbs.row_flow_v2, the learned row-flow warp of `--method row_flow_v2` (iw3/models/row_flow_v2.py) */
+    NB200_MODEL_SOD_V1 = 17                /* iw3.sod_v1, the U^2-Net-p saliency network of `--convergence-mode sod_v1` (iw3/models/sod_v1.py) */
 };
 
 /* Create a model from named fp32 host tensors using the reference's state_dict
@@ -216,6 +217,21 @@ int nb200_backward_warp_delta_f16(const float* c, const float* delta, int B, int
 int nb200_backward_warp_delta_sym(const float* c, const float* delta, int B, int H, int W, int h, int w, double delta_scale,
                                   int warp_left, int warp_right, float* left, float* right, void* stream);
 
+/* iw3 auto-convergence (--convergence-mode sod_v1, iw3/convergence_estimator.py).
+ * nb200_sod_forward: SODV1.infer(rgb, depth) (iw3/models/sod_v1.py:47-54) of a NB200_MODEL_SOD_V1 model under CUDA autocast:
+ *   rgb [B][3][H][W], depth [B][1][h][w] fp32 -> saliency [B][1][192][192] (fp32 holding the fp16 sigmoid(d0)) and depth192
+ *   [B][1][192][192] fp32 (F.interpolate(depth, (192, 192), bilinear, align_corners=False)).
+ * nb200_sod_position: ConvergenceEstimator.depth_position_from_ratio(saliency, depth192, pos) (:33-58): per image the depth
+ *   values where saliency > 0.5, their torch.quantile 0.1 / 0.9, the centre / range rule, clamp [0, 1] -> out [B] fp32.
+ *   saliency, depth [B][n]; n <= 49152.  No host synchronisation.
+ * nb200_sod_ema: the EMA of ConvergenceEstimator.__call__ (:60-81) over z [B] in batch order -> out [B].  state: 2 floats on
+ *   the device {ema, has_value}; zero them for reset().  reset_host: B host ints (NULL = none), a non-zero entry clears the
+ *   state after that frame.  B <= 1024. */
+int nb200_sod_forward(nb200_model* m, const float* rgb, int B, int H, int W, const float* depth, int h, int w, float* saliency,
+                      float* depth192, void* stream);
+int nb200_sod_position(const float* saliency, const float* depth, int B, int n, double pos, float* out, void* stream);
+int nb200_sod_ema(float* state, const float* z, int B, const int* reset_host, double decay, float* out, void* stream);
+
 /* AlphaBorderPadding.forward (nunif/utils/alpha.py:32-57): rgb [3][H][W], alpha [1][H][W] fp32 ->
  * out [3][H][W]: transparent pixels are filled from their opaque neighbours, `offset` rounds
  * (offset = the model's i2i_offset, waifu2x/utils.py:271), then clamped to [0,1]. */
@@ -248,6 +264,12 @@ int nb200_backward_warp(const float* c, const float* depth, int B, int H, int W,
                         double divergence, double convergence, int synthetic_view, int compose,
                         float* left, float* right, void* stream);
 
+/* The same warp with a per-frame convergence tensor (auto-convergence, iw3/utils.py:303-307): convergence is a device array
+ * of B fp32 values, and shift_size * convergence is then the fp32 tensor op fp32(shift_size) * convergence[b]. */
+int nb200_backward_warp_conv(const float* c, const float* depth, int B, int H, int W, int h, int w,
+                             double divergence, const float* convergence, int synthetic_view, int compose,
+                             float* left, float* right, void* stream);
+
 /* iw3/forward_warp.py:246-256 apply_divergence_forward_warp (inconsistent_shift=False).
  * depth: [B][1][h][w]; if (h,w)!=(H,W) it is resized like forward_warp.py:146-148.
  * fill!=0 <=> method=="forward_fill".  masks may be NULL (return_mask=False).
@@ -257,6 +279,12 @@ int nb200_forward_warp(const float* c, const float* depth, int B, int H, int W, 
                        double divergence, double convergence, int fill, int synthetic_view,
                        int width_base, int compose, float* left, float* right,
                        float* left_mask, float* right_mask, void* workspace, void* stream);
+
+/* nb200_forward_warp with a per-frame convergence tensor: device array of B fp32 values, as nb200_backward_warp_conv. */
+int nb200_forward_warp_conv(const float* c, const float* depth, int B, int H, int W, int h, int w,
+                            double divergence, const float* convergence, int fill, int synthetic_view,
+                            int width_base, int compose, float* left, float* right,
+                            float* left_mask, float* right_mask, void* workspace, void* stream);
 
 /* iw3/dilation.py:115-142 dilate_edge(x, [x_iter, y_iter]); x,out: [B][1][h][w];
  * workspace: nb200_dilate_edge_workspace() bytes. */

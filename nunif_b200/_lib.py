@@ -88,6 +88,13 @@ SIGNATURES = {
     "nb200_equirectangular": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_backward_warp": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_double, c_int, c_int,
                                     c_void_p, c_void_p, c_void_p]),
+    "nb200_backward_warp_conv": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_void_p, c_int, c_int,
+                                         c_void_p, c_void_p, c_void_p]),
+    "nb200_forward_warp_conv": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_void_p, c_int, c_int,
+                                        c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "nb200_sod_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "nb200_sod_position": (c_int, [c_void_p, c_void_p, c_int, c_int, c_double, c_void_p, c_void_p]),
+    "nb200_sod_ema": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_double, c_void_p, c_void_p]),
     "nb200_forward_warp_workspace": (c_size_t, [c_int] * 5),
     "nb200_forward_warp": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_double, c_int, c_int,
                                    c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

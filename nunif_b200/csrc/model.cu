@@ -14,6 +14,7 @@
 #include "zoe_kernels.h"
 #include "inpaint_kernels.h"
 #include "window_mha.h"
+#include "sod_kernels.h"
 #include "../../include/nunif_b200.h"
 #include <map>
 #include <vector>
@@ -246,6 +247,7 @@ struct nb200_model {
     std::shared_ptr<ZoeW> zoe;
     std::shared_ptr<InpW> inp;
     std::shared_ptr<Rf2W> rf2;
+    std::shared_ptr<SodW> sod;
     uint8_t* ws = nullptr;
     size_t ws_bytes = 0;
     cudaStream_t copy_stream = nullptr;   // D2H side stream of nb200_tiled_render_host
@@ -493,6 +495,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 #include "mlbw_model.inl"
 #include "zoe_model.inl"
 #include "inpaint_model.inl"
+#include "sod_model.inl"
 
 // ---------------------------------------------------------------------------------------------
 // C ABI
@@ -500,7 +503,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* names, const float* const* data,
                                   const int64_t* numel, int no_clip, nb200_model** out) {
     NB_CHECK(out && names && data && numel, "null pointer");
-    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_ROW_FLOW_V2, "unknown model kind");
+    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_SOD_V1, "unknown model kind");
     int dev = 0;
     NB_CUDA(cudaGetDevice(&dev));
     if (nb200_check_device(dev)) return 1;
@@ -536,6 +539,7 @@ extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* na
         case NB200_MODEL_VGG_7: m->lg = pack_legacy(pk, false); m->scale = 1; m->offset = 7; m->blend = 0; break;     // vgg_7.py:11
         case NB200_MODEL_LIGHT_INPAINT_V1: m->inp = pack_light_inpaint(pk); m->scale = 1; m->offset = 16; m->blend = 8; break;  // light_inpaint_v1.py:56
         case NB200_MODEL_ROW_FLOW_V2: m->rf2 = pack_row_flow_v2(pk); m->scale = 1; m->offset = 28; m->blend = 4; break;   // row_flow_v2.py:14
+        case NB200_MODEL_SOD_V1: m->sod = pack_sod(pk); m->scale = 1; break;                                           // sod_v1.py:15
     }
     if (pk.err.empty())
         for (auto& kv : pk.src)
@@ -828,6 +832,15 @@ extern "C" int nb200_row_flow_v2_delta(nb200_model* m, const float* x, int B, in
     NB_CHECK(m->kind == NB200_MODEL_ROW_FLOW_V2 && m->rf2, "model is not sbs.row_flow_v2");
     NB_CHECK(B > 0 && h > 0 && w > 0, "bad shape");
     return rf2_forward((cudaStream_t)stream, m->blob + m->rf2->params, x, B, h, w, delta);
+}
+
+// SODV1.infer (iw3/models/sod_v1.py:47-54) under autocast: sigmoid(U2NETP(cat(rgb, d, d ** 0.5, d ** 2))) at 192 x 192
+extern "C" int nb200_sod_forward(nb200_model* m, const float* rgb, int B, int H, int W, const float* depth, int h, int w,
+                                 float* saliency, float* depth192, void* stream) {
+    NB_CHECK(m && rgb && depth && saliency && depth192, "null pointer");
+    NB_CHECK(m->kind == NB200_MODEL_SOD_V1 && m->sod, "model is not iw3.sod_v1");
+    NB_CHECK(B > 0 && H > 0 && W > 0 && h > 0 && w > 0, "bad shape");
+    return sod_forward((cudaStream_t)stream, m->blob, *m->sod, rgb, B, H, W, depth, h, w, saliency, depth192);
 }
 
 // iw3/dilation.py:67-98: n = max(round(W / base_width * n_iter), 1) (Python's round: half to even), 0 when n_iter <= 0

@@ -62,6 +62,7 @@ struct BwParams {
     int B, H, W, h, w;
     float shift;        // divergence * 0.01 (x2 for single-view synthesis)
     float shift_conv;   // shift * convergence
+    const float* conv = nullptr;   // per-frame convergence [B] (nb200_backward_warp_conv): shift_conv = fp32(shift) * conv[b]
     float delta_scale;  // max(h, w) / w
     float sy, sx;       // (h-1)/(H-1), (w-1)/(W-1)  align_corners scales (fp32, like ATen)
     float step_x;       // 2/(w-1)
@@ -79,6 +80,8 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
     const float* __restrict__ dep = p.depth + (size_t)b * p.h * p.w;
     const float* __restrict__ crow = p.c + ((size_t)b * 3 * p.H + y) * p.W;
     const size_t plane = (size_t)p.H * p.W;
+    // a convergence tensor makes shift_size * convergence an fp32 tensor op (backward_warp.py:106)
+    const float shift_conv = p.conv ? __fmul_rn(p.shift, __ldg(p.conv + b)) : p.shift_conv;
 
     // vertical source coordinate in the depth map (align_corners=True bilinear)
     const bool same = (p.h == p.H) && (p.w == p.W);
@@ -99,7 +102,7 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
         float gl, gr;  // normalised grid x of left (-delta) and right (+delta)
         if (x < p.W) {
             if (same) {
-                float is = __fsub_rn(__fmul_rn(dep[(size_t)y * p.w + x], p.shift), p.shift_conv);
+                float is = __fsub_rn(__fmul_rn(dep[(size_t)y * p.w + x], p.shift), shift_conv);
                 float lx = linspace_m1_1(x, p.w, p.step_x);
                 // each product and sum rounded on its own, as in the row-staged kernel's grid table (no FMA contraction)
                 const float d = __fmul_rn(is, p.delta_scale);
@@ -110,10 +113,10 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
                 int j0 = min((int)srcx, p.w - 1);
                 int j1 = min(j0 + 1, p.w - 1);
                 float lx1 = srcx - (float)j0, lx0 = 1.f - lx1;
-                float is00 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i0 * p.w + j0), p.shift), p.shift_conv);
-                float is01 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i0 * p.w + j1), p.shift), p.shift_conv);
-                float is10 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + j0), p.shift), p.shift_conv);
-                float is11 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + j1), p.shift), p.shift_conv);
+                float is00 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i0 * p.w + j0), p.shift), shift_conv);
+                float is01 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i0 * p.w + j1), p.shift), shift_conv);
+                float is10 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + j0), p.shift), shift_conv);
+                float is11 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + j1), p.shift), shift_conv);
                 float l0 = linspace_m1_1(j0, p.w, p.step_x), l1 = linspace_m1_1(j1, p.w, p.step_x);
                 const float ds = p.delta_scale;
                 const float d00 = __fmul_rn(is00, ds), d01 = __fmul_rn(is01, ds), d10 = __fmul_rn(is10, ds), d11 = __fmul_rn(is11, ds);
@@ -208,6 +211,7 @@ __global__ void __launch_bounds__(256) backward_warp_row_kernel(BwParams p, int 
     const size_t plane = (size_t)p.H * p.W;
     const float* __restrict__ crow = p.c + ((size_t)b * 3 * p.H + y) * p.W;
     const float* __restrict__ dep = p.depth + (size_t)b * p.h * p.w;
+    const float shift_conv = p.conv ? __fmul_rn(p.shift, __ldg(p.conv + b)) : p.shift_conv;
 
     const bool same = (p.h == p.H) && (p.w == p.W);
     int i0 = y, i1 = y;
@@ -235,8 +239,8 @@ __global__ void __launch_bounds__(256) backward_warp_row_kernel(BwParams p, int 
     for (int j = tid; j <= p.w; j += 256) {
         const int jj = min(j, p.w - 1);
         const float lx = linspace_m1_1(jj, p.w, p.step_x);
-        const float is0 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i0 * p.w + jj), p.shift), p.shift_conv);
-        const float is1 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + jj), p.shift), p.shift_conv);
+        const float is0 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i0 * p.w + jj), p.shift), shift_conv);
+        const float is1 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + jj), p.shift), shift_conv);
         float d0 = __fmul_rn(is0, p.delta_scale), d1 = __fmul_rn(is1, p.delta_scale);
         if (F16_PRODUCT) {
             d0 = __half2float(__float2half_rn(d0));
@@ -358,9 +362,9 @@ __global__ void __launch_bounds__(256) anaglyph_dubois_kernel(const float* __res
 
 using namespace nb200;
 
-extern "C" int nb200_backward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w,
-                                   double divergence, double convergence, int synthetic_view, int compose,
-                                   float* left, float* right, void* stream) {
+static int backward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w, double divergence,
+                         double convergence, const float* conv, int synthetic_view, int compose, float* left, float* right,
+                         void* stream) {
     NB_CHECK(c && depth && left, "null pointer");
     NB_CHECK(compose != NB200_COMPOSE_NONE || right, "right output required for compose=NONE");
     NB_CHECK(B > 0 && H > 0 && W > 0 && h > 0 && w > 0, "bad shape");
@@ -373,6 +377,7 @@ extern "C" int nb200_backward_warp(const float* c, const float* depth, int B, in
     double shift = div * 0.01;                                       // :105
     p.shift = (float)shift;
     p.shift_conv = (float)(shift * convergence);             // :106
+    p.conv = conv;
     p.delta_scale = (float)((double)(h > w ? h : w) / (double)w);    // :108
     p.sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
     p.sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
@@ -409,6 +414,19 @@ extern "C" int nb200_backward_warp(const float* c, const float* depth, int B, in
     }
     NB_LAUNCHED();
     return 0;
+}
+
+extern "C" int nb200_backward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w,
+                                   double divergence, double convergence, int synthetic_view, int compose,
+                                   float* left, float* right, void* stream) {
+    return backward_warp(c, depth, B, H, W, h, w, divergence, convergence, nullptr, synthetic_view, compose, left, right, stream);
+}
+
+extern "C" int nb200_backward_warp_conv(const float* c, const float* depth, int B, int H, int W, int h, int w,
+                                        double divergence, const float* convergence, int synthetic_view, int compose,
+                                        float* left, float* right, void* stream) {
+    NB_CHECK(convergence, "null convergence");
+    return backward_warp(c, depth, B, H, W, h, w, divergence, 0.0, convergence, synthetic_view, compose, left, right, stream);
 }
 
 extern "C" int nb200_anaglyph_dubois(const float* l, const float* r, int B, int H, int W, int clip_before,

@@ -40,6 +40,7 @@ struct FwParams {
     int B, H, W, h, w, P, Wp;
     float shift_size;  // divergence*0.01*base*0.5
     float conv_term;   // shift_size*convergence
+    const float* conv = nullptr;  // per-frame convergence [B] (nb200_forward_warp_conv): conv_term = fp32(shift_size) * conv[b]
     int fill, do_left, do_right, compose;
     float scale_y, scale_x;  // AA resize scales (h-1)/(H-1), (w-1)/(W-1)
     const float4* coltab;    // per output column: {xmin (as int bits), w0, w1, w2} of the AA resize (upsampling only), or null
@@ -157,6 +158,8 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
         __syncthreads();
     }
 
+    // a convergence tensor makes shift_size * convergence an fp32 tensor op (forward_warp.py:167)
+    const float conv_term = p.conv ? __fmul_rn(p.shift_size, __ldg(p.conv + b)) : p.conv_term;
     for (int eye = 0; eye < 2; ++eye) {
         if (eye == 0 ? !p.do_left : !p.do_right) continue;
         const float sg = eye == 0 ? 1.f : -1.f;  // left: +index_shift, right: -index_shift (:176-177)
@@ -171,7 +174,7 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
         // ---- pass 1: z-buffer -- make_bilinear_data :75-85 + ordered_index_copy :88-110
         for (int xp = tid; xp < Wp; xp += FW_THREADS) {
             float d = DEP[xp];
-            float is = __fsub_rn(__fmul_rn(d, p.shift_size), p.conv_term);
+            float is = __fsub_rn(__fmul_rn(d, p.shift_size), conv_term);
             float fi = fminf(fmaxf(__fadd_rn((float)xp, sg * is), 0.f), (float)(Wp - 1));
             int fl = (int)floorf(fi), ce = (int)ceilf(fi);
             unsigned key = depth_key(d);
@@ -182,7 +185,7 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
         // ---- pass 2: winners (unique per visible cell, see header)
         for (int xp = tid; xp < Wp; xp += FW_THREADS) {
             float d = DEP[xp];
-            float is = __fsub_rn(__fmul_rn(d, p.shift_size), p.conv_term);
+            float is = __fsub_rn(__fmul_rn(d, p.shift_size), conv_term);
             float fi = fminf(fmaxf(__fadd_rn((float)xp, sg * is), 0.f), (float)(Wp - 1));
             int fl = (int)floorf(fi), ce = (int)ceilf(fi);
             unsigned key = depth_key(d);
@@ -198,7 +201,7 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
             float Fw = 0.f, Cw = 0.f, Fv[4] = {-1.f, -1.f, -1.f, -1.f}, Cv[4] = {-1.f, -1.f, -1.f, -1.f};
             if (a >= 0) {
                 float d = DEP[a];
-                float is = __fsub_rn(__fmul_rn(d, p.shift_size), p.conv_term);
+                float is = __fsub_rn(__fmul_rn(d, p.shift_size), conv_term);
                 float fi = fminf(fmaxf(__fadd_rn((float)a, sg * is), 0.f), (float)(Wp - 1));
                 float cw = fminf(fmaxf(__fsub_rn(fi, floorf(fi)), (float)1e-5), (float)(1.0 - 1e-5));
                 Fw = __fsub_rn(1.0f, cw);
@@ -210,7 +213,7 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
             }
             if (cidx >= 0) {
                 float d = DEP[cidx];
-                float is = __fsub_rn(__fmul_rn(d, p.shift_size), p.conv_term);
+                float is = __fsub_rn(__fmul_rn(d, p.shift_size), conv_term);
                 float fi = fminf(fmaxf(__fadd_rn((float)cidx, sg * is), 0.f), (float)(Wp - 1));
                 Cw = fminf(fmaxf(__fsub_rn(fi, floorf(fi)), (float)1e-5), (float)(1.0 - 1e-5));
                 int sx = min(max(cidx - P, 0), W - 1);
@@ -339,10 +342,9 @@ extern "C" size_t nb200_forward_warp_workspace(int B, int H, int W, int h, int w
     return (h != H || w != W) ? (size_t)W * sizeof(float4) : 0;
 }
 
-extern "C" int nb200_forward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w,
-                                  double divergence, double convergence, int fill, int synthetic_view,
-                                  int width_base, int compose, float* left, float* right,
-                                  float* left_mask, float* right_mask, void* workspace, void* stream) {
+static int forward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w, double divergence,
+                        double convergence, const float* conv, int fill, int synthetic_view, int width_base, int compose,
+                        float* left, float* right, float* left_mask, float* right_mask, void* workspace, void* stream) {
     NB_CHECK(c && depth && left, "null pointer");
     NB_CHECK(compose == NB200_COMPOSE_NONE || compose == NB200_COMPOSE_SBS, "compose must be NONE or SBS");
     NB_CHECK(compose == NB200_COMPOSE_SBS || right, "right output required");
@@ -358,6 +360,7 @@ extern "C" int nb200_forward_warp(const float* c, const float* depth, int B, int
     const double shift_size = div * 0.01 * base * 0.5;               // :166
     p.shift_size = (float)shift_size;
     p.conv_term = (float)(shift_size * convergence);         // :167
+    p.conv = conv;
     p.fill = fill;
     p.do_left = synthetic_view != NB200_VIEW_RIGHT;
     p.do_right = synthetic_view != NB200_VIEW_LEFT;
@@ -390,6 +393,23 @@ extern "C" int nb200_forward_warp(const float* c, const float* depth, int B, int
         NB_LAUNCHED();
     }
     return 0;
+}
+
+extern "C" int nb200_forward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w,
+                                  double divergence, double convergence, int fill, int synthetic_view,
+                                  int width_base, int compose, float* left, float* right,
+                                  float* left_mask, float* right_mask, void* workspace, void* stream) {
+    return forward_warp(c, depth, B, H, W, h, w, divergence, convergence, nullptr, fill, synthetic_view, width_base, compose, left,
+                        right, left_mask, right_mask, workspace, stream);
+}
+
+extern "C" int nb200_forward_warp_conv(const float* c, const float* depth, int B, int H, int W, int h, int w,
+                                       double divergence, const float* convergence, int fill, int synthetic_view,
+                                       int width_base, int compose, float* left, float* right,
+                                       float* left_mask, float* right_mask, void* workspace, void* stream) {
+    NB_CHECK(convergence, "null convergence");
+    return forward_warp(c, depth, B, H, W, h, w, divergence, 0.0, convergence, fill, synthetic_view, width_base, compose, left,
+                        right, left_mask, right_mask, workspace, stream);
 }
 
 extern "C" int nb200_depth_resize_aa(const float* depth, int B, int h, int w, int H, int W, float* out, void* stream) {

@@ -25,4 +25,5 @@ from .depth_aa import DepthAA  # noqa: F401
 from .postprocess import postprocess_image, postprocess_padding, resize_bicubic_aa, equirectangular_projection  # noqa: F401
 from .forward_inpaint import ForwardInpaint, LightInpaintV1  # noqa: F401
 from .mlbw_inpaint import MLBWInpaint  # noqa: F401
+from .convergence_estimator import ConvergenceEstimator, SODV1  # noqa: F401
 from .utils import apply_divergence, process_image  # noqa: F401

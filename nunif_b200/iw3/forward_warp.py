@@ -34,8 +34,15 @@ def apply_divergence_forward_warp(c, depth, divergence, convergence, method=None
     ws_bytes = _lib.lib().nb200_forward_warp_workspace(B, H, W, h, w)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().nb200_forward_warp(
-            _lib.ptr(c), _lib.ptr(depth), B, H, W, h, w, float(divergence), float(convergence), fill,
+        if torch.is_tensor(convergence):
+            # per-frame convergence (auto-convergence): B,1,1,1, one value per frame
+            conv = prep(convergence, "convergence").reshape(-1)
+            assert conv.numel() == B, "convergence tensor must hold one value per frame"
+            fn, cv = _lib.lib().nb200_forward_warp_conv, _lib.ptr(conv)
+        else:
+            fn, cv = _lib.lib().nb200_forward_warp, float(convergence)
+        _lib.check(fn(
+            _lib.ptr(c), _lib.ptr(depth), B, H, W, h, w, float(divergence), cv, fill,
             VIEWS[synthetic_view], 1 if width_base else 0, compose, _lib.ptr(left), _lib.ptr(right),
             _lib.ptr(lm if synthetic_view != "right" else None), _lib.ptr(rm if synthetic_view != "left" else None),
             _lib.ptr(ws), _lib.stream_ptr(dev)))

@@ -146,11 +146,16 @@ def make_input(depth, divergence, convergence, preserve_screen_border=False, ima
     """make_input_tensor(None, depth, ...) for a batch (iw3/backward_warp.py:18-63): depth, divergence feature, convergence
     feature; with preserve_screen_border the two features fade linearly to zero over `border_pix` columns at both edges.
     ``image_width`` is the base width of the feature values: max(H, W) in apply_divergence_nn_delta (the default), W in
-    apply_divergence_nn_symmetric."""
+    apply_divergence_nn_symmetric.  ``convergence`` is a float or a B,1,1,1 tensor (one value per frame)."""
     B, _, H, W = depth.shape
     base = max(H, W) if image_width is None else image_width
     dv, cv = make_divergence_feature_value(divergence, convergence, base)
-    df, cf = torch.full_like(depth, dv), torch.full_like(depth, cv)
+    df = torch.full_like(depth, dv)
+    if torch.is_tensor(cv):
+        # a B,1,1,1 convergence tensor: (-divergence_pix * c) / 32 per frame in fp32, expanded over the map (:24-25)
+        cf = cv.to(device=depth.device, dtype=depth.dtype).reshape(B, 1, 1, 1).expand_as(depth).clone()
+    else:
+        cf = torch.full_like(depth, cv)
     if preserve_screen_border:
         bp = round(divergence * 0.75 * 0.01 * base * (W / base))                               # :36
         if bp > 0:

@@ -4,7 +4,8 @@ layers, which stay in the reference's host code).
 
 ``args`` is the reference's argparse namespace; the fields read here are the ones the reference reads on this path:
 ``method, mapper, convergence, divergence, synthetic_view, warp_steps, preserve_screen_border, stereo_width, disable_amp,
-mask_inner_dilation, mask_outer_dilation, inpaint_max_width, state["convergence_model"]``.  Anything the engine does not implement raises ``NotImplementedError`` - never a silent
+mask_inner_dilation, mask_outer_dilation, inpaint_max_width, state["convergence_model"]``.  A convergence model must be the
+engine's ``ConvergenceEstimator`` (``--convergence-mode sod_v1``).  Anything the engine does not implement raises ``NotImplementedError`` - never a silent
 fallback."""
 import torch
 
@@ -13,6 +14,7 @@ from .forward_warp import apply_divergence_forward_warp
 from .depth_scaler import depth_mapper
 from .row_flow import apply_divergence_nn_LR
 from .postprocess import postprocess_image
+from .convergence_estimator import ConvergenceEstimator
 
 _WARP = {"grid_sample": "backward", "backward": "backward", "forward": "forward", "forward_fill": "forward"}
 
@@ -27,11 +29,17 @@ def apply_divergence(depth, im, args, side_model, reset_pts=None):
     if not batched:
         depth, im = depth.unsqueeze(0), im.unsqueeze(0)
     state = _arg(args, "state", None) or {}
-    if state.get("convergence_model") is not None:
-        raise NotImplementedError("auto-convergence (args.state['convergence_model']) is not implemented by the H100 engine")
+    convergence_model = state.get("convergence_model")
+    if convergence_model is not None and not isinstance(convergence_model, ConvergenceEstimator):
+        raise NotImplementedError("auto-convergence needs the engine's estimator in args.state['convergence_model'] "
+                                  f"(nunif_b200.iw3.ConvergenceEstimator), got {type(convergence_model).__name__}")
     if not _arg(args, "disable_amp", False) is False:
         raise NotImplementedError("--disable-amp (fp32 side model) is not implemented: the engine runs the CUDA autocast numerics")
-    convergence = args.convergence
+    if convergence_model is not None:
+        # --convergence-mode sod_v1 (:303-307): a B,1,1,1 convergence per frame, mapped like the depth
+        convergence = depth_mapper(convergence_model(im, depth, reset_pts=reset_pts), args.mapper)
+    else:
+        convergence = args.convergence
     depth = depth_mapper(depth, args.mapper)                                    # get_mapper(args.mapper)(depth), :313
     method = args.method
     if method == "NULL":

@@ -550,3 +550,52 @@ def light_inpaint_v1_state_dict(seed=0):
     _conv(sd, g, "to_image.1", 48, C, 3, 3, gain=0.05, bias_std=0.0)
     sd["to_image.1.bias"] = 0.5 + _normal(g, (48,), 0.05)
     return sd
+
+
+# ----------------------------------------------------------------------------
+# iw3.sod_v1 (iw3/models/sod_v1.py: U2NETP(in_ch=6), nunif/utils/u2netp.py)
+# ----------------------------------------------------------------------------
+
+# the outconv bias of sod_v1_state_dict: with it the saliency > 0.5 mask covers part of each golden frame, neither none nor
+# all of it (oracle/gen_golden_sod.py prints and checks the fraction)
+SOD_OUT_BIAS = 0.76
+
+SOD_STAGES = (("stage1", 7, 6), ("stage2", 6, 64), ("stage3", 5, 64), ("stage4", 4, 64), ("stage5", 0, 64), ("stage6", 0, 64),
+              ("stage5d", 0, 128), ("stage4d", 4, 128), ("stage3d", 5, 128), ("stage2d", 6, 128), ("stage1d", 7, 128))
+
+
+def sod_rebnconvs():
+    """(name, cin, cout, dilation) of every REBNCONV of U2NETP(in_ch=6) in forward order; RSU4F is n = 0."""
+    out = []
+    for stage, n, cin in SOD_STAGES:
+        p = f"u2netp.{stage}.rebnconv"
+        out += [(p + "in", cin, 64, 1), (p + "1", 64, 16, 1)]
+        if n == 0:
+            out += [(p + "2", 16, 16, 2), (p + "3", 16, 16, 4), (p + "4", 16, 16, 8), (p + "3d", 32, 16, 4), (p + "2d", 32, 16, 2)]
+        else:
+            out += [(p + str(k), 16, 16, 1) for k in range(2, n)] + [(p + str(n), 16, 16, 2)]
+            out += [(p + f"{k}d", 32, 16, 1) for k in range(n - 1, 1, -1)]
+        out.append((p + "1d", 32, 64, 1))
+    return out
+
+
+def sod_v1_state_dict(seed=0):
+    """Seeded weights with the key names of `iw3.sod_v1` (SODV1.u2netp).  Every BatchNorm has non-trivial statistics
+    (running_var != 1, gamma, beta, mean) so that the folding of U2NETP.fuse() matters; the gains keep the activations of
+    the residual stages in fp16 range, and SOD_OUT_BIAS sets the share of salient pixels."""
+    g = torch.Generator().manual_seed(60_000 + seed)
+    sd = {}
+    for name, cin, cout, _ in sod_rebnconvs():
+        sd[name + ".conv_s1.weight"] = torch.randn(cout, cin, 3, 3, generator=g) * (1.4 / (9 * cin)) ** 0.5
+        sd[name + ".conv_s1.bias"] = torch.randn(cout, generator=g) * 0.05
+        sd[name + ".bn_s1.weight"] = 0.8 + 0.4 * torch.rand(cout, generator=g)
+        sd[name + ".bn_s1.bias"] = 0.02 + torch.randn(cout, generator=g) * 0.05
+        sd[name + ".bn_s1.running_mean"] = torch.randn(cout, generator=g) * 0.1
+        sd[name + ".bn_s1.running_var"] = 0.5 + 1.5 * torch.rand(cout, generator=g)
+        sd[name + ".bn_s1.num_batches_tracked"] = torch.tensor(1000, dtype=torch.int64)
+    for k in range(1, 7):
+        sd[f"u2netp.side{k}.weight"] = torch.randn(1, 64, 3, 3, generator=g) * (1.0 / (9 * 64)) ** 0.5
+        sd[f"u2netp.side{k}.bias"] = torch.randn(1, generator=g) * 0.1
+    sd["u2netp.outconv.weight"] = (0.5 + torch.rand(1, 6, 1, 1, generator=g)) / 3
+    sd["u2netp.outconv.bias"] = torch.tensor([SOD_OUT_BIAS])
+    return sd
