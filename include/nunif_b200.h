@@ -96,7 +96,19 @@ enum {
     NB200_MODEL_VGG_7 = 14,                /* waifu2x.vgg_7    (waifu2x/models/vgg_7.py:6-36): scale 1, offset 7 */
     NB200_MODEL_LIGHT_INPAINT_V1 = 15,     /* inpaint.light_inpaint_v1, iw3's image-mode hole inpainting (iw3/models/light_inpaint_v1.py) */
     NB200_MODEL_ROW_FLOW_V2 = 16,          /* sbs.row_flow_v2, the learned row-flow warp of `--method row_flow_v2` (iw3/models/row_flow_v2.py) */
-    NB200_MODEL_SOD_V1 = 17                /* iw3.sod_v1, the U^2-Net-p saliency network of `--convergence-mode sod_v1` (iw3/models/sod_v1.py) */
+    NB200_MODEL_SOD_V1 = 17,               /* iw3.sod_v1, the U^2-Net-p saliency network of `--convergence-mode sod_v1` (iw3/models/sod_v1.py) */
+    /* ZoeD_Any_N / ZoeD_Any_K, iw3's default depth model: third-party net the reference loads through torch.hub
+     * "nagadomi/Depth-Anything_iw3" DepthAnythingMetricDepth (iw3/zoedepth_model.py:12-20,154-170); a Depth-Anything V1 encoder
+     * and DPT head under the ZoeDepth bins head, keys `core.core.pretrained.*`, `core.core.depth_head.*`, `conv2`, ...
+     * N (indoor) has the "softplus" bins head of ZoeD_N, K (outdoor) the "normed" one (max_depth 80).  Widths read off the
+     * tensor sizes.  Run through nb200_zoedepth_forward. */
+    NB200_MODEL_ZOEDEPTH_ANY_N = 18,
+    NB200_MODEL_ZOEDEPTH_ANY_K = 19,
+    /* Depth-Anything V1 Any_S / Any_B / Any_L (iw3/depth_anything_model.py:36-38): the V2 S/B/L networks with the hooks on the
+     * last four blocks; checkpoints depth_anything_vit{s,b,l}14.pth.  Run through nb200_depth_anything_forward. */
+    NB200_MODEL_DEPTH_ANYTHING_V1_S = 20,
+    NB200_MODEL_DEPTH_ANYTHING_V1_B = 21,
+    NB200_MODEL_DEPTH_ANYTHING_V1_L = 22
 };
 
 /* Create a model from named fp32 host tensors using the reference's state_dict
@@ -136,7 +148,7 @@ int nb200_tiled_render(nb200_model* m, const float* x, int C, int H, int W, int 
 int nb200_tiled_render_host(nb200_model* m, const float* x_host, int C, int H, int W, int tile_size,
                             int batch_size, int downscale, float* out_host, void* stream);
 
-/* DepthAnythingV2.forward as called by DepthAnythingModel._forward (iw3/depth_anything_model.py:113-119):
+/* DepthAnythingV2.forward (or the V1 DepthAnything.forward) as called by DepthAnythingModel._forward (iw3/depth_anything_model.py:113-119):
  * x [B][3][H][W] fp32, ImageNet-normalised (nb200_da_preprocess), H and W multiples of 14
  * -> depth [B][H][W] fp32 (relative inverse depth, larger = nearer). */
 int nb200_depth_anything_forward(nb200_model* m, const float* x, int B, int H, int W, float* depth,
@@ -144,7 +156,8 @@ int nb200_depth_anything_forward(nb200_model* m, const float* x, int B, int H, i
 
 /* ZoeDepth.forward(x)['metric_depth'] as called by zoedepth_model._forward (iw3/zoedepth_model.py:23-27):
  * x [B][3][H][W] fp32, normalised (x - 0.5) / 0.5 and reflection padded (nb200_zoe_preprocess), H and W multiples of 32
- * -> depth [B][H][W] fp32 (metric depth, larger = farther; batch_infer negates it, zoedepth_model.py:124-130). */
+ * (ZoeD_N) or of 14 (ZoeD_Any_N / ZoeD_Any_K, prep_mod 14) -> depth [B][H][W] fp32 (metric depth, larger = farther; batch_infer
+ * negates it, zoedepth_model.py:124-130). */
 int nb200_zoedepth_forward(nb200_model* m, const float* x, int B, int H, int W, float* depth, void* stream);
 /* Host-only helper of the same path: the per-block relative-position table ((2g-1)^2 + 3 rows x heads, learned on a g x g token
  * grid) resampled for a ph x pw grid as MiDaS backbones/beit.py `_get_rel_pos_bias` does (bilinear, the 3 class-token rows kept). */
@@ -406,7 +419,8 @@ int nb200_equirectangular(const float* c, int C, int H, int W, float* out, void*
  * bench.py for the live roofline figure.  report writes a JSON object
  * {"gemm": {"launches": n, "ms": t, "work": flops_or_bytes}, ...} and synchronises the device. */
 int nb200_tune_set(int key, int value);   /* kernel-selection knobs (csrc/gemm.cu g_tune), for tests and A/B runs */
-int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermediate `id` of nb200_zoedepth_forward (ids 0..14)
+int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermediate `id` of nb200_zoedepth_forward (ids 0..14,
+                                                               15 = the sorted centres of a normed head, DESIGN.md §5)
                                                                or nb200_light_inpaint (ids 100..173, DESIGN.md §5) to dev_buf */
 int nb200_profile_enable(int on);
 int nb200_profile_report(char* buf, size_t cap);

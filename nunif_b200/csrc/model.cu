@@ -476,7 +476,7 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
 #include "cunet_model.inl"
 #include "legacy_model.inl"
 // debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth or light_inpaint_v1 forward is copied to `g_tap_buf`
-// (ZoeDepth ids 0..14 in zoe_model.inl; light_inpaint_v1 ids 100..173, table in DESIGN.md §5)
+// (ZoeDepth ids 0..15 in zoe_model.inl; light_inpaint_v1 ids 100..173, table in DESIGN.md §5)
 static int g_tap_id = -1;
 static void* g_tap_buf = nullptr;
 static size_t g_tap_cap = 0;
@@ -503,7 +503,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* names, const float* const* data,
                                   const int64_t* numel, int no_clip, nb200_model** out) {
     NB_CHECK(out && names && data && numel, "null pointer");
-    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_SOD_V1, "unknown model kind");
+    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_DEPTH_ANYTHING_V1_L, "unknown model kind");
     int dev = 0;
     NB_CUDA(cudaGetDevice(&dev));
     if (nb200_check_device(dev)) return 1;
@@ -540,6 +540,11 @@ extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* na
         case NB200_MODEL_LIGHT_INPAINT_V1: m->inp = pack_light_inpaint(pk); m->scale = 1; m->offset = 16; m->blend = 8; break;  // light_inpaint_v1.py:56
         case NB200_MODEL_ROW_FLOW_V2: m->rf2 = pack_row_flow_v2(pk); m->scale = 1; m->offset = 28; m->blend = 4; break;   // row_flow_v2.py:14
         case NB200_MODEL_SOD_V1: m->sod = pack_sod(pk); m->scale = 1; break;                                           // sod_v1.py:15
+        case NB200_MODEL_ZOEDEPTH_ANY_N: m->zoe = pack_zoedepth_any(pk, false); m->scale = 1; break;                    // zoedepth_model.py:20
+        case NB200_MODEL_ZOEDEPTH_ANY_K: m->zoe = pack_zoedepth_any(pk, true); m->scale = 1; break;
+        case NB200_MODEL_DEPTH_ANYTHING_V1_S: m->da = pack_depth_anything(pk, 0, "", true); m->scale = 1; break;     // depth_anything_model.py:36-38
+        case NB200_MODEL_DEPTH_ANYTHING_V1_B: m->da = pack_depth_anything(pk, 1, "", true); m->scale = 1; break;
+        case NB200_MODEL_DEPTH_ANYTHING_V1_L: m->da = pack_depth_anything(pk, 2, "", true); m->scale = 1; break;
     }
     if (pk.err.empty())
         for (auto& kv : pk.src)

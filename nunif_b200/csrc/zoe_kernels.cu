@@ -1,5 +1,5 @@
-// Non-GEMM kernels of the ZoeD_N metric depth network (BEiT-L/16 encoder + MiDaS DPT head + ZoeDepth bins head) that
-// Depth-Anything does not already provide (depth_kernels.cu: add+LayerNorm, flash attention, relu/upsample/im2col helpers).
+// Non-GEMM kernels of the ZoeDepth metric depth networks (ZoeD_N: BEiT-L/16 encoder + MiDaS DPT head, ZoeD_Any: Depth-Anything
+// encoder + DPT head; both with the ZoeDepth bins head, "softplus" or "normed") that Depth-Anything does not already provide (depth_kernels.cu: add+LayerNorm, flash attention, relu/upsample/im2col helpers).
 // The reference runs the network under fp16 autocast (iw3/zoedepth_model.py:23-27): convs / Linears in fp16 with fp32
 // accumulate, softplus / log / softmax / interpolate-of-fp32 in fp32 - mirrored here: everything that feeds a GEMM is
 // fp16 NHWC, the bin centres and the final log-binomial mixture are fp32.
@@ -182,6 +182,98 @@ __global__ void __launch_bounds__(256) zoe_attractor_kernel(const __half* __rest
     out[i] = c + delta / (float)na;
 }
 
+// ------------------------------------------------------------------------------------------ normed bins head (ZoeD_Any_K)
+// SeedBinRegressor (normed): one warp per pixel, lane l owns bins 2l, 2l+1.  w = fp16(relu + 1e-3) (the reference adds the eps
+// to the fp16 conv output); widths = (max - min) * w / sum(w) in fp32 (autocast runs sum and cumsum in fp32); edges = min, then
+// the running sum (a warp scan); centres = edge midpoints; out = (centres - min) / (max - min), the b_prev of the first level.
+__global__ void __launch_bounds__(256) zoe_seed_normed_kernel(const __half* __restrict__ s, long long npix, float lo, float span,
+                                                               float* __restrict__ out) {
+    if (threadIdx.x == 0) NB_PDL_TRIGGER();
+    const long long pix = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (pix >= npix) return;
+    const float2 r = __half22float2(__ldg(reinterpret_cast<const __half2*>(s + (size_t)pix * NBINS) + lane));
+    const float w0 = __half2float(__float2half_rn(r.x + 1e-3f)), w1 = __half2float(__float2half_rn(r.y + 1e-3f));
+    float sum = w0 + w1;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    const float b0 = span * (w0 / sum), b1 = span * (w1 / sum);
+    float incl = b0 + b1;                          // inclusive scan of the pair widths over the lanes
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const float v = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += v;
+    }
+    const float e0 = lo + (incl - (b0 + b1)), e1 = e0 + b0, e2 = e1 + b1;
+    const float2 c = make_float2((0.5f * (e0 + e1) - lo) / span, (0.5f * (e1 + e2) - lo) / span);
+    reinterpret_cast<float2*>(out + (size_t)pix * NBINS)[lane] = c;
+}
+
+// AttractorLayer (normed): one warp per pixel, lane l owns bins l and l + 32.  c = bilinear(align_corners)(prev), a_j =
+// fp16(relu + 1e-3) of pre-activation channel 2j (the upstream view(n, na, 2)[:, :, 0] without the normalisation), b_new = c +
+// mean_j inv_attractor(a_j - c) -> out.  With `sorted`: (max - min) b_new + min, sorted along the 64 bins (a bitonic network over
+// the lanes' registers) and clipped to [min, max].
+__global__ void __launch_bounds__(256) zoe_attractor_normed_kernel(const __half* __restrict__ apre, int lda, int na, const float* __restrict__ prev,
+                                                                    int B, int h, int w, int H, int W, float sy, float sx, float lo, float span,
+                                                                    float* __restrict__ out, float* __restrict__ sorted) {
+    if (threadIdx.x == 0) NB_PDL_TRIGGER();
+    const long long npix = (long long)B * H * W;
+    const long long pix = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (pix >= npix) return;
+    const int X = (int)(pix % W);
+    const long long r = pix / W;
+    const int Y = (int)(r % H), b = (int)(r / H);
+    const Lerp ly = lerp_ac(Y, sy, h), lx = lerp_ac(X, sx, w);
+    const float* p = prev + (size_t)b * h * w * NBINS + lane;
+    float v[2];
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+        const float c00 = __ldg(p + ((size_t)ly.i0 * w + lx.i0) * NBINS + 32 * j), c01 = __ldg(p + ((size_t)ly.i0 * w + lx.i1) * NBINS + 32 * j);
+        const float c10 = __ldg(p + ((size_t)ly.i1 * w + lx.i0) * NBINS + 32 * j), c11 = __ldg(p + ((size_t)ly.i1 * w + lx.i1) * NBINS + 32 * j);
+        v[j] = ly.l0 * (lx.l0 * c00 + lx.l1 * c01) + ly.l1 * (lx.l0 * c10 + lx.l1 * c11);
+    }
+    const __half* ap = apre + (size_t)pix * lda;
+    float d0 = 0.f, d1 = 0.f;
+    for (int j = 0; j < na; ++j) {
+        const float a = __half2float(__float2half_rn(__half2float(__ldg(ap + 2 * j)) + 1e-3f));
+        const float x0 = a - v[0], x1 = a - v[1];
+        d0 += x0 / (1.f + 300.f * (x0 * x0));       // inv_attractor with its default alpha = 300, gamma = 2 (upstream quirk)
+        d1 += x1 / (1.f + 300.f * (x1 * x1));
+    }
+    v[0] += d0 / (float)na;
+    v[1] += d1 / (float)na;
+    float* o = out + (size_t)pix * NBINS + lane;
+    o[0] = v[0];
+    o[32] = v[1];
+    if (!sorted) return;
+    v[0] = span * v[0] + lo;
+    v[1] = span * v[1] + lo;
+    // bitonic sort of element i = lane + 32 j, ascending
+#pragma unroll
+    for (int k = 2; k <= NBINS; k <<= 1) {
+#pragma unroll
+        for (int s = k >> 1; s > 0; s >>= 1) {
+            if (s == 32) {                          // partner in the other register of this lane (k == 64: ascending)
+                const float a = fminf(v[0], v[1]), c = fmaxf(v[0], v[1]);
+                v[0] = a; v[1] = c;
+            } else {
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    const int i = lane + 32 * j;
+                    const float other = __shfl_xor_sync(0xffffffffu, v[j], s);
+                    const bool keep_min = ((i & s) == 0) == ((i & k) == 0);
+                    v[j] = keep_min ? fminf(v[j], other) : fmaxf(v[j], other);
+                }
+            }
+        }
+    }
+    const float hi = lo + span;
+    float* so = sorted + (size_t)pix * NBINS + lane;
+    so[0] = fminf(fmaxf(v[0], lo), hi);
+    so[32] = fminf(fmaxf(v[1], lo), hi);
+}
+
 // one thread per (pixel, group of 8 channels): groups 0..15 = the resampled embedding, 16..19 = the activation, 20 = relative
 // depth + zeros, 21..23 = zeros (channel order chosen at pack time, zoe_model.inl)
 __global__ void __launch_bounds__(256) zoe_clb_concat_kernel(const __half* __restrict__ act, const float* __restrict__ rel,
@@ -354,6 +446,24 @@ int zoe_attractor(cudaStream_t st, const __half* apre, int lda, int na, const fl
     NB_CHECK(na >= 1 && na <= lda, "bad attractor count");
     const long long total = (long long)B * H * W * NBINS;
     zoe_attractor_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(apre, lda, na, prev_bin, B, h, w, H, W, ac_scale(h, H), ac_scale(w, W), out);
+    NB_LAUNCHED();
+    return 0;
+}
+
+int zoe_seed_normed(cudaStream_t st, const __half* s, long long npix, float min_depth, float max_depth, float* out) {
+    NB_CHECK(max_depth > min_depth, "max_depth must exceed min_depth");
+    zoe_seed_normed_kernel<<<(unsigned)cdiv64(npix * 32, 256), 256, 0, st>>>(s, npix, min_depth, max_depth - min_depth, out);
+    NB_LAUNCHED();
+    return 0;
+}
+
+int zoe_attractor_normed(cudaStream_t st, const __half* apre, int lda, int na, const float* prev_bin, int B, int h, int w, int H, int W,
+                         float min_depth, float max_depth, float* out, float* sorted) {
+    NB_CHECK(na >= 1 && 2 * na <= lda, "bad attractor count");
+    NB_CHECK(max_depth > min_depth, "max_depth must exceed min_depth");
+    const long long npix = (long long)B * H * W;
+    zoe_attractor_normed_kernel<<<(unsigned)cdiv64(npix * 32, 256), 256, 0, st>>>(apre, lda, na, prev_bin, B, h, w, H, W, ac_scale(h, H),
+                                                                                  ac_scale(w, W), min_depth, max_depth - min_depth, out, sorted);
     NB_LAUNCHED();
     return 0;
 }

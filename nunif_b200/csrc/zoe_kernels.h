@@ -24,6 +24,14 @@ int zoe_softplus(cudaStream_t st, const __half* x, float* out, long long n);
 // (apre fp16, row stride lda); out[pix][k] = c_k + mean_j inv_attractor(a_j - c_k), inv_attractor(dx) = dx / (1 + 300 dx^2)
 int zoe_attractor(cudaStream_t st, const __half* apre, int lda, int na, const float* prev_bin, int B, int h, int w, int H, int W,
                   float* out);
+// SeedBinRegressor (normed, ZoeD_Any_K): s fp16 [npix][64] = ReLU'd seed logits -> out fp32 [npix][64] = the bin centres in
+// [0, 1] units, (centres - min) / (max - min), centres = midpoints of the edges min + cumsum((max - min) * w / sum(w)), w = s + 1e-3
+int zoe_seed_normed(cudaStream_t st, const __half* s, long long npix, float min_depth, float max_depth, float* out);
+// AttractorLayer (normed): c = bilinear(align_corners)(prev_bin [B][h][w][64] -> H x W); a_j = apre[pix][2j] + 1e-3 (apre fp16 ReLU'd,
+// row stride lda >= 2 na); out[pix][k] = c_k + mean_j inv_attractor(a_j - c_k).  sorted (may be null): (max - min) out + min, sorted
+// ascending over the 64 bins and clipped to [min, max] (what the last level hands to the log-binomial mixture)
+int zoe_attractor_normed(cudaStream_t st, const __half* apre, int lda, int na, const float* prev_bin, int B, int h, int w, int H, int W,
+                         float min_depth, float max_depth, float* out, float* sorted);
 // ConditionalLogBinomial input: A[pix][0..128) = bilinear(align_corners)(emb [B][h][w][128] -> H x W), [128..160) = act, [160] = rel,
 // [161..192) = 0 (the packed weight uses the same channel order);  act fp16 [B][H][W][32], rel fp32 [B][H][W]
 int zoe_clb_concat(cudaStream_t st, const __half* act, const float* rel, const __half* emb, int B, int h, int w, int H, int W, __half* A);

@@ -1,5 +1,5 @@
 """Mirror of iw3/depth_anything_model.py (DepthAnythingModel / batch_infer, lines 113-253) for the
-Depth-Anything-V2 ViT-S network on the H100 engine.
+Depth-Anything-V2 (Any_V2_S/B/L) and V1 (Any_S/B/L) relative-depth networks on the H100 engine.
 
 The reference obtains the network from torch.hub ("nagadomi/Depth-Anything_iw3:main", DepthAnything(encoder="v2_vits"),
 depth_anything_model.py:223-230); here the same checkpoint (upstream key names ``pretrained.*`` / ``depth_head.*``) is
@@ -15,18 +15,24 @@ from .base_depth_model import BaseDepthModel, HUB_MODEL_DIR
 from .depth_anything_preprocess import batch_preprocess
 from .dilation import dilate_edge, edge_dilation_is_enabled
 
-# NB200_MODEL_DEPTH_ANYTHING_V2_{S,B,L}; model types as in iw3/depth_anything_model.py NAME_MAP
+# NB200_MODEL_DEPTH_ANYTHING_V2_{S,B,L}, NB200_MODEL_DEPTH_ANYTHING_V1_{S,B,L}; model types as in iw3/depth_anything_model.py
+# NAME_MAP.  V1 is the same network with the hooks on the last four blocks.
 KINDS = {"vits": 6, "vitb": 8, "vitl": 9}
-ENCODER_OF = {"Any_V2_S": "vits", "Any_V2_B": "vitb", "Any_V2_L": "vitl"}
+V1_KINDS = {"vits": 20, "vitb": 21, "vitl": 22}
+ENCODER_OF = {"Any_V2_S": "vits", "Any_V2_B": "vitb", "Any_V2_L": "vitl", "Any_S": "vits", "Any_B": "vitb", "Any_L": "vitl"}
+V1_MODELS = {"Any_S", "Any_B", "Any_L"}
+AA_SUPPORTED_MODELS = {"Any_V2_S", "Any_V2_B", "Any_V2_L"}   # depth_anything_model.py:61-65
 
 
 class DepthAnythingNet:
-    """The packed network: ``net(x)`` == ``DepthAnythingV2.forward`` (x: B,3,H,W normalised, H,W % 14 == 0 -> B,H,W)."""
+    """The packed network: ``net(x)`` == ``DepthAnythingV2.forward`` (or the V1 ``DepthAnything.forward`` with ``v1=True``)
+    (x: B,3,H,W normalised, H,W % 14 == 0 -> B,H,W)."""
 
-    def __init__(self, state_dict, device="cuda:0", encoder="vits"):
+    def __init__(self, state_dict, device="cuda:0", encoder="vits", v1=False):
         if encoder not in KINDS:
             raise ValueError(f"encoder: choose from {list(KINDS)}")
         self.encoder = encoder
+        self.v1 = v1
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
@@ -37,7 +43,7 @@ class DepthAnythingNet:
         numels = (ctypes.c_int64 * n)(*[v.numel() for _, v in items])
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().nb200_model_create(KINDS[encoder], n, names, datas, numels, 0, ctypes.byref(h)))
+            _lib.check(_lib.lib().nb200_model_create((V1_KINDS if v1 else KINDS)[encoder], n, names, datas, numels, 0, ctypes.byref(h)))
         self._h = h
         self.metric_depth = False
         self.prep_lower_bound = 392
@@ -93,7 +99,10 @@ def batch_infer(model, im, flip_aug=True, low_vram=False, enable_amp=False, outp
     return z.to(output_device)
 
 
-MODEL_FILES = {   # depth_anything_model.py:37-42 (the relative-depth V2 checkpoints)
+MODEL_FILES = {   # depth_anything_model.py:37-42 (the relative-depth V1 and V2 checkpoints)
+    "Any_S": path.join(HUB_MODEL_DIR, "checkpoints", "depth_anything_vits14.pth"),
+    "Any_B": path.join(HUB_MODEL_DIR, "checkpoints", "depth_anything_vitb14.pth"),
+    "Any_L": path.join(HUB_MODEL_DIR, "checkpoints", "depth_anything_vitl14.pth"),
     "Any_V2_S": path.join(HUB_MODEL_DIR, "checkpoints", "depth_anything_v2_vits.pth"),
     "Any_V2_B": path.join(HUB_MODEL_DIR, "checkpoints", "depth_anything_v2_vitb.pth"),
     "Any_V2_L": path.join(HUB_MODEL_DIR, "checkpoints", "depth_anything_v2_vitl.pth"),
@@ -105,7 +114,7 @@ class DepthAnythingModel(BaseDepthModel):
 
     def __init__(self, model_type="Any_V2_S"):
         if model_type not in ENCODER_OF:
-            raise ValueError(f"the H100 engine implements {list(ENCODER_OF)} (Depth-Anything-V2 relative-depth models)")
+            raise ValueError(f"the H100 engine implements {list(ENCODER_OF)} (Depth-Anything V1 / V2 relative-depth models)")
         super().__init__(model_type)
 
     @classmethod
@@ -124,7 +133,7 @@ class DepthAnythingModel(BaseDepthModel):
         return False
 
     def _wrap(self, state_dict, resolution, device):
-        net = DepthAnythingNet(state_dict, device, encoder=ENCODER_OF[self.model_type])
+        net = DepthAnythingNet(state_dict, device, encoder=ENCODER_OF[self.model_type], v1=self.model_type in V1_MODELS)
         lb = resolution or 392                                        # :232-235 (GUI 512 -> 518)
         if lb % 14 != 0:
             lb += 14 - lb % 14
@@ -148,7 +157,8 @@ class DepthAnythingModel(BaseDepthModel):
         return self
 
     def infer(self, x, tta=False, low_vram=False, enable_amp=True, edge_dilation=0, depth_aa=False, **kwargs):
-        """depth_anything_model.py:241-253."""
+        """depth_anything_model.py:241-253.  The V1 models have no depth_aa (:190-194): ``depth_aa=True`` runs without it."""
+        depth_aa = depth_aa and self.model_type in AA_SUPPORTED_MODELS
         if not enable_amp:
             raise NotImplementedError("nunif_b200 implements the reference's CUDA autocast (fp16) forward only")
         if not torch.is_tensor(x):
@@ -166,7 +176,9 @@ class DepthAnythingModel(BaseDepthModel):
 
     def load_depth_aa(self, state_dict):
         """The learned anti-aliasing filter the reference attaches in load() (:190-194); ``state_dict`` with the keys of
-        `iw3.depth_aa` (the ``state_dict`` entry of iw3_depth_aa_20250530.pth)."""
+        `iw3.depth_aa` (the ``state_dict`` entry of iw3_depth_aa_20250530.pth).  Only the V2 models take it."""
+        if self.model_type not in AA_SUPPORTED_MODELS:
+            raise ValueError(f"depth_aa is attached to {sorted(AA_SUPPORTED_MODELS)} only (depth_anything_model.py:61-65), not {self.model_type}")
         from .depth_aa import DepthAA
         self.depth_aa = DepthAA(state_dict, self.device)
         return self

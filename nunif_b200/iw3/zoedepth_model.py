@@ -8,8 +8,9 @@ same checkpoint (ZoeD_M12_N.pt, upstream key names `core.core.pretrained.*`, `co
 kernels in csrc/depth_kernels.cu / zoe_kernels.cu.  ``infer`` keeps the reference's signature and output convention:
 B,1,h,w (or 1,h,w) float32 on ``x.device`` = the NEGATED metric depth of the unpadded frame (larger = nearer).
 
-Not built: ZoeD_K / ZoeD_NK (two bin heads + the patch-transformer domain classifier) and the Depth-Anything-metric
-checkpoints ZoeD_Any_N / ZoeD_Any_K - `supported()` says so and the constructor raises.
+Not built: ZoeD_K / ZoeD_NK (two bin heads + the patch-transformer domain classifier) - `supported()` says so and the
+constructor raises.  The Depth-Anything-metric checkpoints ZoeD_Any_N / ZoeD_Any_K run through ZoeDepthAnythingModel
+(zoedepth_any_model.py), a subclass that shares this class's loading and ``infer``.
 """
 import ctypes
 from os import path
@@ -37,7 +38,7 @@ class ZoeDepthNet:
     """The packed network: ``net(x)`` == ``ZoeDepth.forward(x)['metric_depth']`` (x: B,3,H,W normalised, H,W % 32 == 0
     -> B,1,H,W metric depth)."""
 
-    def __init__(self, state_dict, device="cuda:0"):
+    def __init__(self, state_dict, device="cuda:0", kind=KIND_ZOEDEPTH_N):
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
@@ -49,7 +50,7 @@ class ZoeDepthNet:
         numels = (ctypes.c_int64 * n)(*[v.numel() for _, v in items])
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().nb200_model_create(KIND_ZOEDEPTH_N, n, names, datas, numels, 0, ctypes.byref(h)))
+            _lib.check(_lib.lib().nb200_model_create(kind, n, names, datas, numels, 0, ctypes.byref(h)))
         self._h = h
         self.metric_depth = True
         self.prep_mod = 32                      # zoedepth_model.py:172-180
@@ -108,10 +109,12 @@ def batch_infer(model, im, flip_aug=True, low_vram=False, enable_amp=False, outp
 
 class ZoeDepthModel(BaseDepthModel):
     """iw3/zoedepth_model.py:151-233 on the engine: the full BaseDepthModel surface (load / infer / EMA normaliser)."""
+    MODEL_FILES = MODEL_FILES
 
     def __init__(self, model_type="ZoeD_N"):
-        if model_type not in MODEL_FILES:
-            raise ValueError(f"the H100 engine implements {list(MODEL_FILES)}; ZoeD_K / ZoeD_NK / ZoeD_Any_* are not built")
+        if not self.supported(model_type):
+            hint = " (ZoeD_Any_N / ZoeD_Any_K: use ZoeDepthAnythingModel or create_depth_model)" if model_type.startswith("ZoeD_Any") else ""
+            raise ValueError(f"{type(self).__name__} implements {sorted(self.MODEL_FILES)}; ZoeD_K / ZoeD_NK are not built{hint}")
         super().__init__(model_type)
 
     @classmethod
@@ -120,11 +123,11 @@ class ZoeDepthModel(BaseDepthModel):
 
     @classmethod
     def supported(cls, model_type):
-        return model_type in MODEL_FILES
+        return model_type in cls.MODEL_FILES
 
     @classmethod
     def get_model_path(cls, model_type):
-        return MODEL_FILES[model_type]
+        return cls.MODEL_FILES[model_type]
 
     def is_metric(self):
         return True

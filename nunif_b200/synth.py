@@ -240,54 +240,59 @@ def depth_anything_v2_state_dict(seed=0, encoder="vits", pos_grid=37):
         return torch.randn(*shape, generator=g) * std
 
     sd = {}
-    sd["pretrained.cls_token"] = rn(1, 1, dim, std=0.02)
-    sd["pretrained.pos_embed"] = rn(1, 1 + pos_grid * pos_grid, dim, std=0.2)
-    sd["pretrained.mask_token"] = torch.zeros(1, dim)
-    sd["pretrained.patch_embed.proj.weight"] = rn(dim, 3, 14, 14, std=1.0 / (3 * 14 * 14) ** 0.5)
-    sd["pretrained.patch_embed.proj.bias"] = rn(dim, std=0.02)
+    _depth_anything_body(sd, rn, "", dim, depth, feat, oc, pos_grid)
+    return sd
+
+
+def _depth_anything_body(sd, rn, pre, dim, depth, feat, oc, pos_grid):
+    """DINOv2 encoder (`pretrained.*`) + Depth-Anything DPT head (`depth_head.*`) under key prefix `pre`."""
+    sd[pre + "pretrained.cls_token"] = rn(1, 1, dim, std=0.02)
+    sd[pre + "pretrained.pos_embed"] = rn(1, 1 + pos_grid * pos_grid, dim, std=0.2)
+    sd[pre + "pretrained.mask_token"] = torch.zeros(1, dim)
+    sd[pre + "pretrained.patch_embed.proj.weight"] = rn(dim, 3, 14, 14, std=1.0 / (3 * 14 * 14) ** 0.5)
+    sd[pre + "pretrained.patch_embed.proj.bias"] = rn(dim, std=0.02)
     for i in range(depth):
         p = f"pretrained.blocks.{i}."
-        sd[p + "norm1.weight"] = 1.0 + rn(dim, std=0.1)
-        sd[p + "norm1.bias"] = rn(dim, std=0.05)
-        sd[p + "attn.qkv.weight"] = rn(3 * dim, dim, std=1.2 / dim ** 0.5)
-        sd[p + "attn.qkv.bias"] = rn(3 * dim, std=0.02)
-        sd[p + "attn.proj.weight"] = rn(dim, dim, std=1.0 / dim ** 0.5)
-        sd[p + "attn.proj.bias"] = rn(dim, std=0.02)
-        sd[p + "ls1.gamma"] = 0.3 + rn(dim, std=0.05)
-        sd[p + "norm2.weight"] = 1.0 + rn(dim, std=0.1)
-        sd[p + "norm2.bias"] = rn(dim, std=0.05)
-        sd[p + "mlp.fc1.weight"] = rn(4 * dim, dim, std=1.0 / dim ** 0.5)
-        sd[p + "mlp.fc1.bias"] = rn(4 * dim, std=0.02)
-        sd[p + "mlp.fc2.weight"] = rn(dim, 4 * dim, std=1.0 / (4 * dim) ** 0.5)
-        sd[p + "mlp.fc2.bias"] = rn(dim, std=0.02)
-        sd[p + "ls2.gamma"] = 0.3 + rn(dim, std=0.05)
-    sd["pretrained.norm.weight"] = 1.0 + rn(dim, std=0.1)
-    sd["pretrained.norm.bias"] = rn(dim, std=0.05)
+        sd[pre + p + "norm1.weight"] = 1.0 + rn(dim, std=0.1)
+        sd[pre + p + "norm1.bias"] = rn(dim, std=0.05)
+        sd[pre + p + "attn.qkv.weight"] = rn(3 * dim, dim, std=1.2 / dim ** 0.5)
+        sd[pre + p + "attn.qkv.bias"] = rn(3 * dim, std=0.02)
+        sd[pre + p + "attn.proj.weight"] = rn(dim, dim, std=1.0 / dim ** 0.5)
+        sd[pre + p + "attn.proj.bias"] = rn(dim, std=0.02)
+        sd[pre + p + "ls1.gamma"] = 0.3 + rn(dim, std=0.05)
+        sd[pre + p + "norm2.weight"] = 1.0 + rn(dim, std=0.1)
+        sd[pre + p + "norm2.bias"] = rn(dim, std=0.05)
+        sd[pre + p + "mlp.fc1.weight"] = rn(4 * dim, dim, std=1.0 / dim ** 0.5)
+        sd[pre + p + "mlp.fc1.bias"] = rn(4 * dim, std=0.02)
+        sd[pre + p + "mlp.fc2.weight"] = rn(dim, 4 * dim, std=1.0 / (4 * dim) ** 0.5)
+        sd[pre + p + "mlp.fc2.bias"] = rn(dim, std=0.02)
+        sd[pre + p + "ls2.gamma"] = 0.3 + rn(dim, std=0.05)
+    sd[pre + "pretrained.norm.weight"] = 1.0 + rn(dim, std=0.1)
+    sd[pre + "pretrained.norm.bias"] = rn(dim, std=0.05)
     for i, c in enumerate(oc):
-        sd[f"depth_head.projects.{i}.weight"] = rn(c, dim, 1, 1, std=1.0 / dim ** 0.5)
-        sd[f"depth_head.projects.{i}.bias"] = rn(c, std=0.02)
-        sd[f"depth_head.scratch.layer{i + 1}_rn.weight"] = rn(feat, c, 3, 3, std=1.0 / (9 * c) ** 0.5)
-    sd["depth_head.resize_layers.0.weight"] = rn(oc[0], oc[0], 4, 4, std=1.0 / oc[0] ** 0.5)
-    sd["depth_head.resize_layers.0.bias"] = rn(oc[0], std=0.02)
-    sd["depth_head.resize_layers.1.weight"] = rn(oc[1], oc[1], 2, 2, std=1.0 / oc[1] ** 0.5)
-    sd["depth_head.resize_layers.1.bias"] = rn(oc[1], std=0.02)
-    sd["depth_head.resize_layers.3.weight"] = rn(oc[3], oc[3], 3, 3, std=1.0 / (9 * oc[3]) ** 0.5)
-    sd["depth_head.resize_layers.3.bias"] = rn(oc[3], std=0.02)
+        sd[pre + f"depth_head.projects.{i}.weight"] = rn(c, dim, 1, 1, std=1.0 / dim ** 0.5)
+        sd[pre + f"depth_head.projects.{i}.bias"] = rn(c, std=0.02)
+        sd[pre + f"depth_head.scratch.layer{i + 1}_rn.weight"] = rn(feat, c, 3, 3, std=1.0 / (9 * c) ** 0.5)
+    sd[pre + "depth_head.resize_layers.0.weight"] = rn(oc[0], oc[0], 4, 4, std=1.0 / oc[0] ** 0.5)
+    sd[pre + "depth_head.resize_layers.0.bias"] = rn(oc[0], std=0.02)
+    sd[pre + "depth_head.resize_layers.1.weight"] = rn(oc[1], oc[1], 2, 2, std=1.0 / oc[1] ** 0.5)
+    sd[pre + "depth_head.resize_layers.1.bias"] = rn(oc[1], std=0.02)
+    sd[pre + "depth_head.resize_layers.3.weight"] = rn(oc[3], oc[3], 3, 3, std=1.0 / (9 * oc[3]) ** 0.5)
+    sd[pre + "depth_head.resize_layers.3.bias"] = rn(oc[3], std=0.02)
     for r in (1, 2, 3, 4):
         p = f"depth_head.scratch.refinenet{r}."
-        sd[p + "out_conv.weight"] = rn(feat, feat, 1, 1, std=1.0 / feat ** 0.5)
-        sd[p + "out_conv.bias"] = rn(feat, std=0.02)
+        sd[pre + p + "out_conv.weight"] = rn(feat, feat, 1, 1, std=1.0 / feat ** 0.5)
+        sd[pre + p + "out_conv.bias"] = rn(feat, std=0.02)
         for u in (1, 2):
             for cv in (1, 2):
-                sd[p + f"resConfUnit{u}.conv{cv}.weight"] = rn(feat, feat, 3, 3, std=0.7 / (9 * feat) ** 0.5)
-                sd[p + f"resConfUnit{u}.conv{cv}.bias"] = rn(feat, std=0.02)
-    sd["depth_head.scratch.output_conv1.weight"] = rn(feat // 2, feat, 3, 3, std=1.0 / (9 * feat) ** 0.5)
-    sd["depth_head.scratch.output_conv1.bias"] = rn(feat // 2, std=0.02)
-    sd["depth_head.scratch.output_conv2.0.weight"] = rn(32, feat // 2, 3, 3, std=1.4 / (9 * feat // 2) ** 0.5)
-    sd["depth_head.scratch.output_conv2.0.bias"] = 0.2 + rn(32, std=0.05)
-    sd["depth_head.scratch.output_conv2.2.weight"] = rn(1, 32, 1, 1, std=1.0 / 32 ** 0.5).abs()
-    sd["depth_head.scratch.output_conv2.2.bias"] = torch.full((1,), 0.3)
-    return sd
+                sd[pre + p + f"resConfUnit{u}.conv{cv}.weight"] = rn(feat, feat, 3, 3, std=0.7 / (9 * feat) ** 0.5)
+                sd[pre + p + f"resConfUnit{u}.conv{cv}.bias"] = rn(feat, std=0.02)
+    sd[pre + "depth_head.scratch.output_conv1.weight"] = rn(feat // 2, feat, 3, 3, std=1.0 / (9 * feat) ** 0.5)
+    sd[pre + "depth_head.scratch.output_conv1.bias"] = rn(feat // 2, std=0.02)
+    sd[pre + "depth_head.scratch.output_conv2.0.weight"] = rn(32, feat // 2, 3, 3, std=1.4 / (9 * feat // 2) ** 0.5)
+    sd[pre + "depth_head.scratch.output_conv2.0.bias"] = 0.2 + rn(32, std=0.05)
+    sd[pre + "depth_head.scratch.output_conv2.2.weight"] = rn(1, 32, 1, 1, std=1.0 / 32 ** 0.5).abs()
+    sd[pre + "depth_head.scratch.output_conv2.2.bias"] = torch.full((1,), 0.3)
 
 
 def row_flow_v3_state_dict(seed=0):
@@ -499,19 +504,61 @@ def zoedepth_state_dict(seed=0, cfg=None):
     conv(sc + "output_conv.2", 32, feat // 2, 3, gain=1.4, bias=0.05, bias_mean=0.2)
     sd[sc + "output_conv.4.weight"] = rn(1, 32, 1, 1, std=1.0 / 32 ** 0.5).abs()
     sd[sc + "output_conv.4.bias"] = torch.full((1,), 0.3)
-    # bins head (zoedepth_v1.py): conv2, SeedBinRegressorUnnormed (mlp_dim 256), Projector (mlp_dim 128), AttractorLayerUnnormed
+    _zoe_bins_head(conv, feat, normed=False)
+    return sd
+
+
+def _zoe_bins_head(conv, feat, normed):
+    """The ZoeDepth bins head (zoedepth_v1.py): conv2, the seed regressor (mlp_dim 256), Projectors (mlp_dim 128), the
+    attractor layers, the conditional log-binomial.  softplus head (SeedBinRegressorUnnormed / AttractorLayerUnnormed):
+    logits around 1.  normed head (SeedBinRegressor / AttractorLayer, both ReLU'd): seed logits of which about a third
+    are cut to 0 by the ReLU, so the bin widths span 1e-3 .. ~3 and bins crowd together; attractor points (the first of
+    each output pair) spread over [0, 1], the range of the normalised centres, so that every level moves the bins."""
     conv("conv2", feat, feat, 1)
     conv("seed_bin_regressor._net.0", 256, feat, 1, gain=1.4)
-    conv("seed_bin_regressor._net.2", 64, 256, 1, gain=2.0, bias=1.0, bias_mean=1.0)
+    if normed:
+        conv("seed_bin_regressor._net.2", 64, 256, 1, gain=2.0, bias=0.5, bias_mean=0.5)
+    else:
+        conv("seed_bin_regressor._net.2", 64, 256, 1, gain=2.0, bias=1.0, bias_mean=1.0)
     conv("seed_projector._net.0", 128, feat, 1, gain=1.4)
     conv("seed_projector._net.2", 128, 128, 1, gain=1.4)
     for i, na in enumerate((16, 8, 4, 1)):
         conv(f"projectors.{i}._net.0", 128, feat, 1, gain=1.4)
         conv(f"projectors.{i}._net.2", 128, 128, 1, gain=1.4)
         conv(f"attractors.{i}._net.0", 128, 128, 1, gain=1.4)
-        conv(f"attractors.{i}._net.2", na, 128, 1, gain=2.0, bias=1.0, bias_mean=1.0)
+        if normed:
+            conv(f"attractors.{i}._net.2", 2 * na, 128, 1, gain=0.5, bias=0.3, bias_mean=0.5)
+        else:
+            conv(f"attractors.{i}._net.2", na, 128, 1, gain=2.0, bias=1.0, bias_mean=1.0)
     conv("conditional_log_binomial.mlp.0", (33 + 128) // 2, 33 + 128, 1, gain=1.4)
     conv("conditional_log_binomial.mlp.2", 4, (33 + 128) // 2, 1, gain=2.0, bias=0.5)
+
+
+# ZoeD_Any (Depth-Anything metric depth): ViT-L/14 encoder + Depth-Anything DPT head; the reduced test configuration keeps
+# head dim 64 and every width the engine needs a multiple of 32 / 64
+ZOED_ANY = dict(dim=1024, depth=24, feat=256, oc=(256, 512, 1024, 1024), pos_grid=37)
+ZOED_ANY_MINI = dict(dim=256, depth=4, feat=128, oc=(64, 128, 256, 256), pos_grid=6)
+
+
+def zoedepth_any_state_dict(seed=0, cfg=None, normed=False):
+    """Seeded ZoeD_Any_N (normed=False) / ZoeD_Any_K (normed=True) weights with the upstream key names
+    (depth_anything_metric_depth_{indoor,outdoor}.pt: `core.core.pretrained.*` = DINOv2, `core.core.depth_head.*` = the
+    Depth-Anything DPT head, the rest = the ZoeDepth bins head).  `cfg`: ZOED_ANY (default) or ZOED_ANY_MINI.  The
+    encoder and head use the gains of depth_anything_v2_state_dict."""
+    cfg = cfg or ZOED_ANY
+    dim, depth, feat, oc, grid = cfg["dim"], cfg["depth"], cfg["feat"], cfg["oc"], cfg["pos_grid"]
+    g = torch.Generator().manual_seed(50_000 + seed + (1000 if normed else 0))
+
+    def rn(*shape, std=1.0):
+        return torch.randn(*shape, generator=g) * std
+
+    def conv(name, cout, cin, k, gain=1.0, bias=0.02, bias_mean=0.0):
+        sd[name + ".weight"] = rn(cout, cin, k, k, std=gain / (cin * k * k) ** 0.5)
+        sd[name + ".bias"] = bias_mean + rn(cout, std=bias)
+
+    sd = {}
+    _depth_anything_body(sd, rn, "core.core.", dim, depth, feat, oc, grid)
+    _zoe_bins_head(conv, feat, normed)
     return sd
 
 
