@@ -108,7 +108,11 @@ enum {
      * last four blocks; checkpoints depth_anything_vit{s,b,l}14.pth.  Run through nb200_depth_anything_forward. */
     NB200_MODEL_DEPTH_ANYTHING_V1_S = 20,
     NB200_MODEL_DEPTH_ANYTHING_V1_B = 21,
-    NB200_MODEL_DEPTH_ANYTHING_V1_L = 22
+    NB200_MODEL_DEPTH_ANYTHING_V1_L = 22,
+    /* TransNetV2, the shot-boundary network of iw3's --scene-detect (nunif/utils/transnetv2.py, F=16 L=3 S=2 D=1024); keys
+     * `SDDCNN.*`, `frame_sim_layer.*`, `color_hist_layer.fc.*`, `fc1.*`, `cls_layer1.*`, `cls_layer2.*`.  Every BatchNorm is
+     * folded into its branch's temporal conv.  Run through nb200_transnetv2_forward. */
+    NB200_MODEL_TRANSNET_V2 = 23
 };
 
 /* Create a model from named fp32 host tensors using the reference's state_dict
@@ -244,6 +248,12 @@ int nb200_sod_forward(nb200_model* m, const float* rgb, int B, int H, int W, con
                       float* depth192, void* stream);
 int nb200_sod_position(const float* saliency, const float* depth, int B, int n, double pos, float* out, void* stream);
 int nb200_sod_ema(float* state, const float* z, int B, const int* reset_host, double decay, float* out, void* stream);
+
+/* TransNetV2.forward (nunif/utils/transnetv2.py:49-87) of a NB200_MODEL_TRANSNET_V2 model on B windows of T frames each
+ * (T >= 1; each window is zero-padded in time on its own, as a separate batch entry of the reference):
+ *   x [B][T][3][27][48] fp32 (any scale; the colour histograms truncate it to int) -> one_hot [B][T], many_hot [B][T] fp32
+ *   logits.  No host synchronisation.  Debug taps 200..205 (DESIGN.md §5). */
+int nb200_transnetv2_forward(nb200_model* m, const float* x, int B, int T, float* one_hot, float* many_hot, void* stream);
 
 /* AlphaBorderPadding.forward (nunif/utils/alpha.py:32-57): rgb [3][H][W], alpha [1][H][W] fp32 ->
  * out [3][H][W]: transparent pixels are filled from their opaque neighbours, `offset` rounds
@@ -421,7 +431,8 @@ int nb200_equirectangular(const float* c, int C, int H, int W, float* out, void*
 int nb200_tune_set(int key, int value);   /* kernel-selection knobs (csrc/gemm.cu g_tune), for tests and A/B runs */
 int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermediate `id` of nb200_zoedepth_forward (ids 0..14,
                                                                15 = the sorted centres of a normed head, DESIGN.md §5)
-                                                               or nb200_light_inpaint (ids 100..173, DESIGN.md §5) to dev_buf */
+                                                               or nb200_light_inpaint (ids 100..173, DESIGN.md §5)
+                                                               or nb200_transnetv2_forward (ids 200..205) to dev_buf */
 int nb200_profile_enable(int on);
 int nb200_profile_report(char* buf, size_t cap);
 int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launch: class,ms,work,read_bytes,write_bytes */

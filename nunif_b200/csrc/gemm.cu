@@ -126,6 +126,16 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
             strides[3] = is;
             break;
         }
+        case CG_TCONV3: {
+            NB_CHECK(g.dil >= 1 && g.dil <= 127, "temporal dilation must be in [1, 127]");
+            p.B = g.B; p.Ho = g.Hi; p.Wo = g.Wi; p.TH = 8; p.TW = 16;
+            p.taps = 3; ktap = g.Cin;
+            for (int t = 0; t < 3; ++t) { p.tap_dy[t] = (int8_t)((t - 1) * g.dil); p.tap_dx[t] = 0; p.tap_dyi[t] = 0; }
+            dims[0] = g.Cin; dims[1] = g.Wi; dims[2] = 1; dims[3] = g.Hi; dims[4] = g.B;
+            strides[0] = g.Ci * e; strides[1] = rs; strides[2] = rs;
+            strides[3] = is;
+            break;
+        }
         case CG_DOWN2: {
             NB_CHECK(g.Hi % 2 == 0 && g.Wi % 2 == 0, "2x2 stride-2 conv needs even H and W");
             NB_CHECK(g.Cin == g.Ci, "2x2 stride-2 conv needs a dense channel dimension");
@@ -225,7 +235,7 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
     const int m_tiles = p.tiles_x * p.tiles_y * p.B;
     const double Mrows = (double)p.B * p.Ho * p.Wo;
     // algorithmic HBM traffic: the input region once (taps re-read from L2), the residual, the output
-    const double in_px = g.kind == CG_DOWN2 ? 4.0 * Mrows : (g.kind == CG_CONV3 ? (double)p.B * g.Hi * g.Wi : Mrows);
+    const double in_px = g.kind == CG_DOWN2 ? 4.0 * Mrows : ((g.kind == CG_CONV3 || g.kind == CG_TCONV3) ? (double)p.B * g.Hi * g.Wi : Mrows);
     ProfScope ps(st, PC_GEMM, 2.0 * Mrows * (double)g.N * (double)K,
                  in_px * (g.kind == CG_LINEAR_FLAT ? g.Cin * g.a_planes : g.Cin) * 2.0 + (g.res ? Mrows * g.N * 2.0 : 0.0) + (double)g.N * K * 2.0,
                  Mrows * (double)g.N * 2.0);

@@ -4,7 +4,9 @@
 
 namespace nb200 {
 
-enum : int { CG_LINEAR_FLAT = 0, CG_LINEAR_2D = 1, CG_CONV3 = 2, CG_DOWN2 = 3 };
+// CG_TCONV3: a (3,1,1) convolution over time with dilation `dil` and zero padding `dil`; A is viewed as [B][T = Hi][Wi][Ci]
+// (Wi = the pixels of one frame), taps t - dil, t, t + dil
+enum : int { CG_LINEAR_FLAT = 0, CG_LINEAR_2D = 1, CG_CONV3 = 2, CG_DOWN2 = 3, CG_TCONV3 = 5 };
 
 struct ConvGemm {
     const __half* A = nullptr;  // NHWC fp16 activations [B][Hi][Wi][Ci]
@@ -15,6 +17,7 @@ struct ConvGemm {
     long long a_img_stride = 0; // elements between images     (0 = Hi*a_row_stride)
     int kind = CG_LINEAR_FLAT;
     int pad = 0;                // CG_CONV3: zero padding (0 = valid conv, 1 = 'same'); the halo comes from the TMA's out-of-bounds zero fill
+    int dil = 1;                // CG_TCONV3: temporal dilation (1..127); the time padding is the same out-of-bounds zero fill
     const __half* Wt = nullptr; // packed weights [N][taps*Cin_tap], K ordered (ky, kx, c)
     int N = 0;
     const float* bias = nullptr;

@@ -15,6 +15,7 @@
 #include "inpaint_kernels.h"
 #include "window_mha.h"
 #include "sod_kernels.h"
+#include "transnet_kernels.h"
 #include "../../include/nunif_b200.h"
 #include <map>
 #include <vector>
@@ -248,6 +249,7 @@ struct nb200_model {
     std::shared_ptr<InpW> inp;
     std::shared_ptr<Rf2W> rf2;
     std::shared_ptr<SodW> sod;
+    std::shared_ptr<TnW> tn;
     uint8_t* ws = nullptr;
     size_t ws_bytes = 0;
     cudaStream_t copy_stream = nullptr;   // D2H side stream of nb200_tiled_render_host
@@ -475,8 +477,9 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
 
 #include "cunet_model.inl"
 #include "legacy_model.inl"
-// debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth or light_inpaint_v1 forward is copied to `g_tap_buf`
-// (ZoeDepth ids 0..15 in zoe_model.inl; light_inpaint_v1 ids 100..173, table in DESIGN.md §5)
+// debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth, light_inpaint_v1 or TransNetV2 forward is copied to
+// `g_tap_buf` (ZoeDepth ids 0..15 in zoe_model.inl; light_inpaint_v1 ids 100..173, table in DESIGN.md §5; TransNetV2 ids
+// 200..205 in transnet_model.inl)
 static int g_tap_id = -1;
 static void* g_tap_buf = nullptr;
 static size_t g_tap_cap = 0;
@@ -496,6 +499,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 #include "zoe_model.inl"
 #include "inpaint_model.inl"
 #include "sod_model.inl"
+#include "transnet_model.inl"
 
 // ---------------------------------------------------------------------------------------------
 // C ABI
@@ -503,7 +507,7 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
 extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* names, const float* const* data,
                                   const int64_t* numel, int no_clip, nb200_model** out) {
     NB_CHECK(out && names && data && numel, "null pointer");
-    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_DEPTH_ANYTHING_V1_L, "unknown model kind");
+    NB_CHECK(kind >= NB200_MODEL_UPCUNET && kind <= NB200_MODEL_TRANSNET_V2, "unknown model kind");
     int dev = 0;
     NB_CUDA(cudaGetDevice(&dev));
     if (nb200_check_device(dev)) return 1;
@@ -545,6 +549,7 @@ extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* na
         case NB200_MODEL_DEPTH_ANYTHING_V1_S: m->da = pack_depth_anything(pk, 0, "", true); m->scale = 1; break;     // depth_anything_model.py:36-38
         case NB200_MODEL_DEPTH_ANYTHING_V1_B: m->da = pack_depth_anything(pk, 1, "", true); m->scale = 1; break;
         case NB200_MODEL_DEPTH_ANYTHING_V1_L: m->da = pack_depth_anything(pk, 2, "", true); m->scale = 1; break;
+        case NB200_MODEL_TRANSNET_V2: m->tn = pack_transnet(pk); m->scale = 1; break;                                    // transnetv2.py:7-47
     }
     if (pk.err.empty())
         for (auto& kv : pk.src)
@@ -846,6 +851,14 @@ extern "C" int nb200_sod_forward(nb200_model* m, const float* rgb, int B, int H,
     NB_CHECK(m->kind == NB200_MODEL_SOD_V1 && m->sod, "model is not iw3.sod_v1");
     NB_CHECK(B > 0 && H > 0 && W > 0 && h > 0 && w > 0, "bad shape");
     return sod_forward((cudaStream_t)stream, m->blob, *m->sod, rgb, B, H, W, depth, h, w, saliency, depth192);
+}
+
+// TransNetV2.forward (nunif/utils/transnetv2.py:49-87) on B windows of T frames: the one_hot and many_hot logits
+extern "C" int nb200_transnetv2_forward(nb200_model* m, const float* x, int B, int T, float* one_hot, float* many_hot, void* stream) {
+    NB_CHECK(m && x && one_hot && many_hot, "null pointer");
+    NB_CHECK(m->kind == NB200_MODEL_TRANSNET_V2 && m->tn, "model is not TransNetV2");
+    NB_CHECK(B > 0 && T > 0 && (long long)B * T <= (1 << 20), "bad shape");
+    return transnet_forward(m, (cudaStream_t)stream, x, B, T, one_hot, many_hot);
 }
 
 // iw3/dilation.py:67-98: n = max(round(W / base_width * n_iter), 1) (Python's round: half to even), 0 when n_iter <= 0

@@ -646,3 +646,101 @@ def sod_v1_state_dict(seed=0):
     sd["u2netp.outconv.weight"] = (0.5 + torch.rand(1, 6, 1, 1, generator=g)) / 3
     sd["u2netp.outconv.bias"] = torch.tensor([SOD_OUT_BIAS])
     return sd
+
+
+# ----------------------------------------------------------------------------
+# TransNetV2 (nunif/utils/transnetv2.py, F=16 L=3 S=2 D=1024), iw3's --scene-detect
+# ----------------------------------------------------------------------------
+
+# the cls_layer1 bias of transnetv2_state_dict: with it 19 % of the frames of the golden sequences have a boundary
+# probability above 0.5 (oracle/gen_golden_transnetv2.py prints the share)
+TRANSNET_CLS_BIAS = 0.35
+TRANSNET_DILATIONS = (1, 2, 4, 8)
+
+
+def transnetv2_keys():
+    """The state_dict key names of TransNetV2() in the order its modules register them."""
+    keys = []
+    for s in range(3):
+        for j in range(2):
+            p = f"SDDCNN.{s}.DDCNN.{j}"
+            keys += [f"{p}.Conv3D_{d}.layers.{k}.weight" for d in TRANSNET_DILATIONS for k in (0, 1)]
+            keys += [f"{p}.bn.{n}" for n in ("weight", "bias", "running_mean", "running_var", "num_batches_tracked")]
+    for p in ("frame_sim_layer.projection", "frame_sim_layer.fc", "color_hist_layer.fc", "fc1", "cls_layer1", "cls_layer2"):
+        keys += [p + ".weight", p + ".bias"]
+    return keys
+
+
+def transnetv2_state_dict(seed=0):
+    """Seeded weights with the key names of TransNetV2().  Every BatchNorm has non-trivial statistics; the gains keep the
+    stack activations O(1) and the logits spread over a few units, and TRANSNET_CLS_BIAS sets the share of boundaries."""
+    g = torch.Generator().manual_seed(70_000 + seed)
+    sd = {}
+    for s in range(3):
+        F = 16 << s
+        for j in range(2):
+            cin = 4 * F if j == 1 else (3 if s == 0 else 2 * F)
+            p = f"SDDCNN.{s}.DDCNN.{j}"
+            for d in TRANSNET_DILATIONS:
+                sd[f"{p}.Conv3D_{d}.layers.0.weight"] = torch.randn(2 * F, cin, 1, 3, 3, generator=g) * (2.0 / (9 * cin)) ** 0.5
+                sd[f"{p}.Conv3D_{d}.layers.1.weight"] = torch.randn(F, 2 * F, 3, 1, 1, generator=g) * (1.0 / (3 * 2 * F)) ** 0.5
+            sd[f"{p}.bn.weight"] = 0.8 + 0.4 * torch.rand(4 * F, generator=g)
+            sd[f"{p}.bn.bias"] = torch.randn(4 * F, generator=g) * 0.05
+            sd[f"{p}.bn.running_mean"] = torch.randn(4 * F, generator=g) * 0.05
+            sd[f"{p}.bn.running_var"] = 0.3 + 0.7 * torch.rand(4 * F, generator=g)
+            sd[f"{p}.bn.num_batches_tracked"] = torch.tensor(1000, dtype=torch.int64)
+    _linear(sd, g, "frame_sim_layer.projection", 128, 448, gain=4.0)
+    _linear(sd, g, "frame_sim_layer.fc", 128, 101, gain=1.4)
+    _linear(sd, g, "color_hist_layer.fc", 128, 101, gain=1.4)
+    _linear(sd, g, "fc1", 1024, 4864, gain=1.4)
+    _linear(sd, g, "cls_layer1", 1, 1024, gain=0.5)
+    _linear(sd, g, "cls_layer2", 1, 1024, gain=0.5)
+    sd["cls_layer1.bias"] = torch.tensor([TRANSNET_CLS_BIAS])
+    return {k: sd[k] for k in transnetv2_keys()}
+
+
+def shot_sequence(seed, n, use_16bit=False):
+    """A seeded 27 x 48 video of n frames, HWC uint8 (or uint16): shots of moving gradients and blobs, hard cuts between
+    most shots and one cross-dissolve of 8 frames."""
+    g = torch.Generator().manual_seed(80_000 + seed)
+    yy, xx = torch.meshgrid(torch.arange(27.0), torch.arange(48.0), indexing="ij")
+
+    def shot():
+        base = torch.rand(3, generator=g)
+        grad = (torch.rand(3, 2, generator=g) - 0.5) * 0.04
+        c = torch.rand(2, generator=g) * torch.tensor([27.0, 48.0])
+        v = (torch.rand(2, generator=g) - 0.5) * 3.0
+        col = torch.rand(3, generator=g)
+        r = 4.0 + 6.0 * float(torch.rand(1, generator=g))
+
+        def frame(t):
+            img = base.view(3, 1, 1) + grad[:, 0].view(3, 1, 1) * yy + grad[:, 1].view(3, 1, 1) * (xx + 2.0 * t)
+            cy, cx = c + v * t
+            blob = torch.exp(-((yy - cy) ** 2 + (xx - cx) ** 2) / (r * r))
+            return img * (1 - blob) + col.view(3, 1, 1) * blob
+        return frame
+
+    frames, t, cur = [], 0, shot()
+    length = int(torch.randint(12, 40, (1,), generator=g))
+    dissolve_at = n // 2
+    for i in range(n):
+        if t >= length:
+            nxt = shot()
+            if abs(i - dissolve_at) < 20 and dissolve_at >= 0:
+                for k in range(8):
+                    if len(frames) < n:
+                        a = (k + 1) / 9.0
+                        frames.append(cur(t + k) * (1 - a) + nxt(k) * a)
+                dissolve_at = -1
+            cur, t = nxt, 0
+            length = int(torch.randint(12, 40, (1,), generator=g))
+        if len(frames) >= n:
+            break
+        frames.append(cur(t))
+        t += 1
+    x = torch.stack(frames[:n]).clamp(0, 1).permute(0, 2, 3, 1)
+    noise = torch.rand(x.shape, generator=g) * 0.02
+    x = (x + noise).clamp(0, 1)
+    if use_16bit:
+        return (x * 65535).round().to(torch.int32).numpy().astype("uint16")
+    return (x * 255).round().to(torch.uint8).numpy()
