@@ -364,6 +364,13 @@ int nb200_conv_gemm_f16(const void* A, int B, int Hi, int Wi, int Ci, int Cin, i
                         int out_mode, int cout, const void* res, int ldr, int res_H, int res_W,
                         int res_cy, int res_cx, int res_before_act, void* stream);
 
+/* kind 1 with out_mode 1 and, instead of a residual, a second A operand A2 [B][2 Hi][2 Wi][ld2] fp16: output pixel
+ * (2y+dy, 2x+dx) also multiplies the first Cin2 channels of A2 at that pixel with K columns [Ci, Ci + Cin2) of
+ * Wt [N][Ci + Cin2] (a Linear of the skip tensor folded into the GEMM).  cout must be a multiple of 64 or 96. */
+int nb200_conv_gemm_pixshuf_a2_f16(const void* A, int B, int Hi, int Wi, int Ci, const void* Wt, int N,
+                                   const float* bias, int act, void* out, int ldo, int cout, const void* A2,
+                                   int Cin2, int ld2, void* stream);
+
 /* shifted-window attention core between the qkv and proj Linears
  * (torchvision swin_transformer.py:166-221), window 6x6, 6 heads.
  * qkv: three dense planes q | k | v, each [B][H][W][C] fp16 (how the engine's qkv GEMM writes them)

@@ -113,6 +113,8 @@ SIGNATURES = {
     "nb200_conv_gemm_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
                                     c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),
+    "nb200_conv_gemm_pixshuf_a2_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                               c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
     "nb200_tune_set": (c_int, [c_int, c_int]),
     "nb200_debug_tap": (c_int, [c_int, c_void_p, ctypes.c_size_t]),
     "nb200_profile_enable": (c_int, [c_int]),

@@ -40,10 +40,10 @@ int encode(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, c
     return 0;
 }
 
-template <int BN, int BK>
+template <int BN, int BK, bool A2 = false>
 static int launch_t(cudaStream_t st, const GemmMaps& maps, const GemmParams& p, int m_tiles, int n_tiles) {
     using Cfg = GemmCfg<BN, BK>;
-    if (ensure_dyn_smem((const void*)gemm_conv_kernel<BN, BK>, Cfg::SMEM_BYTES)) return 1;
+    if (ensure_dyn_smem((const void*)gemm_conv_kernel<BN, BK, A2>, Cfg::SMEM_BYTES)) return 1;
     // programmatic dependent launch: this grid may be scheduled while the previous kernel of the stream drains (that kernel
     // executes griddepcontrol.launch_dependents); barrier set-up and tensor-map prefetch then overlap the predecessor's tail,
     // and the producer warp blocks in griddepcontrol.wait before the first load.
@@ -54,13 +54,18 @@ static int launch_t(cudaStream_t st, const GemmMaps& maps, const GemmParams& p, 
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    NB_CUDA(cudaLaunchKernelEx(&cfg, gemm_conv_kernel<BN, BK>, maps, p));
+    NB_CUDA(cudaLaunchKernelEx(&cfg, gemm_conv_kernel<BN, BK, A2>, maps, p));
     NB_LAUNCHED();
     return 0;
 }
 
 template <int BK>
 static int launch_bn(int bn, cudaStream_t st, const GemmMaps& maps, const GemmParams& p, int m_tiles, int n_tiles) {
+    if (p.k2) switch (bn) {
+        case 64: return launch_t<64, BK, true>(st, maps, p, m_tiles, n_tiles);
+        case 96: return launch_t<96, BK, true>(st, maps, p, m_tiles, n_tiles);
+        default: return fail("second A operand: unsupported BLOCK_N");
+    }
     switch (bn) {
         case 16: return launch_t<16, BK>(st, maps, p, m_tiles, n_tiles);
         case 32: return launch_t<32, BK>(st, maps, p, m_tiles, n_tiles);
@@ -150,8 +155,14 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
         default: return fail("conv_gemm: unknown kind");
     }
     NB_CHECK(ktap % 32 == 0, "K per tap must be a multiple of 32");
-    const int BK = (ktap % 64 == 0) ? 64 : 32;
+    const bool a2 = g.A2 != nullptr;
+    if (a2) {
+        NB_CHECK(g.out_mode == OUT_PIXSHUF2 && !g.res, "a second A operand needs the pixel-shuffle output and no residual");
+        NB_CHECK(g.Cin2 > 0 && g.Cin2 % 32 == 0 && g.Cin2 <= g.ld2 && g.ld2 % 8 == 0, "second A operand: bad channel count");
+    }
+    const int BK = (ktap % 64 == 0 && g.Cin2 % 64 == 0) ? 64 : 32;
     p.cpt = ktap / BK;
+    p.k2 = a2 ? g.Cin2 / BK : 0;
     p.tiles_x = cdiv(p.Wo, p.TW);
     p.tiles_y = cdiv(p.Ho, p.TH);
     p.N = g.N;
@@ -175,7 +186,9 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
     static const int cands[] = {128, 96, 64, 48, 32, 16};
     for (int c : cands) {
         const int w = (c % 64 == 0) ? 64 : ((c % 32 == 0) ? 32 : 16);
-        if (g.N % c == 0 && (!shuf || g.cout % w == 0) && (!split || g.cout % c == 0)) { bn = c; cw = w; break; }
+        if (g.N % c == 0 && (!shuf || g.cout % w == 0) && (!split || g.cout % c == 0) && (!a2 || ((c == 96 || c == 64) && g.cout % c == 0))) {
+            bn = c; cw = w; break;
+        }
     }
     NB_CHECK(bn > 0, "no BLOCK_N divides N");
     if (!shuf) {
@@ -196,7 +209,7 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
     GemmMaps maps;
     memset(&maps, 0, sizeof(maps));
     if (encode(&maps.a, g.A, 5, dims, strides, box, BK * 2)) return 1;
-    const int K = p.taps * ktap;
+    const int K = p.taps * ktap + (a2 ? g.Cin2 : 0);
     cuuint64_t bdims[2] = {(cuuint64_t)K, (cuuint64_t)g.N};
     cuuint64_t bstr[1] = {(cuuint64_t)K * e};
     cuuint32_t bbox[2] = {(cuuint32_t)BK, (cuuint32_t)bn};
@@ -231,13 +244,22 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
             }
         }
         p.res_cx = p.res_cy = 0;
+        if (a2) {
+            // (c, dx, x, dy, b*Ho + y) over [B][2 Ho][2 Wo][ld2]: an image is Ho rows of the (dy, y) pair, so b and y merge
+            const cuuint64_t px = (cuuint64_t)g.ld2 * e;
+            cuuint64_t d2[5] = {(cuuint64_t)g.Cin2, 2, (cuuint64_t)p.Wo, 2, (cuuint64_t)p.B * p.Ho};
+            cuuint64_t s2[4] = {px, 2 * px, (cuuint64_t)OW * px, 2 * (cuuint64_t)OW * px};
+            cuuint32_t b2[5] = {(cuuint32_t)BK, 1, (cuuint32_t)p.TW, 1, (cuuint32_t)p.TH};
+            if (encode(&maps.a2, g.A2, 5, d2, s2, b2, BK * 2)) return 1;
+        }
     }
     const int m_tiles = p.tiles_x * p.tiles_y * p.B;
     const double Mrows = (double)p.B * p.Ho * p.Wo;
     // algorithmic HBM traffic: the input region once (taps re-read from L2), the residual, the output
     const double in_px = g.kind == CG_DOWN2 ? 4.0 * Mrows : ((g.kind == CG_CONV3 || g.kind == CG_TCONV3) ? (double)p.B * g.Hi * g.Wi : Mrows);
     ProfScope ps(st, PC_GEMM, 2.0 * Mrows * (double)g.N * (double)K,
-                 in_px * (g.kind == CG_LINEAR_FLAT ? g.Cin * g.a_planes : g.Cin) * 2.0 + (g.res ? Mrows * g.N * 2.0 : 0.0) + (double)g.N * K * 2.0,
+                 in_px * (g.kind == CG_LINEAR_FLAT ? g.Cin * g.a_planes : g.Cin) * 2.0 + (g.res ? Mrows * g.N * 2.0 : 0.0) +
+                     4.0 * Mrows * g.Cin2 * (a2 ? 2.0 : 0.0) + (double)g.N * K * 2.0,
                  Mrows * (double)g.N * 2.0);
     return BK == 64 ? launch_bn<64>(bn, st, maps, p, m_tiles, p.n_tiles) : launch_bn<32>(bn, st, maps, p, m_tiles, p.n_tiles);
 }
@@ -258,6 +280,17 @@ extern "C" int nb200_conv_gemm_f16(const void* A, int B, int Hi, int Wi, int Ci,
     g.Wt = (const __half*)Wt; g.N = N; g.bias = bias; g.act = act; g.out = (__half*)out; g.ldo = ldo;
     g.out_mode = out_mode; g.cout = cout; g.res = (const __half*)res; g.ldr = ldr; g.res_H = res_H; g.res_W = res_W;
     g.res_cy = res_cy; g.res_cx = res_cx; g.res_before_act = res_before_act;
+    return conv_gemm((cudaStream_t)stream, g);
+}
+
+// The pixel-shuffle GEMM (kind 1, out_mode 1) with a second A operand instead of a residual (ConvGemm::A2).
+extern "C" int nb200_conv_gemm_pixshuf_a2_f16(const void* A, int B, int Hi, int Wi, int Ci, const void* Wt, int N, const float* bias,
+                                              int act, void* out, int ldo, int cout, const void* A2, int Cin2, int ld2, void* stream) {
+    ConvGemm g;
+    g.A = (const __half*)A; g.B = B; g.Hi = Hi; g.Wi = Wi; g.Ci = Ci; g.Cin = Ci; g.kind = CG_LINEAR_2D;
+    g.Wt = (const __half*)Wt; g.N = N; g.bias = bias; g.act = act; g.out = (__half*)out; g.ldo = ldo;
+    g.out_mode = OUT_PIXSHUF2; g.cout = cout; g.A2 = (const __half*)A2; g.Cin2 = Cin2; g.ld2 = ld2;
+    NB_CHECK(g.A2, "null pointer");
     return conv_gemm((cudaStream_t)stream, g);
 }
 

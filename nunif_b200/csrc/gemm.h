@@ -30,6 +30,10 @@ struct ConvGemm {
     long long a_plane_stride = 0;
     const __half* res = nullptr;
     int ldr = 0, res_H = 0, res_W = 0, res_cy = 0, res_cx = 0, res_before_act = 0;
+    // OUT_PIXSHUF2 only, instead of res: a second A operand [B][2 Ho][2 Wo][ld2] whose first Cin2 channels at each output
+    // pixel are K columns [taps*Cin, taps*Cin + Cin2) of Wt (a Linear of the skip folded into the GEMM)
+    const __half* A2 = nullptr;
+    int Cin2 = 0, ld2 = 0;
 };
 
 int conv_gemm(cudaStream_t st, const ConvGemm& g);

@@ -41,13 +41,18 @@ struct GemmParams {
                          // OUT_SPLIT: N = nsplit*cout, block g goes to its own dense [M][cout] plane (maps o[g])
     int has_res, res_cy, res_cx;
     int res_before_act;  // 0: out = act(acc+bias) + res ; 1: out = act(acc+bias+res)
+    int k2;              // OUT_PIXSHUF2 with a second A operand (maps.a2): its BK-chunks, after the taps*cpt of A
 };
 
 // All tensor maps of one launch (a single __grid_constant__ parameter).
 struct GemmMaps {
     CUtensorMap a, b;
     CUtensorMap o[4];    // output: NHWC view (c, x, y, b); pixel-shuffle mode: one stride-2 view per (dy,dx)
-    CUtensorMap r[4];    // residual, same tiling as the output
+    union {
+        CUtensorMap r[4];    // residual, same tiling as the output
+        CUtensorMap a2;      // or the second A operand (the two exclude each other): full-resolution pixels of a pixel-shuffle
+                             // output as (c, dx, x, dy, b*Ho + y), stride-2 in x and y
+    };
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -273,7 +278,9 @@ __device__ __forceinline__ uint32_t sw64_off(int r, int col) {
     return (uint32_t)((col >> 5) * (ROWS * 64)) + stage_off<32>(r, (col & 31) >> 3) + (uint32_t)((col & 7) * 2);
 }
 
-template <int BLOCK_N, int BK>
+// A2: OUT_PIXSHUF2 with a second A operand.  Its K-chunks follow those of A, and each output pixel (2y+dy, 2x+dx) reads the
+// second operand at that same position; (dy, dx) is fixed by the CTA's N-block, so BLOCK_N must divide cout.
+template <int BLOCK_N, int BK, bool A2 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 2) gemm_conv_kernel(const __grid_constant__ GemmMaps maps,
                                                                     const __grid_constant__ GemmParams p) {
     using Cfg = GemmCfg<BLOCK_N, BK>;
@@ -294,7 +301,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) gemm_conv_kernel(const __grid
     const int b = tile / (p.tiles_x * p.tiles_y);
     const int x0 = tx_i * p.TW, y0 = ty_i * p.TH;
     const int n0 = n_tile * BLOCK_N;
-    const int k_iters = p.taps * p.cpt;
+    const int k_iters = p.taps * p.cpt + (A2 ? p.k2 : 0);
 
     if (threadIdx.x == GEMM_CONSUMER_THREADS) {
         tma_prefetch_desc(&maps.a);
@@ -323,7 +330,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) gemm_conv_kernel(const __grid
                 uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
                 uint8_t* sb = sa + Cfg::A_BYTES;
                 mbar_expect_tx(&full_bar[s], Cfg::A_BYTES + Cfg::B_BYTES);
-                tma_load_5d(&maps.a, &full_bar[s], sa, ch * BK, x0 + p.tap_dx[tap], p.tap_dyi[tap], y0 + p.tap_dy[tap], b);
+                if (A2 && tap >= p.taps) {
+                    // rows y >= Ho of a bottom edge tile read the next image; the output store clips them
+                    const int q = n0 / p.cout;
+                    tma_load_5d(&maps.a2, &full_bar[s], sa, (it - p.taps * p.cpt) * BK, q & 1, x0, q >> 1, b * p.Ho + y0);
+                } else {
+                    tma_load_5d(&maps.a, &full_bar[s], sa, ch * BK, x0 + p.tap_dx[tap], p.tap_dyi[tap], y0 + p.tap_dy[tap], b);
+                }
                 tma_load_2d(&maps.b, &full_bar[s], sb, it * BK, n0);
             }
         }

@@ -103,18 +103,24 @@ static Lin pack_linear(Packer& pk, const std::string& name, int N, int K, int n_
     return l;
 }
 // Linear followed by pixel_shuffle(2): rows reordered so n = (dy*2+dx)*cout + co  (F.pixel_shuffle: c*4 + dy*2 + dx)
-static Lin pack_linear_pixshuf2(Packer& pk, const std::string& name, int cout, int K) {
+// With `skip`, the Linear [cout][Ks] of the skip tensor that is added to the result is appended to every row (the GEMM's
+// second A operand, ConvGemm::A2): row n = [up row | skip row co], K + Ks columns, bias = both biases summed in fp32.
+static Lin pack_linear_pixshuf2(Packer& pk, const std::string& name, int cout, int K, const std::string& skip = "", int Ks = 0) {
     Lin l;
     l.N = 4 * cout;
-    l.K = K;
+    l.K = K + Ks;
     const float* w = pk.get(name + ".weight", (int64_t)4 * cout * K);
     const float* b = pk.get(name + ".bias", 4 * cout);
-    if (!w || !b) return l;
-    std::vector<float> wv((size_t)l.N * K), bv(l.N);
+    const float* ws = Ks ? pk.get(skip + ".weight", (int64_t)cout * Ks) : nullptr;
+    const float* bs = Ks ? pk.get(skip + ".bias", cout) : nullptr;
+    if (!w || !b || (Ks && (!ws || !bs))) return l;
+    std::vector<float> wv((size_t)l.N * l.K), bv(l.N);
     for (int co = 0; co < cout; ++co)
         for (int g = 0; g < 4; ++g) {
-            memcpy(&wv[((size_t)g * cout + co) * K], &w[((size_t)co * 4 + g) * K], (size_t)K * 4);
-            bv[g * cout + co] = b[co * 4 + g];
+            float* row = &wv[((size_t)g * cout + co) * l.K];
+            memcpy(row, &w[((size_t)co * 4 + g) * K], (size_t)K * 4);
+            if (Ks) memcpy(row + K, &ws[(size_t)co * Ks], (size_t)Ks * 4);
+            bv[g * cout + co] = b[co * 4 + g] + (Ks ? bs[co] : 0.f);
         }
     l.w = pk.add_f16(wv);
     l.b = pk.add_f32(bv);
@@ -201,7 +207,7 @@ struct SwinBlockW {
 
 struct SwinW {
     int C = 96, r = 4, cs = 48;
-    Lin stem, conv2, down1, down2, up2, up1, proj2, toimg;
+    Lin stem, conv2, down1, down2, up2, up1, toimg;   // 4x: up1 carries proj2 (pack_linear_pixshuf2 with a skip)
     std::vector<SwinBlockW> s1, s2, s3, s4, s5;
 };
 
@@ -370,8 +376,7 @@ static void pack_swin(Packer& pk, SwinW& w, int r) {
     w.up2 = pack_linear_pixshuf2(pk, "unet.up2.proj", 2 * C, 2 * C);
     pack_swin_blocks(pk, w.s4, "unet.swin4", 2 * C, 2);
     if (r == 4) {
-        w.proj2 = pack_linear(pk, "unet.proj2", 2 * C, C);
-        w.up1 = pack_linear_pixshuf2(pk, "unet.up1.proj", 2 * C, 2 * C);
+        w.up1 = pack_linear_pixshuf2(pk, "unet.up1.proj", 2 * C, 2 * C, "unet.proj2", C);
         pack_swin_blocks(pk, w.s5, "unet.swin5", 2 * C, 2);
         w.toimg = pack_linear(pk, "unet.to_image.proj", 3 * r * r, 2 * C, w.cs);
     } else {
@@ -396,13 +401,16 @@ static int linear_flat(cudaStream_t st, const nb200_model* m, const Lin& l, cons
     return conv_gemm(st, g);
 }
 
-static int swin_block(cudaStream_t st, const nb200_model* m, const SwinBlockW& w, __half* X, int n, int H, __half* ATT) {
+// toimg != nullptr: the block's output is not written to X; Y = output . Wtoimg^T + b ([T][toimg->N]) is, by the tail kernel
+static int swin_block(cudaStream_t st, const nb200_model* m, const SwinBlockW& w, __half* X, int n, int H, __half* ATT,
+                      const Lin* toimg = nullptr, __half* Y = nullptr) {
     const int C = w.C;
     const long long T = (long long)n * H * H;
     // two launches per block: q/k/v, x1 and the hidden tensor stay in shared memory / registers
     if (swin_attn_fused(st, X, m->at<__half>(w.qkv.w), m->at<float>(w.qkv.b), m->at<float>(w.table), ATT, n, H, H, C, w.shift)) return 1;
     return swin_mlp_fused(st, X, ATT, T, C, m->at<__half>(w.proj.w), m->at<float>(w.proj.b), m->at<__half>(w.fc1.w), m->at<float>(w.fc1.b),
-                          m->at<__half>(w.fc2.w), m->at<float>(w.fc2.b));
+                          m->at<__half>(w.fc2.w), m->at<float>(w.fc2.b), toimg ? Y : nullptr, toimg ? toimg->N : 0,
+                          toimg ? m->at<__half>(toimg->w) : nullptr, toimg ? m->at<float>(toimg->b) : nullptr);
 }
 
 static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n, int T, int down, void* z) {
@@ -411,7 +419,7 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
     const int C = w.C, Hc = T - 16, H2 = Hc / 2, H3 = Hc / 4, S1w = T - 2;
     const int C5 = w.r == 4 ? 2 * C : C;
     const size_t t1 = (size_t)n * Hc * Hc;
-    __half *S1, *X1, *ATT, *X2, *X3, *X4, *P2, *X5, *Y;
+    __half *S1, *X1, *ATT, *X2, *X3, *X4, *X5, *Y;
     if (m->carve([&](Arena& a) {
             S1 = a.take<__half>((size_t)n * S1w * S1w * 64);
             X1 = a.take<__half>(t1 * C);
@@ -419,7 +427,6 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
             X2 = a.take<__half>(t1 / 4 * 2 * C);
             X3 = a.take<__half>(t1 / 16 * 2 * C);
             X4 = a.take<__half>(t1 / 4 * 2 * C);
-            P2 = a.take<__half>(t1 * 2 * C);
             X5 = a.take<__half>(t1 * C5);
             Y = a.take<__half>(t1 * w.cs);
         })) return 1;
@@ -456,20 +463,18 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
         if (conv_gemm(st, g)) return 1;
     }
     for (const auto& b : w.s4) if (swin_block(st, m, b, X4, n, H2, ATT)) return 1;
-    const __half* skip = X1;
-    if (w.r == 4) {  // proj2(x3), swin_unet.py:159,195
-        if (linear_flat(st, m, w.proj2, X1, (long long)t1, C, P2, 2 * C, ACT_NONE)) return 1;
-        skip = P2;
-    }
-    {   // up1 + skip
+    {   // up1 + skip; 4x: the skip is proj2(x3) (swin_unet.py:159,195), the GEMM's second A operand
         ConvGemm g;
         g.A = X4; g.B = n; g.Hi = H2; g.Wi = H2; g.Ci = 2 * C; g.Cin = 2 * C; g.kind = CG_LINEAR_2D;
         g.Wt = m->at<__half>(w.up1.w); g.N = w.up1.N; g.bias = m->at<float>(w.up1.b); g.out = X5; g.ldo = C5;
-        g.out_mode = OUT_PIXSHUF2; g.cout = C5; g.res = skip; g.ldr = C5; g.res_H = Hc; g.res_W = Hc;
+        g.out_mode = OUT_PIXSHUF2; g.cout = C5;
+        if (w.r == 4) { g.A2 = X1; g.Cin2 = C; g.ld2 = C; }
+        else { g.res = X1; g.ldr = C5; g.res_H = Hc; g.res_W = Hc; }
         if (conv_gemm(st, g)) return 1;
     }
-    for (const auto& b : w.s5) if (swin_block(st, m, b, X5, n, Hc, ATT)) return 1;
-    if (linear_flat(st, m, w.toimg, X5, (long long)t1, C5, Y, w.cs, ACT_NONE)) return 1;      // ToImage.proj :109
+    // the last block's tail also runs ToImage.proj (:109) and writes only its result Y
+    for (size_t i = 0; i < w.s5.size(); ++i)
+        if (swin_block(st, m, w.s5[i], X5, n, Hc, ATT, i + 1 == w.s5.size() ? &w.toimg : nullptr, Y)) return 1;
     return to_image(st, Y, z, n, Hc, Hc, w.cs, w.r, down);
 }
 

@@ -11,6 +11,9 @@
 //               of fc2); per hidden chunk fc1 into registers, bias + GELU, packed to fp16 A fragments in registers and fed
 //               straight to the fc2 wgmma (A from registers), whose C-wide accumulator lives in registers for the whole tile;
 //               the output is written in place over the x tile and stored with TMA.
+// With CS > 0 (the last block of the network) the output tile is not stored: it is the A operand of one more wgmma,
+// y = x . Wy^T + by (to_image's Linear, [T][CS]), whose weights come through the ring as one more stage after the last W2
+// stage, and y is stored instead.  This block's x is dead afterwards, so it never reaches HBM.
 // Each ring stage is one wgmma commit group and is released when that group has retired, so the tensor pipe is never drained
 // inside a GEMM.  fc1 of chunk h + 1 goes into a second hidden accumulator before the GELU of chunk h, so that it runs with
 // tensor work in flight.  That takes ~210 registers per consumer thread (fc2's accumulator alone is C/2): with 288 threads
@@ -35,7 +38,7 @@ struct FmCfg {
 };
 
 struct FmMaps {
-    CUtensorMap x, att, wp, w1, w2;
+    CUtensorMap x, att, wp, w1, w2, y, wy;
 };
 
 template <int K>
@@ -62,11 +65,14 @@ __device__ __forceinline__ void wgmma_wait_n(int n) {
     else wgmma_wait<1>();
 }
 
-// PROJ (att != nullptr) is a template parameter: wgmmas under a run-time branch make ptxas serialise all of them.
-template <int C, bool PROJ>
+// PROJ (att != nullptr) and CS (the width of y, 0: store x) are template parameters: wgmmas under a run-time branch make
+// ptxas serialise all of them.
+template <int C, bool PROJ, int CS>
 __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __grid_constant__ FmMaps maps, const float* __restrict__ bp,
-                                                                     const float* __restrict__ b1, const float* __restrict__ b2) {
+                                                                     const float* __restrict__ b1, const float* __restrict__ b2,
+                                                                     const float* __restrict__ by) {
     using Cfg = FmCfg<C>;
+    static_assert(CS % 16 == 0 && 2 * C * CS <= Cfg::STAGE && CS * 256 <= Cfg::TILE, "Wy must fit a ring stage, y the att tile");
     constexpr int KB = Cfg::KB, NP = (KB + 1) / 2, NH = 2 * C / 64, NHALF = C / 96;
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -83,6 +89,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
         tma_prefetch_desc(&maps.x);
         tma_prefetch_desc(&maps.w1);
         tma_prefetch_desc(&maps.w2);
+        if (CS) tma_prefetch_desc(&maps.wy);
         if (PROJ) {
             tma_prefetch_desc(&maps.att);
             tma_prefetch_desc(&maps.wp);
@@ -132,6 +139,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
                 if (hc + 1 < NH) push(&maps.w1, 0, (hc + 1) * 64, 64, KB);
                 push(&maps.w2, hc * 64, 0, C, 2);
             }
+            if (CS) push(&maps.wy, 0, 0, CS, KB);
             if (!acts) load_acts();
         }
         return;
@@ -263,7 +271,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
     }
     retire(0);
     wgmma_fence_operands(oacc);
-    // x <- x1 + mlp(x1) (:454), in place over the x1 tile, then one TMA store per 32-column box
+    // x <- x1 + mlp(x1) (:454), in place over the x1 tile, then one TMA store per 32-column box (CS == 0) or the A operand of y
 #pragma unroll
     for (int j = 0; j < C / 8; ++j) {
         const int col = 8 * j + cq;
@@ -276,9 +284,45 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
         }
     }
     fence_async_smem();
+    if constexpr (CS > 0) {
+        // y = x . Wy^T + by from this warpgroup's 64 rows of the tile, in the K order of a GEMM over the stored x, so y is
+        // the same as to_image's Linear run on this block's output
+        asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+        float yacc[CS / 2];
+#pragma unroll
+        for (int j = 0; j < CS / 2; ++j) yacc[j] = 0.f;
+        wgmma_fence_operands(yacc);
+        const uint32_t bb = take();
+        wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < KB; ++kb) {
+            const uint32_t a = x_base + kb * (FM_ROWS * 64), b = bb + kb * (CS * 64);
+            wgmma_f16<CS>(yacc, make_kmajor_desc<64>(a), make_kmajor_desc<64>(b), 1u);
+            wgmma_f16<CS>(yacc, make_kmajor_desc<64>(a + 32), make_kmajor_desc<64>(b + 32), 1u);
+        }
+        commit();
+        retire(0);
+        wgmma_fence_operands(yacc);
+        // staged in the att tile (dead since proj) as CS/16 boxes of [128][16] with the 32B swizzle
+#pragma unroll
+        for (int j = 0; j < CS / 8; ++j) {
+            const int col = 8 * j + cq;
+            const float2 bq = __ldg(reinterpret_cast<const float2*>(by + col));
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                __half2* p = reinterpret_cast<__half2*>(satt + (col >> 4) * (FM_ROWS * 32) + stage_off<16>(row0 + 8 * i, (col & 15) >> 3) +
+                                                        (col & 7) * 2);
+                *p = __floats2half2_rn(yacc[4 * j + 2 * i] + bq.x, yacc[4 * j + 2 * i + 1] + bq.y);
+            }
+        }
+        fence_async_smem();
+    }
     consumer_bar_sync();
     if (tid == 0) {
-        for (int kb = 0; kb < KB; ++kb) tma_store_2d(&maps.x, sx + kb * (FM_ROWS * 64), kb * 32, row_base);   // rows >= T are clipped
+        if constexpr (CS > 0)
+            for (int c = 0; c < CS / 16; ++c) tma_store_2d(&maps.y, satt + c * (FM_ROWS * 32), 16 * c, row_base);
+        else
+            for (int kb = 0; kb < KB; ++kb) tma_store_2d(&maps.x, sx + kb * (FM_ROWS * 64), kb * 32, row_base);   // rows >= T are clipped
         tma_store_commit();
         tma_store_wait_read();
     }
@@ -291,9 +335,10 @@ static int map2d(CUtensorMap* m, const void* base, int cols, long long rows, int
     return encode(m, base, 2, dims, strides, box, 64);
 }
 
-template <int C, bool PROJ>
-static int launch_mlp(cudaStream_t st, unsigned grid, const FmMaps& maps, const float* bp, const float* b1, const float* b2) {
-    if (ensure_dyn_smem((const void*)swin_mlp_fused_kernel<C, PROJ>, FmCfg<C>::SMEM)) return 1;
+template <int C, bool PROJ, int CS = 0>
+static int launch_mlp(cudaStream_t st, unsigned grid, const FmMaps& maps, const float* bp, const float* b1, const float* b2,
+                      const float* by = nullptr) {
+    if (ensure_dyn_smem((const void*)swin_mlp_fused_kernel<C, PROJ, CS>, FmCfg<C>::SMEM)) return 1;
     // programmatic dependent launch (as gemm.cu): the producer's set-up and first weight stages overlap the head's last wave
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(FM_THREADS); cfg.dynamicSmemBytes = FmCfg<C>::SMEM;
@@ -302,24 +347,35 @@ static int launch_mlp(cudaStream_t st, unsigned grid, const FmMaps& maps, const 
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    NB_CUDA(cudaLaunchKernelEx(&cfg, swin_mlp_fused_kernel<C, PROJ>, maps, bp, b1, b2));
+    NB_CUDA(cudaLaunchKernelEx(&cfg, swin_mlp_fused_kernel<C, PROJ, CS>, maps, bp, b1, b2, by));
     NB_LAUNCHED();
     return 0;
 }
 
 int swin_mlp_fused(cudaStream_t st, __half* x, const __half* att, long long T, int C, const __half* wp, const float* bp,
-                   const __half* w1, const float* b1, const __half* w2, const float* b2) {
-    NB_CHECK(x && w1 && b1 && w2 && b2 && (!att || (wp && bp)), "null pointer");
+                   const __half* w1, const float* b1, const __half* w2, const float* b2, __half* y, int cs, const __half* wy,
+                   const float* by) {
+    NB_CHECK(x && w1 && b1 && w2 && b2 && (!att || (wp && bp)) && (!y || (att && wy && by)), "null pointer");
     NB_CHECK(C == 96 || C == 192, "C must be 96 or 192");
+    NB_CHECK(!y || (C == 192 && cs == 48) || (C == 96 && cs == 16), "y: cs must be 48 at C = 192 and 16 at C = 96");
     NB_CHECK(T > 0 && T < (1LL << 31), "token count out of range");
     FmMaps maps;
     memset(&maps, 0, sizeof(maps));
     if (map2d(&maps.x, x, C, T, FM_ROWS)) return 1;
     if (att && (map2d(&maps.att, att, C, T, FM_ROWS) || map2d(&maps.wp, wp, C, C, C))) return 1;
     if (map2d(&maps.w1, w1, C, 2 * C, 64) || map2d(&maps.w2, w2, 2 * C, C, C)) return 1;
+    if (y) {
+        if (map2d(&maps.wy, wy, C, cs, cs)) return 1;
+        const cuuint64_t dims[2] = {(cuuint64_t)cs, (cuuint64_t)T};
+        const cuuint64_t strides[1] = {(cuuint64_t)cs * 2};
+        const cuuint32_t box[2] = {16, FM_ROWS};
+        if (encode(&maps.y, y, 2, dims, strides, box, 32)) return 1;
+    }
     const double Td = (double)T;
-    ProfScope ps(st, PC_FUSED_MLP, Td * C * C * 2 * ((att ? 1 : 0) + 4), Td * C * 2 * (att ? 2 : 1), Td * C * 2);
+    ProfScope ps(st, PC_FUSED_MLP, Td * C * 2 * (C * ((att ? 1 : 0) + 4) + (y ? cs : 0)), Td * C * 2 * (att ? 2 : 1),
+                 Td * (y ? cs : C) * 2);
     const unsigned grid = (unsigned)((T + FM_ROWS - 1) / FM_ROWS);
+    if (y) return C == 96 ? launch_mlp<96, true, 16>(st, grid, maps, bp, b1, b2, by) : launch_mlp<192, true, 48>(st, grid, maps, bp, b1, b2, by);
     if (C == 96) return att ? launch_mlp<96, true>(st, grid, maps, bp, b1, b2) : launch_mlp<96, false>(st, grid, maps, bp, b1, b2);
     return att ? launch_mlp<192, true>(st, grid, maps, bp, b1, b2) : launch_mlp<192, false>(st, grid, maps, bp, b1, b2);
 }
@@ -331,7 +387,7 @@ using namespace nb200;
 extern "C" int nb200_swin_mlp_fused_f16(void* x, const void* att, long long T, int C, const void* wp, const float* bp,
                                         const void* w1, const float* b1, const void* w2, const float* b2, void* stream) {
     return swin_mlp_fused((cudaStream_t)stream, (__half*)x, (const __half*)att, T, C, (const __half*)wp, bp, (const __half*)w1, b1,
-                          (const __half*)w2, b2);
+                          (const __half*)w2, b2, nullptr, 0, nullptr, nullptr);
 }
 
 extern "C" int nb200_swin_attn_fused_f16(const void* x, const void* wqkv, const float* bqkv, const float* bias_table, void* att,

@@ -14,8 +14,10 @@ int window_attention(cudaStream_t st, const __half* qkv, const float* bias_frag,
 int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const float* bqkv, const float* bias_frag, __half* att,
                     int B, int H, int W, int C, int shift);
 // fused block tail (swin_block.cu): x1 = x + att . Wp^T + bp (att == nullptr: x1 = x); x <- x1 + gelu(x1 W1^T + b1) W2^T + b2
+// y != nullptr (needs att): x is not written; y [T][cs] = x . Wy^T + by instead (Wy [cs][C]; cs = 48 at C = 192, 16 at C = 96)
 int swin_mlp_fused(cudaStream_t st, __half* x, const __half* att, long long T, int C, const __half* wp, const float* bp,
-                   const __half* w1, const float* b1, const __half* w2, const float* b2);
+                   const __half* w1, const float* b1, const __half* w2, const float* b2, __half* y, int cs, const __half* wy,
+                   const float* by);
 // z: fp16 [n][3][S][S] for down == 1, fp32 for down in {2, 4}
 int to_image(cudaStream_t st, const __half* y, void* z, int n, int Hs, int Ws, int cs, int r, int down);
 }  // namespace nb200
