@@ -371,6 +371,34 @@ int nb200_conv_gemm_pixshuf_a2_f16(const void* A, int B, int Hi, int Wi, int Ci,
                                    const float* bias, int act, void* out, int ldo, int cout, const void* A2,
                                    int Cin2, int ld2, void* stream);
 
+/* Every field of the engine's implicit-GEMM launch (csrc/gemm.h ConvGemm), for tests that replay the engine's launches.
+ * kind: 0 linear over flattened pixels, 1 linear with 2-D tiling, 2 conv3x3 (pad 0 or 1), 3 conv2x2 stride 2,
+ *       5 (3,1,1) conv over time: A viewed as [B][T = Hi][Wi][Ci], taps t - dil, t, t + dil, zero padding dil.
+ * A: [B][Hi][Wi] pixels of Ci channels, of which the first Cin are read; a_row_stride / a_img_stride (elements, 0 = dense)
+ * let A be a cropped view; kind 0 with a_planes > 1 reads K as a_planes planes of Cin channels, a_plane_stride apart.
+ * out_mode 0: NHWC output, channel stride ldo; 1: pixel shuffle(2), N = 4*cout; 2: N/cout dense planes split_stride apart.
+ * res (optional): residual [B][res_H][res_W][ldr] read at (y + res_cy, x + res_cx), added before the activation when
+ * res_before_act.  A2 (out_mode 1, no res): second A operand [B][2 Ho][2 Wo][ld2], its first Cin2 channels are the last
+ * Cin2 K columns of Wt. */
+typedef struct nb200_gemm_desc {
+    int kind, pad, dil, B, Hi, Wi, Ci, Cin;
+    long long a_row_stride, a_img_stride;
+    int a_planes;
+    long long a_plane_stride;
+    int N, act, ldo, out_mode, cout;
+    long long split_stride;
+    int ldr, res_H, res_W, res_cy, res_cx, res_before_act;
+    int Cin2, ld2;
+} nb200_gemm_desc;
+int nb200_conv_gemm_ex_f16(const nb200_gemm_desc* desc, const void* A, const void* Wt, const float* bias, void* out,
+                           const void* res, const void* A2, void* stream);
+
+/* The ViT / BEiT attention of the depth models: qkv [B][N][3][heads][64] fp16 -> out [B][N][heads][64] fp16,
+ * softmax(q k^T / 8 + bias) v.  bias_log2e (optional): fp32 [heads][N][ldb], already multiplied by log2(e);
+ * ldb is even and >= N rounded up to 64. */
+int nb200_flash_attention_f16(const void* qkv, void* out, int B, int N, int heads, const float* bias_log2e, int ldb,
+                              void* stream);
+
 /* shifted-window attention core between the qkv and proj Linears
  * (torchvision swin_transformer.py:166-221), window 6x6, 6 heads.
  * qkv: three dense planes q | k | v, each [B][H][W][C] fp16 (how the engine's qkv GEMM writes them)
@@ -385,6 +413,14 @@ int nb200_window_attention_f16(const void* qkv, const float* bias_table, void* o
 int nb200_swin_mlp_fused_f16(void* x, const void* att, long long T, int C, const void* wp,
                              const float* bp, const void* w1, const float* b1, const void* w2,
                              const float* b2, void* stream);
+
+/* The same tail as the network's last block runs it, with to_image's Linear fused: the block output is not written to x
+ * (x is left unchanged); y [T][cs] = output @ wy^T + by is written instead.  att is required; wy [cs][C] fp16, by [cs]
+ * fp32; cs = 48 at C = 192, 16 at C = 96. */
+int nb200_swin_mlp_fused_y_f16(void* x, const void* att, long long T, int C, const void* wp,
+                               const float* bp, const void* w1, const float* b1, const void* w2,
+                               const float* b2, void* y, int cs, const void* wy, const float* by,
+                               void* stream);
 
 /* Head of one SwinTransformerBlock: qkv Linear + shifted 6x6 window attention (swin_transformer.py:166-221;
  * everything but the proj Linear), the engine's GEMM and window-attention kernels (csrc/swin_block.cu).
@@ -443,6 +479,16 @@ int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermedia
 int nb200_profile_enable(int on);
 int nb200_profile_report(char* buf, size_t cap);
 int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launch: class,ms,work,read_bytes,write_bytes */
+
+/* Launch recorder for tests: on = 1 clears the record and appends one CSV line per launch of the implicit GEMM, the ViT
+ * attention and the fused Swin-block head and tail; on = 0 stops.  Off by default; recording changes no launch.  Lines:
+ *   gemm,kind,pad,dil,B,Hi,Wi,Ci,Cin,a_row_stride,a_img_stride,a_planes,a_plane_stride,N,act,ldo,out_mode,cout,
+ *        split_stride,has_bias,has_res,ldr,res_H,res_W,res_cy,res_cx,res_before_act,has_A2,Cin2,ld2,out_is_res,out_is_A,
+ *        block_n,bk,grid
+ *   attn,B,N,heads,has_bias,ldb      swin_attn,B,H,W,C,shift      swin_mlp,T,C,proj,cs
+ * recorded_launches copies them (NUL-terminated) like nb200_profile_dump; it fails if cap is too small. */
+int nb200_record_launches(int on);
+int nb200_recorded_launches(char* buf, size_t cap);
 
 #ifdef __cplusplus
 }

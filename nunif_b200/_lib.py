@@ -33,6 +33,16 @@ class TileConfig(ctypes.Structure):
         }
 
 
+class GemmDesc(ctypes.Structure):
+    """nb200_gemm_desc: every field of one implicit-GEMM launch (csrc/gemm.h ConvGemm) but the pointers."""
+    _fields_ = ([(n, ctypes.c_int) for n in ("kind", "pad", "dil", "B", "Hi", "Wi", "Ci", "Cin")]
+                + [("a_row_stride", ctypes.c_longlong), ("a_img_stride", ctypes.c_longlong), ("a_planes", ctypes.c_int),
+                   ("a_plane_stride", ctypes.c_longlong)]
+                + [(n, ctypes.c_int) for n in ("N", "act", "ldo", "out_mode", "cout")]
+                + [("split_stride", ctypes.c_longlong)]
+                + [(n, ctypes.c_int) for n in ("ldr", "res_H", "res_W", "res_cy", "res_cx", "res_before_act", "Cin2", "ld2")])
+
+
 # name -> (restype, argtypes).  Must list every symbol declared in include/nunif_b200.h
 # (tests/test_abi.py parses the header and checks this table and the .so against it).
 SIGNATURES = {
@@ -115,6 +125,13 @@ SIGNATURES = {
                                     c_void_p]),
     "nb200_conv_gemm_pixshuf_a2_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
                                                c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "nb200_conv_gemm_ex_f16": (c_int, [ctypes.POINTER(GemmDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p]),
+    "nb200_flash_attention_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "nb200_swin_mlp_fused_y_f16": (c_int, [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "nb200_record_launches": (c_int, [c_int]),
+    "nb200_recorded_launches": (c_int, [c_char_p, c_size_t]),
     "nb200_tune_set": (c_int, [c_int, c_int]),
     "nb200_debug_tap": (c_int, [c_int, c_void_p, ctypes.c_size_t]),
     "nb200_profile_enable": (c_int, [c_int]),

@@ -40,6 +40,15 @@ void prof_end(cudaStream_t st) {
     if (!g_prof_recs.empty()) cudaEventRecord(g_prof_recs.back().b, st);
 }
 
+std::atomic<int> g_rec_enabled{0};
+static std::mutex g_rec_mu;
+static std::string g_rec;
+void rec_append(const char* line) {
+    std::lock_guard<std::mutex> lk(g_rec_mu);
+    g_rec += line;
+    g_rec += '\n';
+}
+
 static std::mutex g_attr_mu;
 static std::map<std::pair<int, const void*>, size_t> g_dyn_smem;
 int ensure_dyn_smem(const void* func, size_t bytes) {
@@ -148,5 +157,23 @@ extern "C" int nb200_profile_dump(char* buf, size_t cap) {
     }
     NB_CHECK(s.size() + 1 <= cap, "buffer too small");
     memcpy(buf, s.c_str(), s.size() + 1);
+    return 0;
+}
+
+// Launch recorder: on = 1 clears the record and starts appending, on = 0 stops (the record stays readable).  Host only: a
+// launch made while it is off costs one relaxed atomic load.
+extern "C" int nb200_record_launches(int on) {
+    std::lock_guard<std::mutex> lk(g_rec_mu);
+    if (on) g_rec.clear();
+    g_rec_enabled.store(on ? 1 : 0);
+    return 0;
+}
+
+// One CSV line per recorded launch; the first field names the kind (gemm, attn, swin_attn, swin_mlp), see the header.
+extern "C" int nb200_recorded_launches(char* buf, size_t cap) {
+    NB_CHECK(buf && cap > 0, "null buffer");
+    std::lock_guard<std::mutex> lk(g_rec_mu);
+    NB_CHECK(g_rec.size() + 1 <= cap, "buffer too small: " + std::to_string(g_rec.size() + 1) + " bytes needed");
+    memcpy(buf, g_rec.c_str(), g_rec.size() + 1);
     return 0;
 }

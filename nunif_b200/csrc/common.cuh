@@ -59,6 +59,12 @@ struct ProfScope {
     }
 };
 
+// ---- optional launch recorder (nb200_record_launches): the GEMM, ViT attention and fused Swin-block host code append one CSV
+// line per launch describing it without its pointers, so tests can replay every configuration a network uses
+extern std::atomic<int> g_rec_enabled;
+void rec_append(const char* line);
+inline bool rec_on() { return g_rec_enabled.load(std::memory_order_relaxed) != 0; }
+
 // seam_blend.cu: rows [y0, y1) of the blended output (used by the band-pipelined host render in model.cu)
 int tile_gather_blend_rows(const void* z_all, int z_f32, int C, const ::nb200_tile_config* cfg, int scale, int offset, int tile_size,
                            int blend_size, float* out, int y0, int y1, void* stream);

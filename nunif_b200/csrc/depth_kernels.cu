@@ -425,6 +425,11 @@ int da_attention(cudaStream_t st, const __half* qkv, __half* out, int B, int N, 
     const size_t smem = (size_t)(FA_BM + 4 * FA_BN) * FA_LD * sizeof(__half);
     const double T = (double)B * N * heads * FA_D;
     ProfScope ps(st, PC_ATTN, 4.0 * T * N, T * 3 * 2 + (bias_log2e ? (double)heads * N * N * 4 : 0.0), T * 2);
+    if (rec_on()) {
+        char line[96];
+        snprintf(line, sizeof(line), "attn,%d,%d,%d,%d,%d", B, N, heads, bias_log2e ? 1 : 0, bias_log2e ? ldb : 0);
+        rec_append(line);
+    }
     if (bias_log2e) {
         NB_CHECK(ldb % 2 == 0 && ldb >= cdiv(N, FA_BN) * FA_BN, "bias row stride must be even and cover whole 64-key blocks");
         if (ensure_dyn_smem((const void*)flash_attention_kernel<true>, smem)) return 1;
@@ -478,3 +483,10 @@ int da_head_final(cudaStream_t st, const __half* x, long long npix, int C, const
 }
 
 }  // namespace nb200
+
+// The ViT attention of every Depth-Anything / ZoeDepth block (include/nunif_b200.h)
+extern "C" int nb200_flash_attention_f16(const void* qkv, void* out, int B, int N, int heads, const float* bias_log2e, int ldb,
+                                         void* stream) {
+    NB_CHECK(qkv && out && B > 0 && N > 0 && heads > 0, "bad arguments");
+    return nb200::da_attention((cudaStream_t)stream, (const __half*)qkv, (__half*)out, B, N, heads, bias_log2e, ldb);
+}

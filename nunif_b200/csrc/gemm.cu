@@ -2,6 +2,7 @@
 #include "gemm.h"
 #include "gemm_wgmma.cuh"
 #include "tmap.h"
+#include "../../include/nunif_b200.h"
 #include <mutex>
 #include <cstdlib>
 
@@ -261,6 +262,16 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
                  in_px * (g.kind == CG_LINEAR_FLAT ? g.Cin * g.a_planes : g.Cin) * 2.0 + (g.res ? Mrows * g.N * 2.0 : 0.0) +
                      4.0 * Mrows * g.Cin2 * (a2 ? 2.0 : 0.0) + (double)g.N * K * 2.0,
                  Mrows * (double)g.N * 2.0);
+    if (rec_on()) {
+        char line[512];
+        snprintf(line, sizeof(line),
+                 "gemm,%d,%d,%d,%d,%d,%d,%d,%d,%lld,%lld,%d,%lld,%d,%d,%d,%d,%d,%lld,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d",
+                 g.kind, g.pad, g.dil, g.B, g.Hi, g.Wi, g.Ci, g.Cin, g.a_row_stride, g.a_img_stride, g.a_planes, g.a_plane_stride,
+                 g.N, g.act, g.ldo, g.out_mode, g.cout, g.split_stride, g.bias ? 1 : 0, g.res ? 1 : 0, g.ldr, g.res_H, g.res_W,
+                 g.res_cy, g.res_cx, g.res_before_act, a2 ? 1 : 0, g.Cin2, g.ld2, g.res && (const void*)g.out == (const void*)g.res,
+                 (const void*)g.out == (const void*)g.A, bn, BK, m_tiles * p.n_tiles);
+        rec_append(line);
+    }
     return BK == 64 ? launch_bn<64>(bn, st, maps, p, m_tiles, p.n_tiles) : launch_bn<32>(bn, st, maps, p, m_tiles, p.n_tiles);
 }
 
@@ -291,6 +302,21 @@ extern "C" int nb200_conv_gemm_pixshuf_a2_f16(const void* A, int B, int Hi, int 
     g.Wt = (const __half*)Wt; g.N = N; g.bias = bias; g.act = act; g.out = (__half*)out; g.ldo = ldo;
     g.out_mode = OUT_PIXSHUF2; g.cout = cout; g.A2 = (const __half*)A2; g.Cin2 = Cin2; g.ld2 = ld2;
     NB_CHECK(g.A2, "null pointer");
+    return conv_gemm((cudaStream_t)stream, g);
+}
+
+// Every ConvGemm field through a plain C struct (include/nunif_b200.h nb200_gemm_desc), for tests that replay the engine's launches.
+extern "C" int nb200_conv_gemm_ex_f16(const nb200_gemm_desc* d, const void* A, const void* Wt, const float* bias, void* out,
+                                      const void* res, const void* A2, void* stream) {
+    NB_CHECK(d, "null descriptor");
+    ConvGemm g;
+    g.A = (const __half*)A; g.B = d->B; g.Hi = d->Hi; g.Wi = d->Wi; g.Ci = d->Ci; g.Cin = d->Cin;
+    g.a_row_stride = d->a_row_stride; g.a_img_stride = d->a_img_stride; g.kind = d->kind; g.pad = d->pad; g.dil = d->dil;
+    g.Wt = (const __half*)Wt; g.N = d->N; g.bias = bias; g.act = d->act; g.out = (__half*)out; g.ldo = d->ldo;
+    g.out_mode = d->out_mode; g.cout = d->cout; g.split_stride = d->split_stride; g.a_planes = d->a_planes;
+    g.a_plane_stride = d->a_plane_stride; g.res = (const __half*)res; g.ldr = d->ldr; g.res_H = d->res_H; g.res_W = d->res_W;
+    g.res_cy = d->res_cy; g.res_cx = d->res_cx; g.res_before_act = d->res_before_act;
+    g.A2 = (const __half*)A2; g.Cin2 = d->Cin2; g.ld2 = d->ld2;
     return conv_gemm((cudaStream_t)stream, g);
 }
 

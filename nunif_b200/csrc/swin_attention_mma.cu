@@ -541,6 +541,11 @@ int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const 
     const double T = (double)B * H * W;
     ProfScope ps(st, PC_FUSED_ATTN, T * 3.0 * C * C * 2 + T * C * 36 * 4, T * C * 2, T * C * 2);   // qkv GEMM + QK^T/PV; x in, att out
     const unsigned grid = (unsigned)((nwin + FA_WIN - 1) / FA_WIN);
+    if (rec_on()) {
+        char line[96];
+        snprintf(line, sizeof(line), "swin_attn,%d,%d,%d,%d,%d", B, H, W, C, shift);
+        rec_append(line);
+    }
     const float4* bf = reinterpret_cast<const float4*>(bias_frag_f);
     if (C == 96) {
         if (ensure_dyn_smem((const void*)swin_attn_fused_kernel<96>, FaCfg<96>::SMEM)) return 1;

@@ -375,6 +375,11 @@ int swin_mlp_fused(cudaStream_t st, __half* x, const __half* att, long long T, i
     ProfScope ps(st, PC_FUSED_MLP, Td * C * 2 * (C * ((att ? 1 : 0) + 4) + (y ? cs : 0)), Td * C * 2 * (att ? 2 : 1),
                  Td * (y ? cs : C) * 2);
     const unsigned grid = (unsigned)((T + FM_ROWS - 1) / FM_ROWS);
+    if (rec_on()) {
+        char line[96];
+        snprintf(line, sizeof(line), "swin_mlp,%lld,%d,%d,%d", T, C, att ? 1 : 0, y ? cs : 0);
+        rec_append(line);
+    }
     if (y) return C == 96 ? launch_mlp<96, true, 16>(st, grid, maps, bp, b1, b2, by) : launch_mlp<192, true, 48>(st, grid, maps, bp, b1, b2, by);
     if (C == 96) return att ? launch_mlp<96, true>(st, grid, maps, bp, b1, b2) : launch_mlp<96, false>(st, grid, maps, bp, b1, b2);
     return att ? launch_mlp<192, true>(st, grid, maps, bp, b1, b2) : launch_mlp<192, false>(st, grid, maps, bp, b1, b2);
@@ -388,6 +393,15 @@ extern "C" int nb200_swin_mlp_fused_f16(void* x, const void* att, long long T, i
                                         const void* w1, const float* b1, const void* w2, const float* b2, void* stream) {
     return swin_mlp_fused((cudaStream_t)stream, (__half*)x, (const __half*)att, T, C, (const __half*)wp, bp, (const __half*)w1, b1,
                           (const __half*)w2, b2, nullptr, 0, nullptr, nullptr);
+}
+
+// The tail of the network's last block, which also runs to_image's Linear (the CS instantiations): x is left unchanged
+extern "C" int nb200_swin_mlp_fused_y_f16(void* x, const void* att, long long T, int C, const void* wp, const float* bp,
+                                          const void* w1, const float* b1, const void* w2, const float* b2, void* y, int cs,
+                                          const void* wy, const float* by, void* stream) {
+    NB_CHECK(y, "null pointer");
+    return swin_mlp_fused((cudaStream_t)stream, (__half*)x, (const __half*)att, T, C, (const __half*)wp, bp, (const __half*)w1, b1,
+                          (const __half*)w2, b2, (__half*)y, cs, (const __half*)wy, by);
 }
 
 extern "C" int nb200_swin_attn_fused_f16(const void* x, const void* wqkv, const float* bqkv, const float* bias_table, void* att,

@@ -1,0 +1,842 @@
+"""GPU: replay every launch that the engine's networks make of the wgmma implicit GEMM (gemm_conv_kernel), the ViT flash
+attention (flash_attention_kernel) and the fused Swin block (swin_attn_fused_kernel, swin_mlp_fused_kernel), at their production
+shapes, against float64 references.
+
+A module fixture turns the library's launch recorder on (nb200_record_launches) and runs one forward of each network of
+MODELS.  Each unique recorded configuration is then replayed through a low-level entry point on fresh seeded data:
+  * guards: input elements outside the view the launch describes are fp16 NaN, output elements outside the view it writes
+    hold a sentinel bit pattern (also a NaN), and a guard block sits before and after every buffer.  A replay passes only
+    if its output holds no NaN and every guard element is bit-identical after the call;
+  * the reference is float64, written from the semantics of gemm.h / gemm_wgmma.cuh / the kernels' comments (per-tap shifted
+    slices, not the kernels' tensor-map views), and each element is checked against an error bound derived from the
+    kernel's arithmetic (see the bound helpers).
+"""
+import ctypes
+import math
+import time
+import zlib
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+from tests.util import log_metric
+from nunif_b200 import _lib, synth
+
+pytestmark = pytest.mark.gpu
+DEV = "cuda:0"
+LOG2E = math.log2(math.e)
+SENTINEL = 0x7E5B            # an fp16 NaN payload: guards keep exactly this bit pattern
+GUARD = 4096                 # guard elements before and after every buffer
+CHUNK_BYTES = 2 << 30        # float64 working set of one reference chunk
+
+GEMM_FIELDS = ("kind pad dil B Hi Wi Ci Cin a_row_stride a_img_stride a_planes a_plane_stride N act ldo out_mode cout "
+               "split_stride has_bias has_res ldr res_H res_W res_cy res_cx res_before_act has_a2 Cin2 ld2 out_is_res out_is_a "
+               "block_n bk grid").split()
+FIELDS = {"gemm": GEMM_FIELDS, "attn": "B N heads has_bias ldb".split(), "swin_attn": "B H W C shift".split(),
+          "swin_mlp": "T C proj cs".split()}
+DESC_FIELDS = [f for f, _ in _lib.GemmDesc._fields_]
+# what identifies a GEMM launch (the last three fields are the host code's choices for it)
+GEMM_KEY = [f for f in GEMM_FIELDS if f not in ("block_n", "bk", "grid")]
+# every instantiation gemm.cu launch_bn can select: (BLOCK_N, BK, A2)
+INSTANTIATIONS = {(bn, bk, 0) for bn in (16, 32, 48, 64, 96, 128) for bk in (32, 64)} | {(bn, bk, 1) for bn in (64, 96) for bk in (32, 64)}
+
+
+# ------------------------------------------------------------------------------------------------------------ recorder
+def read_records():
+    lib = _lib.lib()
+    cap = 1 << 20
+    while True:
+        buf = ctypes.create_string_buffer(cap)
+        if lib.nb200_recorded_launches(buf, cap) == 0:
+            break
+        if b"buffer too small" not in lib.nb200_last_error():
+            _lib.check(1)
+        cap *= 4
+    recs = []
+    for line in buf.value.decode().splitlines():
+        kind, *vals = line.split(",")
+        recs.append((kind, dict(zip(FIELDS[kind], (int(v) for v in vals)))))
+    return recs
+
+
+def recorded(fn):
+    """Run fn() with the recorder on; -> its records."""
+    lib = _lib.lib()
+    _lib.check(lib.nb200_record_launches(1))
+    try:
+        fn()
+        torch.cuda.synchronize()
+    finally:
+        lib.nb200_record_launches(0)
+    return read_records()
+
+
+# ------------------------------------------------------------------------------------------------------------ networks
+def _gen(seed):
+    return torch.Generator().manual_seed(seed)
+
+
+def _waifu2x(name, sd_fn, to_2x=False):
+    def run():
+        from nunif_b200.nunif.models import create_model
+        m = create_model(name, sd_fn(), DEV)
+        if to_2x:
+            m = m.to_2x()
+        m(torch.rand(16, 3, 256, 256, generator=_gen(1)).to(DEV))
+    return run
+
+
+def _depth_anything(encoder, v1=False):
+    def run():
+        from nunif_b200.iw3 import DepthAnythingNet
+        from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
+        h, w = preprocess_size(1080, 1920)
+        net = DepthAnythingNet(synth.depth_anything_v2_state_dict(0, encoder=encoder), DEV, encoder=encoder, v1=v1)
+        net(torch.randn(4, 3, h, w, generator=_gen(2)).to(DEV))
+    return run
+
+
+def _zoe_n():
+    from nunif_b200.iw3 import ZoeDepthNet
+    from nunif_b200.iw3.zoedepth_preprocess import preprocess_size
+    _, _, ph, pw, fh, fw = preprocess_size(2160, 3840)
+    ZoeDepthNet(synth.zoedepth_state_dict(0), DEV)(torch.randn(2, 3, fh + 2 * ph, fw + 2 * pw, generator=_gen(3)).clamp_(-1, 1).to(DEV))
+
+
+def _zoe_any_n():
+    from nunif_b200.iw3 import ZoeDepthAnythingNet
+    from nunif_b200.iw3.zoedepth_preprocess import preprocess_size
+    net = ZoeDepthAnythingNet(synth.zoedepth_any_state_dict(0, None, False), DEV, "ZoeD_Any_N")
+    for H, W in ((1080, 1920), (1920, 1080)):
+        _, _, ph, pw, fh, fw = preprocess_size(H, W, h_height=392, v_height=518, ensure_multiple_of=14)
+        net(torch.randn(1, 3, fh + 2 * ph, fw + 2 * pw, generator=_gen(4)).clamp_(-1, 1).to(DEV))
+
+
+def _depth_input(B, h, w):
+    from oracle.row_flow import make_input
+    return make_input(synth.synth_depth(7, B, h, w), 2.5, 0.4).to(DEV)
+
+
+def _row_flow_v3():
+    from nunif_b200.iw3 import RowFlowV3
+    RowFlowV3(synth.row_flow_v3_state_dict(0), DEV)(_depth_input(1, 1080, 1920))
+
+
+def _mlbw(layers):
+    def run():
+        from nunif_b200.iw3 import MLBW
+        MLBW(synth.mlbw_state_dict(0, num_layers=layers), DEV)(_depth_input(1, 1080, 1920))
+    return run
+
+
+def _depth_aa():
+    from nunif_b200.iw3.depth_aa import DepthAA
+    from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
+    h, w = preprocess_size(1080, 1920)
+    DepthAA(synth.depth_aa_state_dict(0), DEV)(synth.synth_depth(8, 4, h, w).to(DEV))
+
+
+def _light_inpaint():
+    from nunif_b200.iw3 import LightInpaintV1
+    x = torch.rand(1, 3, 1080, 1920, generator=_gen(5)).to(DEV)
+    mask = (torch.rand(1, 1, 1080, 1920, generator=_gen(6)) < 0.05).float().to(DEV)
+    LightInpaintV1(synth.light_inpaint_v1_state_dict(0), DEV).infer(x, mask)
+
+
+def _transnet():
+    from nunif_b200.nunif.transnetv2 import TransNetV2
+    m = TransNetV2(synth.transnetv2_state_dict(0), DEV)
+    for B in (1, 8):
+        x = torch.stack([torch.from_numpy(synth.shot_sequence(900 + b, 100)).permute(0, 3, 1, 2).float() for b in range(B)])
+        m(x.to(DEV))
+
+
+MODELS = [
+    ("swin_unet_4x", _waifu2x("waifu2x.swin_unet_4x", lambda: synth.swin_unet_state_dict(0, 4))),   # bench swin4x_4k: tile 256, batch 16
+    ("swin_unet_4x.to_2x", _waifu2x("waifu2x.swin_unet_4x", lambda: synth.swin_unet_state_dict(0, 4), True)),   # bench swin2x_4k
+    ("swin_unet_2x", _waifu2x("waifu2x.swin_unet_2x", lambda: synth.swin_unet_state_dict(0, 2))),   # tiled_render default: tile 256, batch 16
+    ("swin_unet_1x", _waifu2x("waifu2x.swin_unet_1x", lambda: synth.swin_unet_state_dict(0, 1))),   # tiled_render default: tile 256, batch 16
+    ("upcunet", _waifu2x("waifu2x.upcunet", synth.upcunet_state_dict)),      # bench upcunet: tile 256, batch 16
+    ("cunet", _waifu2x("waifu2x.cunet", synth.cunet_state_dict)),            # tiled_render default: tile 256, batch 16
+    ("upconv_7", _waifu2x("waifu2x.upconv_7", synth.upconv7_state_dict)),    # tiled_render default: tile 256, batch 16
+    ("vgg_7", _waifu2x("waifu2x.vgg_7", synth.vgg7_state_dict)),             # tiled_render default: tile 256, batch 16
+    ("depth_anything_v2_s", _depth_anything("vits")),        # bench iw3_1080p: 1080p frames -> 392 x 686, B = 4
+    ("depth_anything_v2_b", _depth_anything("vitb")),        # iw3 Any_V2_B on the same 1080p batch
+    ("depth_anything_v2_l", _depth_anything("vitl")),        # iw3 Any_V2_L on the same 1080p batch
+    ("depth_anything_v1_s", _depth_anything("vits", True)),  # iw3 Any_S (V1) on the same 1080p batch
+    ("zoed_n", _zoe_n),                                      # bench iw3_4k_zoe: 4K frames -> 384 x 704, B = 2
+    ("zoed_any_n", _zoe_any_n),                              # iw3 default model: 1080p landscape (392 x 700) and portrait (v_height 518)
+    ("row_flow_v3", _row_flow_v3),                           # iw3 row_flow_v3 on a 1080p depth map
+    ("mlbw_l2", _mlbw(2)),                                   # iw3 mlbw_l2 on a 1080p depth map
+    ("mlbw_l4", _mlbw(4)),                                   # iw3 mlbw_l4 on a 1080p depth map
+    ("depth_aa", _depth_aa),                                 # iw3 depth_aa on the Depth-Anything output of a 1080p batch (392 x 686, B = 4)
+    ("light_inpaint_v1", _light_inpaint),                    # iw3 forward_inpaint on a 1080p frame
+    ("transnetv2", _transnet),                               # --scene-detect: 100-frame windows, one alone and 8 batched
+]
+
+
+@pytest.fixture(scope="module")
+def production():
+    """name -> unique records (kind, config) of one forward of each network of MODELS."""
+    out = {}
+    for name, fn in MODELS:
+        t0 = time.time()
+        recs = recorded(fn)
+        torch.cuda.empty_cache()
+        print(f"{name}: {len(recs)} launches recorded in {time.time() - t0:.1f} s")
+        uniq = []
+        for kind, r in recs:
+            key = (kind, tuple(r.items()))
+            if key not in uniq:
+                uniq.append(key)
+        out[name] = [(k, dict(r)) for k, r in uniq]
+    return out
+
+
+def _unique(production, kind, extra=()):
+    seen, cases = set(), []
+    for name, recs in production.items():
+        for k, r in recs:
+            if k != kind:
+                continue
+            key = tuple(r[f] for f in (GEMM_KEY if kind == "gemm" else FIELDS[kind]))
+            if key not in seen:
+                seen.add(key)
+                cases.append((name, r))
+    for r in extra:
+        key = tuple(r[f] for f in (GEMM_KEY if kind == "gemm" else FIELDS[kind]))
+        if key not in seen:
+            seen.add(key)
+            cases.append(("synthetic", r))
+    return cases
+
+
+def test_every_network_records_its_launches(production):
+    lines = []
+    for name, _ in MODELS:
+        recs = production[name]
+        counts = {k: sum(1 for kk, _ in recs if kk == k) for k in FIELDS}
+        inst = sorted({(r["block_n"], r["bk"], r["has_a2"]) for k, r in recs if k == "gemm"})
+        lines.append(f"{name:22s} unique: gemm {counts['gemm']:3d} attn {counts['attn']:2d} swin_attn {counts['swin_attn']:2d} "
+                     f"swin_mlp {counts['swin_mlp']:2d}   (BLOCK_N, BK, A2): {inst}")
+        log_metric("replay_configs", model=name, **counts)
+        assert counts["gemm"] > 0, f"{name}: no implicit-GEMM launch was recorded"
+    print("\n" + "\n".join(lines))
+    for name in ("depth_anything_v2_s", "depth_anything_v2_l", "zoed_n", "zoed_any_n"):
+        assert any(k == "attn" for k, _ in production[name]), name
+    for name in ("swin_unet_4x", "swin_unet_2x", "swin_unet_1x"):
+        assert any(k == "swin_attn" for k, _ in production[name]) and any(k == "swin_mlp" and r["cs"] > 0 for k, r in production[name]), name
+
+
+# ------------------------------------------------------------------------------------------------------------ helpers
+def ulp16(x):
+    """fp16 spacing at |x| (float64), floored at 2^-24 (the subnormal spacing)."""
+    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14)))
+    return torch.exp2(e - 10).clamp_min(2.0 ** -24)
+
+
+def guarded(n):
+    """fp16 buffer of GUARD + n + GUARD elements, all SENTINEL."""
+    return torch.full((n + 2 * GUARD,), SENTINEL, dtype=torch.int16, device=DEV).view(torch.float16)
+
+
+def view(buf, shape, strides, offset=0):
+    return buf.as_strided(shape, strides, GUARD + offset)
+
+
+def extent(shape, strides, offset=0):
+    return offset + sum((s - 1) * st for s, st in zip(shape, strides)) + 1
+
+
+def fill_normal(v, g, std=1.0):
+    v.copy_((torch.randn(v.shape, generator=g, device=DEV) * std).to(v.dtype))
+
+
+def bits(t):
+    return t.view(torch.int16)
+
+
+def gelu64(x):
+    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
+
+
+ACT = {0: lambda v: v, 1: lambda v: torch.where(v > 0, v, 0.1 * v), 2: gelu64, 3: lambda v: v.clamp_min(0.0)}
+
+
+# ------------------------------------------------------------------------------------------------------------ GEMM replay
+def _gemm_cfg(**kw):
+    r = dict.fromkeys(GEMM_FIELDS, 0)
+    r.update(dil=1, a_planes=1, has_bias=1)
+    r.update(kw)
+    return r
+
+
+def _synthetic_gemm():
+    """Small launches that, with the production ones, reach every instantiation launch_bn can select, plus the ConvGemm
+    paths a production shape exercises only at one size."""
+    big = 148 * 128   # enough 128-row tiles that the small-M narrowing keeps the widest BLOCK_N
+    out = []
+    for N in (16, 32, 48, 64, 96, 128):
+        for Cin in (32, 64):
+            out.append(_gemm_cfg(kind=0, B=1, Hi=1, Wi=big + 77, Ci=Cin + 8, Cin=Cin, N=N, ldo=N + 16, act=1))
+    for cout, Cin, Cin2 in ((64, 64, 64), (64, 96, 32), (96, 128, 64), (96, 64, 96)):
+        out.append(_gemm_cfg(kind=1, B=2, Hi=21, Wi=19, Ci=Cin, Cin=Cin, N=4 * cout, ldo=cout, out_mode=1, cout=cout, act=1,
+                             has_a2=1, Cin2=Cin2, ld2=Cin2 + 32))
+    # TCONV3 with a dilation that spans most of a short window, a channel slice and ldo > N
+    out.append(_gemm_cfg(kind=5, dil=3, B=2, Hi=7, Wi=45, Ci=96, Cin=32, N=64, ldo=128, act=3))
+    # residual before the activation, cropped residual, cropped A view
+    out.append(_gemm_cfg(kind=2, pad=0, B=2, Hi=19, Wi=37, Ci=64, Cin=64, a_row_stride=41 * 64, a_img_stride=23 * 41 * 64, N=64,
+                         ldo=64, act=2, has_res=1, ldr=72, res_H=21, res_W=39, res_cy=2, res_cx=3, res_before_act=1))
+    out.append(_gemm_cfg(kind=2, pad=1, B=3, Hi=13, Wi=29, Ci=32, Cin=32, N=48, ldo=48, act=1, has_res=1, ldr=48, res_H=13,
+                         res_W=29, res_before_act=0))
+    out.append(_gemm_cfg(kind=0, B=1, Hi=1, Wi=3001, Ci=64, Cin=64, N=192, ldo=64, out_mode=2, cout=64, split_stride=3001 * 64 + 8))
+    out.append(_gemm_cfg(kind=0, B=1, Hi=1, Wi=2000, Ci=64, Cin=64, a_planes=3, a_plane_stride=2000 * 64 + 24, N=96, ldo=96))
+    return out
+
+
+class GemmCase:
+    """Buffers of one replayed launch, laid out from its record with the same strides and aliasing."""
+
+    def __init__(self, r, seed):
+        self.r = r
+        g = torch.Generator(device=DEV).manual_seed(seed)
+        kind = r["kind"]
+        B, Hi, Wi, Ci, Cin = r["B"], r["Hi"], r["Wi"], r["Ci"], r["Cin"]
+        if kind == 0:
+            self.B, self.Ho, self.Wo = 1, 1, B * Hi * Wi
+            self.taps, ktap = r["a_planes"], Cin
+            M = self.Wo
+            ps = r["a_plane_stride"] if r["a_planes"] > 1 else M * Ci
+            self.a_shape, self.a_strides = (r["a_planes"], M, Cin), (ps, Ci, 1)
+        else:
+            rs = r["a_row_stride"] or Wi * Ci
+            ims = r["a_img_stride"] or Hi * rs
+            self.a_shape, self.a_strides = (B, Hi, Wi, Cin), (ims, rs, Ci, 1)
+            self.B = B
+            if kind == 1:
+                self.Ho, self.Wo, self.taps, ktap = Hi, Wi, 1, Cin
+            elif kind == 2:
+                p = r["pad"]
+                self.Ho, self.Wo, self.taps, ktap = Hi - 2 + 2 * p, Wi - 2 + 2 * p, 9, Cin
+            elif kind == 5:
+                self.Ho, self.Wo, self.taps, ktap = Hi, Wi, 3, Cin
+            elif kind == 3:
+                self.Ho, self.Wo, self.taps, ktap = Hi // 2, Wi // 2, 2, 2 * Cin
+            else:
+                raise AssertionError(f"unknown kind {kind}")
+        N, ldo, mode, cout = r["N"], r["ldo"], r["out_mode"], r["cout"]
+        Bo, Ho, Wo = self.B, self.Ho, self.Wo
+        self.K = self.taps * ktap + r["Cin2"]
+        # output view (B, Ho, Wo, g1, g2, cg): n = (g1 * g2dim + g2) * cg + c
+        if mode == 0:
+            self.o_shape, self.o_strides = (Bo, Ho, Wo, 1, 1, N), (Ho * Wo * ldo, Wo * ldo, ldo, 1, 1, 1)
+        elif mode == 2:
+            self.o_shape = (Bo, Ho, Wo, N // cout, 1, cout)
+            self.o_strides = (Ho * Wo * ldo, Wo * ldo, ldo, r["split_stride"], 1, 1)
+        else:
+            self.o_shape, self.o_strides = (Bo, Ho, Wo, 2, 2, cout), (4 * Ho * Wo * ldo, 4 * Wo * ldo, 2 * ldo, 2 * Wo * ldo, ldo, 1)
+        o_ext = extent(self.o_shape, self.o_strides)
+        if mode == 1:
+            o_ext = max(o_ext, Bo * 4 * Ho * Wo * ldo)
+        # residual view, read at (y + res_cy, x + res_cx) of [B][res_H][res_W][ldr] (the whole M row for kind 0)
+        self.res = None
+        if r["has_res"]:
+            rH, rW, cy, cx, ldr = r["res_H"], r["res_W"], r["res_cy"], r["res_cx"], r["ldr"]
+            if kind == 0:
+                rH, rW, cy, cx = 1, Wo, 0, 0
+            if mode == 1:
+                shp, st = (Bo, Ho, Wo, 2, 2, cout), (rH * rW * ldr, 2 * rW * ldr, 2 * ldr, rW * ldr, ldr, 1)
+                assert cy + 1 + 2 * (Ho - 1) < rH and cx + 1 + 2 * (Wo - 1) < rW, r
+            else:
+                shp, st = (Bo, Ho, Wo, 1, 1, N), (rH * rW * ldr, rW * ldr, ldr, 1, 1, 1)
+                assert cy + Ho <= rH and cx + Wo <= rW, f"residual view outside the residual tensor: {r}"
+            self.r_shape, self.r_strides, self.r_off = shp, st, (cy * rW + cx) * ldr
+            r_ext = max(Bo * rH * rW * ldr, extent(shp, st, self.r_off))
+        a_ext = extent(self.a_shape, self.a_strides)
+        # buffers: aliasing as recorded
+        if r["out_is_a"]:
+            self.out = guarded(max(o_ext, a_ext))
+            self.a = self.out
+        else:
+            self.out = guarded(o_ext)
+            self.a = guarded(a_ext)
+        fill_normal(view(self.a, self.a_shape, self.a_strides), g)
+        self.a_ref = view(self.a, self.a_shape, self.a_strides).clone()
+        if r["has_res"]:
+            self.res = self.out if r["out_is_res"] else guarded(r_ext)
+            if r["out_is_res"]:
+                assert self.r_off == 0 and self.r_strides == self.o_strides, f"in-place residual with a different view: {r}"
+            fill_normal(view(self.res, self.r_shape, self.r_strides, self.r_off), g)
+            self.res_ref = view(self.res, self.r_shape, self.r_strides, self.r_off).clone()
+        self.a2 = None
+        if r["has_a2"]:
+            ld2, C2 = r["ld2"], r["Cin2"]
+            self.a2_shape = (Bo, Ho, Wo, 2, 2, C2)
+            self.a2_strides = (4 * Ho * Wo * ld2, 4 * Wo * ld2, 2 * ld2, 2 * Wo * ld2, ld2, 1)
+            self.a2 = guarded(Bo * 4 * Ho * Wo * ld2)
+            fill_normal(view(self.a2, self.a2_shape, self.a2_strides), g)
+        self.W = (torch.randn(N, self.K, generator=g, device=DEV) / math.sqrt(self.K)).half()
+        self.bias = 0.5 * torch.randn(N, generator=g, device=DEV) if r["has_bias"] else None
+        self.snap = {id(t): t.clone() for t in {id(x): x for x in (self.a, self.out, self.res, self.a2) if x is not None}.values()}
+
+    def launch(self):
+        r = self.r
+        d = _lib.GemmDesc(**{f: r[f] for f in DESC_FIELDS})
+        p = lambda t: _lib.ptr(t) if t is None else ctypes.c_void_p(t.data_ptr() + 2 * GUARD)
+        _lib.check(_lib.lib().nb200_conv_gemm_ex_f16(ctypes.byref(d), p(self.a), _lib.ptr(self.W), _lib.ptr(self.bias), p(self.out),
+                                                     p(self.res), p(self.a2), _lib.stream_ptr()))
+        torch.cuda.synchronize()
+
+    def check_guards(self):
+        """-> list of problems: NaN in the output view, guard / unviewed elements changed."""
+        bad = []
+        written = torch.zeros(self.out.numel(), dtype=torch.bool, device=DEV)
+        view(written, self.o_shape, self.o_strides).fill_(True)
+        for buf in {id(x): x for x in (self.a, self.out, self.res, self.a2) if x is not None}.values():
+            keep = ~written if buf is self.out else torch.ones_like(written[:1]).expand(buf.numel())
+            changed = (bits(buf) != bits(self.snap[id(buf)])) & keep
+            if bool(changed.any()):
+                i = int(changed.nonzero()[0]) - GUARD
+                bad.append(f"element {i} outside the written view changed (buffer of {buf.numel() - 2 * GUARD})")
+        if bool(torch.isnan(view(self.out, self.o_shape, self.o_strides)).any()):
+            bad.append("NaN in the output")
+        return bad
+
+    def _tap_slices(self, a16, y0, y1):
+        """(float64 [rows, Cin] slice, first K column) per tap for output rows [y0, y1) of the images in a16."""
+        r, kind, Cin = self.r, self.r["kind"], self.r["Cin"]
+        Wo = self.Wo
+        if kind == 1:
+            yield a16[:, y0:y1], 0
+        elif kind == 2:
+            for t in range(9):
+                ky, kx = divmod(t, 3)
+                yield a16[:, y0 + ky:y1 + ky, kx:kx + Wo], t * Cin
+        elif kind == 5:
+            d = r["dil"]
+            for t in range(3):
+                yield a16[:, y0 + t * d:y1 + t * d], t * Cin
+        elif kind == 3:
+            for t in range(4):
+                dy, dx = divmod(t, 2)
+                yield a16[:, 2 * y0 + dy:2 * y1:2, dx::2], t * Cin
+
+    def reference_chunks(self):
+        """-> iterator of (index into the [B, Ho, Wo, N] output, float64 pre-epilogue accumulator, float64 sum |a w|)."""
+        r, kind, N = self.r, self.r["kind"], self.r["N"]
+        W = self.W.double()
+        Wa = W.abs()
+        if kind == 0:
+            A = self.a_ref
+            M = A.shape[1]
+            rows = max(1, CHUNK_BYTES // (8 * 4 * (N + A.shape[2])))
+            for m0 in range(0, M, rows):
+                m1 = min(M, m0 + rows)
+                acc = torch.zeros(m1 - m0, N, dtype=torch.float64, device=DEV)
+                sab = torch.zeros_like(acc)
+                for p in range(A.shape[0]):
+                    x = A[p, m0:m1].double()
+                    w = W[:, p * r["Cin"]:(p + 1) * r["Cin"]]
+                    acc += x @ w.t()
+                    sab += x.abs() @ Wa[:, p * r["Cin"]:(p + 1) * r["Cin"]].t()
+                yield (0, 0, slice(m0, m1)), acc.view(1, 1, m1 - m0, N), sab.view(1, 1, m1 - m0, N)
+            return
+        Cin = r["Cin"]
+        per_row = self.Wo * 8 * 4 * (N + 2 * Cin + r["Cin2"])
+        rows = max(1, CHUNK_BYTES // per_row)
+        for b in range(self.B):
+            a16 = self.a_ref[b:b + 1]
+            if kind == 2 and r["pad"]:
+                a16 = F.pad(a16, (0, 0, 1, 1, 1, 1))
+            elif kind == 5:
+                d = r["dil"]
+                a16 = F.pad(a16, (0, 0, 0, 0, d, d))
+            for y0 in range(0, self.Ho, rows):
+                y1 = min(self.Ho, y0 + rows)
+                acc = torch.zeros((y1 - y0) * self.Wo, N, dtype=torch.float64, device=DEV)
+                sab = torch.zeros_like(acc)
+                for x, k0 in self._tap_slices(a16, y0, y1):
+                    kw = x.shape[-1]
+                    x = x.double().reshape(-1, kw)
+                    acc += x @ W[:, k0:k0 + kw].t()
+                    sab += x.abs() @ Wa[:, k0:k0 + kw].t()
+                if self.a2 is not None:
+                    C2, cout, k2 = r["Cin2"], r["cout"], self.K - r["Cin2"]
+                    a2 = view(self.a2, self.a2_shape, self.a2_strides)[b:b + 1, y0:y1]
+                    for q in range(4):
+                        x = a2[:, :, :, q // 2, q % 2].double().reshape(-1, C2)
+                        cols = slice(q * cout, (q + 1) * cout)
+                        acc[:, cols] += x @ W[cols, k2:].t()
+                        sab[:, cols] += x.abs() @ Wa[cols, k2:].t()
+                shp = (1, y1 - y0, self.Wo, N)
+                yield (slice(b, b + 1), slice(y0, y1), slice(None)), acc.view(shp), sab.view(shp)
+
+    def check(self):
+        """-> (largest |err| / bound, number of elements over the bound)."""
+        r = self.r
+        act = r["act"]
+        L = 1.13 if act == 2 else 1.0
+        got_all = view(self.out, self.o_shape, self.o_strides)
+        res_all = self.res_ref if self.res is not None else None
+        worst, over = 0.0, 0
+        for idx, acc, sab in self.reference_chunks():
+            v = acc + (self.bias.double() if self.bias is not None else 0.0)
+            if res_all is not None:
+                rv = res_all[idx].double().reshape(v.shape)
+                v = ACT[act](v + rv) if r["res_before_act"] else ACT[act](v) + rv
+            else:
+                v = ACT[act](v)
+            got = got_all[idx].double().reshape(v.shape)
+            bound = ulp16(v) + 2.0 ** -20 * L * sab + (1e-6 if act == 2 else 0.0)
+            ratio = (got - v).abs() / bound
+            worst = max(worst, float(ratio.max()))
+            over += int((ratio > 1).sum())
+        return worst, over
+
+
+def _seed(*parts):
+    return zlib.crc32(repr(parts).encode())
+
+
+def test_gemm_instantiation_coverage(production):
+    """Every (BLOCK_N, BK, A2) instantiation gemm.cu can select is reached by a recorded launch or a synthetic one."""
+    have = {(r["block_n"], r["bk"], r["has_a2"]) for recs in production.values() for k, r in recs if k == "gemm"}
+    rows = []
+    for r in _synthetic_gemm():
+        case = GemmCase(r, 1)
+        recs = recorded(case.launch)
+        rows.append((recs[0][1]["block_n"], recs[0][1]["bk"], recs[0][1]["has_a2"]))
+    table = {i: ("recorded" if i in have else ("synthetic" if i in rows else "MISSING")) for i in sorted(INSTANTIATIONS)}
+    print("\n" + "\n".join(f"BLOCK_N {bn:3d} BK {bk} A2 {a2}: {src}" for (bn, bk, a2), src in table.items()))
+    assert (have | set(rows)) >= INSTANTIATIONS, [i for i, s in table.items() if s == "MISSING"]
+    assert (have | set(rows)) <= INSTANTIATIONS
+
+
+def test_gemm_replay(production):
+    cases = _unique(production, "gemm", _synthetic_gemm())
+    t0, worst, fails = time.time(), 0.0, []
+    for name, r in cases:
+        case = GemmCase(r, _seed(name, tuple(r[f] for f in GEMM_KEY)))
+        case.launch()
+        bad = case.check_guards()
+        ratio, over = case.check()
+        del case
+        cfg = ",".join(f"{f}={r[f]}" for f in GEMM_KEY if r[f])
+        log_metric("replay_gemm", model=name, cfg=cfg, err_over_bound=f"{ratio:.3g}")
+        worst = max(worst, ratio)
+        if bad or over:
+            fails.append(f"{name} {cfg}: {bad} max err/bound {ratio:.3g}, {over} elements over")
+    torch.cuda.empty_cache()
+    print(f"\ngemm: {len(cases)} configurations, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
+    log_metric("replay_gemm_summary", configs=len(cases), worst=worst)
+    assert not fails, "\n".join(fails[:20])
+
+
+# ------------------------------------------------------------------------------------------------------------ flash attention
+SYNTH_ATTN = [dict(B=B, N=N, heads=h, has_bias=bias, ldb=(-(-N // 64) * 64 + (64 if bias and N % 2 else 0)) if bias else 0)
+              for N in (1, 2, 63, 64, 65, 127, 128, 129) for h in (6, 16) for B in (1, 3) for bias in (0, 1)]
+
+
+def _needle_targets(N):
+    tail0 = (N - 1) // 64 * 64
+    return sorted({t for t in (0, 63, 64, tail0, N - 1) if 0 <= t < N})
+
+
+def attention_case(r, needle, seed):
+    """-> (qkv fp16 [B][N][3][heads][64], bias fp32 [heads][N][ldb] or None, chosen key per row or None)."""
+    g = torch.Generator().manual_seed(seed)
+    B, N, H, ldb = r["B"], r["N"], r["heads"], r["ldb"]
+    qkv = torch.randn(B, N, 3, H, 64, generator=g)
+    bias = None
+    targets = None
+    if not needle:
+        qkv[:, :, :2] *= 3 ** 0.5                       # q.k / 8 has a standard deviation of 3
+        if r["has_bias"]:
+            bias = torch.randn(H, N, ldb, generator=g) * LOG2E
+    else:
+        tk = _needle_targets(N)
+        targets = torch.tensor([tk[i % len(tk)] for i in range(N)])
+        if r["has_bias"]:
+            # the bias makes the needle, at a column other than the row (a transposed index moves the output by O(1))
+            for i in range(N):
+                if targets[i] == i and len(tk) > 1:
+                    targets[i] = tk[(i + 1) % len(tk)]
+            qkv[:, :, :2] *= 0.7                        # scores of standard deviation 0.5 around the needle
+            bias = torch.randn(H, N, ldb, generator=g) * 0.5
+            bias[:, torch.arange(N), targets] = 14.0
+            bias *= LOG2E
+        else:
+            # key t_j points along dimension j; each query points at its key
+            qkv[:, :, :2] *= 0.3
+            for j, t in enumerate(tk):
+                qkv[:, t, 1, :, :] = 0.0
+                qkv[:, t, 1, :, j] = 16.0
+            for i in range(N):
+                qkv[:, i, 0, :, tk.index(int(targets[i]))] += 8.0
+    if bias is not None:
+        bias[:, :, N:] = 1e4 * LOG2E                    # an unmasked tail column would take the whole softmax
+        bias = bias.float().to(DEV)
+    return qkv.half().to(DEV), bias, targets
+
+
+def attention_check(r, needle, seed):
+    """Bound per element: 2^-9 sum_j p_j |v_j| covers the fp16 rounding of P before PV (2^-11 relative), its mismatch with
+    the fp32 row sum and ex2.approx.  Where P is below 2^-14 its fp16 value is subnormal and the rounding is absolute, up to
+    2^-25 of the running maximum (which is 1 before the row sum l >= 1 divides): 2^-25 sum_j |v_j| / l = 2^-25 max_j p_j
+    sum_j |v_j|.  A needle row puts its tiny P on every other key, so this term matters there."""
+    B, N, H, ldb = r["B"], r["N"], r["heads"], r["ldb"]
+    qkv, bias, targets = attention_case(r, needle, seed)
+    dim = H * 64
+    out = guarded(B * N * dim + 64 * dim)
+    _lib.check(_lib.lib().nb200_flash_attention_f16(_lib.ptr(qkv), ctypes.c_void_p(out.data_ptr() + 2 * GUARD), B, N, H,
+                                                    _lib.ptr(bias), ldb, _lib.stream_ptr()))
+    torch.cuda.synchronize()
+    bad = []
+    got = view(out, (B, N, H, 64), (N * dim, dim, 64, 1))
+    if bool(torch.isnan(got).any()):
+        bad.append("NaN in the output")
+    if not bool((bits(out[:GUARD]) == SENTINEL).all() and (bits(out[GUARD + B * N * dim:]) == SENTINEL).all()):
+        bad.append("guard rows changed")
+    worst, over = 0.0, 0
+    for b in range(B):
+        q, k, v = (qkv[b, :, i].double().permute(1, 0, 2) for i in range(3))   # [H][N][64]
+        s = q @ k.transpose(1, 2) / 8.0
+        if bias is not None:
+            s = s + bias[:, :, :N].double() / LOG2E
+        p = torch.softmax(s, dim=-1)
+        if targets is not None:
+            mass = p[:, torch.arange(N, device=DEV), targets.to(DEV)]
+            assert float(mass.min()) >= 0.9, float(mass.min())
+        ref = p @ v
+        bound = 2.0 ** -9 * (p @ v.abs()) + 2.0 ** -25 * p.amax(-1, keepdim=True) * v.abs().sum(1, keepdim=True) + ulp16(ref)
+        ratio = (got[b].double().permute(1, 0, 2) - ref).abs() / bound
+        worst = max(worst, float(ratio.max()))
+        over += int((ratio > 1).sum())
+    return worst, over, bad
+
+
+def test_flash_attention_replay(production):
+    cases = _unique(production, "attn", SYNTH_ATTN)
+    t0, worst, fails = time.time(), 0.0, []
+    for name, r in cases:
+        for needle in (False, True):
+            ratio, over, bad = attention_check(r, needle, _seed(name, tuple(r.values()), needle))
+            cfg = ",".join(f"{f}={r[f]}" for f in FIELDS["attn"])
+            log_metric("replay_attn", model=name, cfg=cfg, needle=int(needle), err_over_bound=f"{ratio:.3g}")
+            worst = max(worst, ratio)
+            if bad or over:
+                fails.append(f"{name} {cfg} needle={needle}: {bad} max err/bound {ratio:.3g}, {over} elements over")
+    print(f"\nattention: {len(cases)} configurations x 2 inputs, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
+    log_metric("replay_attn_summary", configs=len(cases), worst=worst)
+    assert not fails, "\n".join(fails[:20])
+
+
+# ------------------------------------------------------------------------------------------------------------ Swin head
+SYNTH_SWIN_ATTN = [dict(B=1, H=6, W=6, C=192, shift=3), dict(B=3, H=18, W=30, C=96, shift=3), dict(B=2, H=24, W=12, C=192, shift=3),
+                   dict(B=5, H=12, W=12, C=192, shift=0)]
+
+
+def window_attention64(qkv, table, C, shift, eqkv=None, ws=6, heads=6):
+    """float64 torchvision shifted_window_attention body (swin_transformer.py:166-221) without the Linears.  qkv [B][H][W][3C]
+    -> output, sum_j p_j |v_j|, max_j p_j sum_j |v_j|, and with eqkv (a bound on the error of each q|k|v element) the first-order bound on the
+    output error they cause: sum_j p_j (|ds_j| |v_j - o| + ev_j), ds_j the score error."""
+    from nunif_b200.synth import relative_position_index
+    B, H, W, _ = qkv.shape
+    d = C // heads
+    s = shift if ws < H else 0
+    nh, nw = H // ws, W // ws
+
+    def windows(t):
+        t = torch.roll(t, shifts=(-s, -s), dims=(1, 2)) if s > 0 else t
+        return t.view(B, nh, ws, nw, ws, 3 * C).permute(0, 1, 3, 2, 4, 5).reshape(B * nh * nw, ws * ws, 3, heads, d).permute(2, 0, 3, 1, 4)
+    xw = windows(qkv)
+    q, k, v = xw[0] * d ** -0.5, xw[1], xw[2]
+    attn = q @ k.transpose(-2, -1)
+    idx = relative_position_index(ws).to(qkv.device)
+    attn = attn + table[idx].view(ws * ws, ws * ws, -1).permute(2, 0, 1).unsqueeze(0)
+    if s > 0:
+        m = torch.zeros((H, W), device=qkv.device, dtype=qkv.dtype)
+        cnt = 0
+        for hs in ((0, -ws), (-ws, -s), (-s, None)):
+            for ws_ in ((0, -ws), (-ws, -s), (-s, None)):
+                m[hs[0]:hs[1], ws_[0]:ws_[1]] = cnt
+                cnt += 1
+        m = m.view(nh, ws, nw, ws).permute(0, 2, 1, 3).reshape(nh * nw, ws * ws)
+        m = m.unsqueeze(1) - m.unsqueeze(2)
+        m = m.masked_fill(m != 0, -100.0).masked_fill(m == 0, 0.0)
+        attn = (attn.view(B, nh * nw, heads, ws * ws, ws * ws) + m.unsqueeze(1).unsqueeze(0)).view(-1, heads, ws * ws, ws * ws)
+    p = attn.softmax(-1)
+    o = p @ v
+    outs = [o, p @ v.abs(), p.amax(-1, keepdim=True) * v.abs().sum(-2, keepdim=True)]
+    if eqkv is not None:
+        ew = windows(eqkv)
+        eq, ek, ev = ew[0] * d ** -0.5, ew[1], ew[2]
+        ds = eq @ (k.abs() + ek).transpose(-2, -1) + q.abs() @ ek.transpose(-2, -1)
+        pd = p * ds
+        # exp(ds) - 1 <= 1.1 ds for the ds << 0.1 seen here: first order with a margin
+        outs.append(1.1 * (pd @ v.abs() + pd.sum(-1, keepdim=True) * o.abs()) + p @ ev)
+    res = []
+    for o in outs:
+        o = o.transpose(1, 2).reshape(-1, ws * ws, C).view(B, nh, nw, ws, ws, C).permute(0, 1, 3, 2, 4, 5).reshape(B, H, W, C)
+        res.append(torch.roll(o, shifts=(s, s), dims=(1, 2)) if s > 0 else o)
+    return res
+
+
+def swin_attn_check(r, seed):
+    B, H, W, C, shift = r["B"], r["H"], r["W"], r["C"], r["shift"]
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    rn = lambda *shape: torch.randn(*shape, generator=g, device=DEV)
+    x = rn(B, H, W, C).half()
+    wqkv = (rn(3 * C, C) / C ** 0.5).half()
+    bqkv = 0.1 * rn(3 * C)
+    table = 0.5 * rn(121, 6)
+    n = B * H * W * C
+    att = guarded(n)
+    x0 = x.clone()
+    _lib.check(_lib.lib().nb200_swin_attn_fused_f16(_lib.ptr(x), _lib.ptr(wqkv), _lib.ptr(bqkv), _lib.ptr(table),
+                                                    ctypes.c_void_p(att.data_ptr() + 2 * GUARD), B, H, W, C, shift, _lib.stream_ptr()))
+    torch.cuda.synchronize()
+    bad = []
+    got = att[GUARD:GUARD + n].view(B, H, W, C)
+    if bool(torch.isnan(got).any()):
+        bad.append("NaN in the output")
+    if not bool((bits(att[:GUARD]) == SENTINEL).all() and (bits(att[GUARD + n:]) == SENTINEL).all()):
+        bad.append("guard changed")
+    if not torch.equal(bits(x), bits(x0)):
+        bad.append("x changed")
+    worst, over = 0.0, 0
+    for b in range(B):
+        # q|k|v are rounded to fp16 after the bias, as the kernel stores them; before that the kernel's fp32 GEMM is within
+        # 2^-20 sum|x w| (+ the bias add) of the float64 one
+        xb = x[b:b + 1].double()
+        v = xb @ wqkv.double().t() + bqkv.double()
+        qkv, eqkv = rounded(v, 2.0 ** -20 * (xb.abs() @ wqkv.double().abs().t()) + 2.0 ** -22 * v.abs())
+        ref, spv, sub, eprop = window_attention64(qkv, table.double(), C, shift, eqkv)
+        # fp16 P, its fp32 row sum and ex2.approx as in the ViT attention; plus the q|k|v rounding differences
+        bound = ulp16(ref) + 2.0 ** -9 * spv + 2.0 ** -25 * sub + eprop
+        ratio = (got[b:b + 1].double() - ref).abs() / bound
+        worst = max(worst, float(ratio.max()))
+        over += int((ratio > 1).sum())
+    return worst, over, bad
+
+
+def test_swin_attn_replay(production):
+    cases = _unique(production, "swin_attn", SYNTH_SWIN_ATTN)
+    t0, worst, fails = time.time(), 0.0, []
+    for name, r in cases:
+        ratio, over, bad = swin_attn_check(r, _seed(name, tuple(r.values())))
+        cfg = ",".join(f"{f}={r[f]}" for f in FIELDS["swin_attn"])
+        log_metric("replay_swin_attn", model=name, cfg=cfg, err_over_bound=f"{ratio:.3g}")
+        worst = max(worst, ratio)
+        if bad or over:
+            fails.append(f"{name} {cfg}: {bad} max err/bound {ratio:.3g}, {over} elements over")
+    print(f"\nswin head: {len(cases)} configurations, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
+    log_metric("replay_swin_attn_summary", configs=len(cases), worst=worst)
+    assert not fails, "\n".join(fails[:20])
+
+
+# ------------------------------------------------------------------------------------------------------------ Swin tail
+SYNTH_SWIN_MLP = [dict(T=16 * 240 * 240, C=192, proj=1, cs=48),      # the 4x model's last block at tile 256, batch 16
+                  dict(T=148 * 128 * 3 + 55, C=192, proj=1, cs=48), dict(T=148 * 128 * 2 + 1, C=96, proj=1, cs=16),
+                  dict(T=148 * 128 + 127, C=192, proj=1, cs=0), dict(T=777, C=96, proj=0, cs=0)]
+
+
+def rounded(v, E):
+    """An fp16 rounding point: the kernel rounds a value within E of the float64 v.  Rounding is monotone, so its result lies
+    between the roundings of v - E and v + E: -> (v rounded, bound on |kernel's rounded value - v rounded|).  The bound is 0
+    wherever no rounding boundary lies within E, so only those few elements carry an error forward."""
+    r = v.half().double()
+    return r, torch.maximum((v + E).half().double() - r, r - (v - E).half().double())
+
+
+def mlp_reference(x, att, wp, bp, w1, b1, w2, b2, wy, by):
+    """float64 block tail with the kernel's fp16 rounding points (x1, hidden, and with wy the block output) -> (reference,
+    bound per element).  Before each rounding point, the kernel's fp32 value differs from the float64 one by at most: 2^-20
+    sum|a w| per GEMM (wgmma fp32 accumulation), 2^-21 |v| for the fp32 bias / residual adds and the GELU evaluation, 1e-6 for
+    the GELU polynomial, and the differences carried from the previous rounding point through the GEMM (GELU's slope is at
+    most 1.13).  rounded() turns that into the difference after rounding."""
+    acc = 2.0 ** -20
+    x = x.double()
+    if att is not None:
+        a = att.double()
+        v = x + a @ wp.double().t() + bp.double()
+        x1, e1 = rounded(v, acc * (a.abs() @ wp.double().abs().t()) + 2.0 ** -21 * (x.abs() + v.abs()))
+    else:
+        x1, e1 = x, torch.zeros_like(x)
+    w1a = w1.double().abs()
+    pre = x1 @ w1.double().t() + b1.double()
+    h, eh = rounded(gelu64(pre), 1.13 * (acc * (x1.abs() @ w1a.t()) + e1 @ w1a.t()) + 2.0 ** -21 * pre.abs() + 1e-6)
+    w2a = w2.double().abs()
+    o = x1 + h @ w2.double().t() + b2.double()
+    eo = e1 + acc * (h.abs() @ w2a.t()) + eh @ w2a.t() + 2.0 ** -21 * (x1.abs() + o.abs())
+    if wy is None:
+        return o, ulp16(o) + eo
+    o, eo = rounded(o, eo)
+    wya = wy.double().abs()
+    y = o @ wy.double().t() + by.double()
+    return y, ulp16(y) + acc * (o.abs() @ wya.t()) + eo @ wya.t()
+
+
+def swin_mlp_check(r, seed):
+    T, C, proj, cs = r["T"], r["C"], r["proj"], r["cs"]
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    rn = lambda *shape: torch.randn(*shape, generator=g, device=DEV)
+    xb = guarded(T * C)
+    x = xb[GUARD:GUARD + T * C].view(T, C)
+    x.copy_(rn(T, C).half())
+    att = rn(T, C).half() if proj else None
+    wp = (rn(C, C) / C ** 0.5).half()
+    bp = 0.1 * rn(C)
+    w1 = (rn(2 * C, C) / C ** 0.5).half()
+    b1 = 0.1 * rn(2 * C)
+    w2 = (rn(C, 2 * C) / (2 * C) ** 0.5).half()
+    b2 = 0.1 * rn(C)
+    wy = (rn(cs, C) / C ** 0.5).half() if cs else None
+    by = rn(cs) if cs else None          # O(1), so a lost bias is an O(1) error
+    x0 = xb.clone()
+    lib = _lib.lib()
+    xp = ctypes.c_void_p(xb.data_ptr() + 2 * GUARD)
+    if cs:
+        yb = guarded(T * cs)
+        _lib.check(lib.nb200_swin_mlp_fused_y_f16(xp, _lib.ptr(att), T, C, _lib.ptr(wp), _lib.ptr(bp), _lib.ptr(w1), _lib.ptr(b1),
+                                                  _lib.ptr(w2), _lib.ptr(b2), ctypes.c_void_p(yb.data_ptr() + 2 * GUARD), cs,
+                                                  _lib.ptr(wy), _lib.ptr(by), _lib.stream_ptr()))
+        outb, width, x_in = yb, cs, x0[GUARD:GUARD + T * C].view(T, C)
+    else:
+        _lib.check(lib.nb200_swin_mlp_fused_f16(xp, _lib.ptr(att), T, C, _lib.ptr(wp), _lib.ptr(bp), _lib.ptr(w1), _lib.ptr(b1),
+                                                _lib.ptr(w2), _lib.ptr(b2), _lib.stream_ptr()))
+        outb, width, x_in = xb, C, x0[GUARD:GUARD + T * C].view(T, C)
+    torch.cuda.synchronize()
+    bad = []
+    got = outb[GUARD:GUARD + T * width].view(T, width)
+    if bool(torch.isnan(got).any()):
+        bad.append("NaN in the output")
+    if not bool((bits(outb[:GUARD]) == SENTINEL).all() and (bits(outb[GUARD + T * width:]) == SENTINEL).all()):
+        bad.append("guard changed")
+    if cs and not torch.equal(bits(xb), bits(x0)):
+        bad.append("x changed although y was requested")
+    worst, over = 0.0, 0
+    rows = 1 << 16
+    for t0 in range(0, T, rows):
+        t1 = min(T, t0 + rows)
+        ref, bound = mlp_reference(x_in[t0:t1], att[t0:t1] if proj else None, wp, bp, w1, b1, w2, b2, wy, by)
+        ratio = (got[t0:t1].double() - ref).abs() / bound
+        worst = max(worst, float(ratio.max()))
+        over += int((ratio > 1).sum())
+    return worst, over, bad
+
+
+def test_swin_mlp_replay(production):
+    cases = _unique(production, "swin_mlp", SYNTH_SWIN_MLP)
+    t0, worst, fails = time.time(), 0.0, []
+    for name, r in cases:
+        ratio, over, bad = swin_mlp_check(r, _seed(name, tuple(r.values())))
+        cfg = ",".join(f"{f}={r[f]}" for f in FIELDS["swin_mlp"])
+        log_metric("replay_swin_mlp", model=name, cfg=cfg, err_over_bound=f"{ratio:.3g}")
+        worst = max(worst, ratio)
+        if bad or over:
+            fails.append(f"{name} {cfg}: {bad} max err/bound {ratio:.3g}, {over} elements over")
+    print(f"\nswin tail: {len(cases)} configurations, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
+    log_metric("replay_swin_mlp_summary", configs=len(cases), worst=worst)
+    assert not fails, "\n".join(fails[:20])
