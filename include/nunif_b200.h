@@ -399,6 +399,40 @@ int nb200_conv_gemm_ex_f16(const nb200_gemm_desc* desc, const void* A, const voi
 int nb200_flash_attention_f16(const void* qkv, void* out, int B, int N, int heads, const float* bias_log2e, int ldb,
                               void* stream);
 
+/* The WindowMHA2d core of the WABlock (row_flow_v3, mlbw, depth_aa; csrc/window_mha.h): qkv fp16 [B][H][W][3C] (q | k | v),
+ * ws x ws windows, `heads` heads of C / heads channels, bias fp32 [N][N] (N = ws * ws) added to the scaled scores,
+ * out fp16 [B][H][W][C].  pad_y / pad_x are 0 or ws / 2 (a shifted direction; the padded grid must tile into whole windows):
+ * padded tokens have k | v = qkv_bias[C..3C) (fp32, required with padding).  Layouts: 3x3 and 4x4 with 2 heads of 32, 4x4
+ * with 4 heads of 32, 8x8 with 2 heads of 16. */
+int nb200_window_mha_f16(const void* qkv, const float* qkv_bias, const float* bias, void* out, int B, int H, int W, int C,
+                         int ws, int heads, int pad_y, int pad_x, void* stream);
+/* ReplicationPad2d(1) of x fp16 [B][H][W][C] -> out [B][H+2][W+2][C]; C % 8 == 0. */
+int nb200_reppad1_f16(const void* x, int B, int H, int W, int C, void* out, void* stream);
+/* The ViT block's residual add + LayerNorm (eps 1e-6) on the fp32 residual stream: x32 [rows][dim] += fp32(delta) (delta
+ * fp16, may be NULL: no add, x32 is not written), out fp16 = LayerNorm(x32) * w + b (may be NULL: no output).
+ * dim in {256, 384, 768, 1024}. */
+int nb200_add_layernorm_f32(float* x32, const void* delta, const float* w, const float* b, void* out, long long rows, int dim,
+                            void* stream);
+/* Bilinear resize, align_corners=True, of x fp16 [B][h][w][C] -> out [B][H][W][C] (fp32 interpolation); C % 8 == 0. */
+int nb200_upsample_bilinear_f16(const void* x, int B, int h, int w, int C, void* out, int H, int W, void* stream);
+
+/* ZoeDepth bins head kernels (csrc/zoe_kernels.h, where each is specified): y = e + bilinear(prev) (fp16 NHWC, C % 8 == 0);
+ * out = softplus(x) (fp32); the normed seed bin centres; the attractor layer (normed = 0: AttractorLayerUnnormed, sorted
+ * must be NULL; normed = 1: AttractorLayer, sorted optional); the ConditionalLogBinomial input concat and its final 4-output
+ * conv + log-binomial mixture; and the BEiT relative-position bias expansion (bias [heads][N][ldb], N = ph * pw + 1,
+ * columns N..ldb-1 are not written). */
+int nb200_zoe_add_upsampled_f16(const void* e, const void* prev, int B, int h, int w, int C, int H, int W, void* y,
+                                void* stream);
+int nb200_zoe_softplus_f32(const void* x, float* out, long long n, void* stream);
+int nb200_zoe_seed_normed_f32(const void* s, long long npix, float min_depth, float max_depth, float* out, void* stream);
+int nb200_zoe_attractor_f32(const void* apre, int lda, int na, const float* prev_bin, int B, int h, int w, int H, int W,
+                            int normed, float min_depth, float max_depth, float* out, float* sorted, void* stream);
+int nb200_zoe_clb_concat_f16(const void* act, const float* rel, const void* emb, int B, int h, int w, int H, int W, void* A,
+                             void* stream);
+int nb200_zoe_clb_final_f32(const void* g, int ldg, const float* w2, const float* b2, const float* bins, int B, int h, int w,
+                            int H, int W, float* depth, void* stream);
+int nb200_zoe_expand_rel_bias_f32(const float* table, int ph, int pw, int heads, float* bias, int ldb, void* stream);
+
 /* shifted-window attention core between the qkv and proj Linears
  * (torchvision swin_transformer.py:166-221), window 6x6, 6 heads.
  * qkv: three dense planes q | k | v, each [B][H][W][C] fp16 (how the engine's qkv GEMM writes them)
@@ -480,13 +514,19 @@ int nb200_profile_enable(int on);
 int nb200_profile_report(char* buf, size_t cap);
 int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launch: class,ms,work,read_bytes,write_bytes */
 
-/* Launch recorder for tests: on = 1 clears the record and appends one CSV line per launch of the implicit GEMM, the ViT
- * attention and the fused Swin-block head and tail; on = 0 stops.  Off by default; recording changes no launch.  Lines:
+/* Launch recorder for tests: a non-zero `on` clears the record and appends one CSV line per launch of the kinds its bits
+ * select; on = 0 stops.  Bit 0 (on = 1): the implicit GEMM, the ViT attention and the fused Swin-block head and tail (gemm,
+ * attn, swin_attn, swin_mlp).  Bit 1 (on = 2): the WABlock core and pad, the ViT add + LayerNorm, the DPT upsample and the
+ * ZoeDepth bins head (the other kinds below).  Other bits are refused.  Off by default; recording changes no launch.  Lines
+ * (has_* / normed: 0 or 1):
  *   gemm,kind,pad,dil,B,Hi,Wi,Ci,Cin,a_row_stride,a_img_stride,a_planes,a_plane_stride,N,act,ldo,out_mode,cout,
  *        split_stride,has_bias,has_res,ldr,res_H,res_W,res_cy,res_cx,res_before_act,has_A2,Cin2,ld2,out_is_res,out_is_A,
  *        block_n,bk,grid
  *   attn,B,N,heads,has_bias,ldb      swin_attn,B,H,W,C,shift      swin_mlp,T,C,proj,cs
- * recorded_launches copies them (NUL-terminated) like nb200_profile_dump; it fails if cap is too small. */
+ *   wmha,B,H,W,C,ws,heads,pad_y,pad_x      reppad,B,H,W,C      ln,rows,dim,has_delta,has_out      upbl,B,h,w,C,H,W
+ *   zadd_up,B,h,w,C,H,W      zsoftplus,n      zseed,npix,min,max      zattr,B,h,w,H,W,lda,na,normed,min,max,has_sorted
+ *   zclb_concat,B,h,w,H,W      zclb_final,B,h,w,H,W,ldg      zrelbias,ph,pw,heads,ldb
+ * (min / max: fp32 depths printed with 9 significant digits, 0 for an unnormed attractor).  recorded_launches copies them (NUL-terminated) like nb200_profile_dump; it fails if cap is too small. */
 int nb200_record_launches(int on);
 int nb200_recorded_launches(char* buf, size_t cap);
 

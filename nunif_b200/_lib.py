@@ -128,6 +128,18 @@ SIGNATURES = {
     "nb200_conv_gemm_ex_f16": (c_int, [ctypes.POINTER(GemmDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                        c_void_p]),
     "nb200_flash_attention_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "nb200_window_mha_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 8 + [c_void_p]),
+    "nb200_reppad1_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "nb200_add_layernorm_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p]),
+    "nb200_upsample_bilinear_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "nb200_zoe_add_upsampled_f16": (c_int, [c_void_p, c_void_p] + [c_int] * 6 + [c_void_p, c_void_p]),
+    "nb200_zoe_softplus_f32": (c_int, [c_void_p, c_void_p, ctypes.c_longlong, c_void_p]),
+    "nb200_zoe_seed_normed_f32": (c_int, [c_void_p, ctypes.c_longlong, c_float, c_float, c_void_p, c_void_p]),
+    "nb200_zoe_attractor_f32": (c_int, [c_void_p, c_int, c_int, c_void_p] + [c_int] * 6 + [c_float, c_float, c_void_p, c_void_p,
+                                                                                            c_void_p]),
+    "nb200_zoe_clb_concat_f16": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_void_p]),
+    "nb200_zoe_clb_final_f32": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_void_p]),
+    "nb200_zoe_expand_rel_bias_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "nb200_swin_mlp_fused_y_f16": (c_int, [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "nb200_record_launches": (c_int, [c_int]),

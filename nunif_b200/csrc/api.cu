@@ -160,16 +160,17 @@ extern "C" int nb200_profile_dump(char* buf, size_t cap) {
     return 0;
 }
 
-// Launch recorder: on = 1 clears the record and starts appending, on = 0 stops (the record stays readable).  Host only: a
-// launch made while it is off costs one relaxed atomic load.
+// Launch recorder: a non-zero mask (REC_GEMMS | REC_AUX bits, common.cuh) clears the record and starts appending the kinds it
+// selects, 0 stops (the record stays readable).  Host only: a launch made while it is off costs one relaxed atomic load.
 extern "C" int nb200_record_launches(int on) {
+    NB_CHECK((on & ~(REC_GEMMS | REC_AUX)) == 0, "unknown recorder bits");
     std::lock_guard<std::mutex> lk(g_rec_mu);
     if (on) g_rec.clear();
-    g_rec_enabled.store(on ? 1 : 0);
+    g_rec_enabled.store(on);
     return 0;
 }
 
-// One CSV line per recorded launch; the first field names the kind (gemm, attn, swin_attn, swin_mlp), see the header.
+// One CSV line per recorded launch; the first field names the kind (gemm, attn, swin_attn, swin_mlp, wmha, ln, z...: see the header).
 extern "C" int nb200_recorded_launches(char* buf, size_t cap) {
     NB_CHECK(buf && cap > 0, "null buffer");
     std::lock_guard<std::mutex> lk(g_rec_mu);

@@ -59,11 +59,14 @@ struct ProfScope {
     }
 };
 
-// ---- optional launch recorder (nb200_record_launches): the GEMM, ViT attention and fused Swin-block host code append one CSV
-// line per launch describing it without its pointers, so tests can replay every configuration a network uses
+// ---- optional launch recorder (nb200_record_launches): the host code of the recorded kernels appends one CSV line per launch
+// describing it without its pointers, so tests can replay every configuration a network uses.  The recorder's mask selects
+// the kinds: REC_GEMMS the GEMM, ViT attention and fused Swin block; REC_AUX the WABlock core, add + LayerNorm, DPT upsample
+// and ZoeDepth bins head.
+enum { REC_GEMMS = 1, REC_AUX = 2 };
 extern std::atomic<int> g_rec_enabled;
 void rec_append(const char* line);
-inline bool rec_on() { return g_rec_enabled.load(std::memory_order_relaxed) != 0; }
+inline bool rec_on(int kinds = REC_GEMMS) { return (g_rec_enabled.load(std::memory_order_relaxed) & kinds) != 0; }
 
 // seam_blend.cu: rows [y0, y1) of the blended output (used by the band-pipelined host render in model.cu)
 int tile_gather_blend_rows(const void* z_all, int z_f32, int C, const ::nb200_tile_config* cfg, int scale, int offset, int tile_size,

@@ -409,6 +409,11 @@ int da_assemble_tokens(cudaStream_t st, const __half* T, const float* cls, const
 
 int da_add_layernorm(cudaStream_t st, float* X32, const __half* delta, const float* w, const float* b, __half* out, long long rows,
                      int dim) {
+    if (rec_on(REC_AUX)) {
+        char line[96];
+        snprintf(line, sizeof(line), "ln,%lld,%d,%d,%d", rows, dim, delta ? 1 : 0, out ? 1 : 0);
+        rec_append(line);
+    }
     const unsigned grid = (unsigned)cdiv64(rows, 8);
     switch (dim) {
         case 256: add_layernorm_kernel<256><<<grid, 256, 0, st>>>(X32, delta, w, b, out, rows); break;
@@ -451,6 +456,11 @@ int da_relu_add(cudaStream_t st, const __half* x, const __half* x0, __half* y, _
 }
 
 int da_upsample_bilinear(cudaStream_t st, const __half* x, int B, int h, int w, int C, __half* out, int H, int W) {
+    if (rec_on(REC_AUX)) {
+        char line[96];
+        snprintf(line, sizeof(line), "upbl,%d,%d,%d,%d,%d,%d", B, h, w, C, H, W);
+        rec_append(line);
+    }
     NB_CHECK(C % 8 == 0, "channels must be a multiple of 8");
     const float sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
     const long long total = (long long)B * H * W * (C / 8);
@@ -489,4 +499,16 @@ extern "C" int nb200_flash_attention_f16(const void* qkv, void* out, int B, int 
                                          void* stream) {
     NB_CHECK(qkv && out && B > 0 && N > 0 && heads > 0, "bad arguments");
     return nb200::da_attention((cudaStream_t)stream, (const __half*)qkv, (__half*)out, B, N, heads, bias_log2e, ldb);
+}
+
+// The residual add + LayerNorm of every ViT block and the DPT head's bilinear upsample (include/nunif_b200.h)
+extern "C" int nb200_add_layernorm_f32(float* x32, const void* delta, const float* w, const float* b, void* out, long long rows, int dim,
+                                       void* stream) {
+    NB_CHECK(x32 && w && b && rows > 0, "bad arguments");
+    return nb200::da_add_layernorm((cudaStream_t)stream, x32, (const __half*)delta, w, b, (__half*)out, rows, dim);
+}
+
+extern "C" int nb200_upsample_bilinear_f16(const void* x, int B, int h, int w, int C, void* out, int H, int W, void* stream) {
+    NB_CHECK(x && out && B > 0 && h > 0 && w > 0 && C > 0 && H > 0 && W > 0, "bad arguments");
+    return nb200::da_upsample_bilinear((cudaStream_t)stream, (const __half*)x, B, h, w, C, (__half*)out, H, W);
 }

@@ -136,7 +136,17 @@ __global__ void __launch_bounds__(256) reppad1_kernel(const uint4* __restrict__ 
 
 int window_mha(cudaStream_t st, const __half* qkv, const float* qkv_bias, const float* bias, __half* out, int B, int H, int W, int C,
                int ws, int heads, int pad_y, int pad_x) {
+    if (rec_on(REC_AUX)) {
+        char line[128];
+        snprintf(line, sizeof(line), "wmha,%d,%d,%d,%d,%d,%d,%d,%d", B, H, W, C, ws, heads, pad_y, pad_x);
+        rec_append(line);
+    }
     NB_CHECK(H % ws == 0 && W % ws == 0, "token grid must be a multiple of the window");
+    // a shifted direction pads ws / 2 on both sides; the padded grid must still tile into whole windows (not so for odd ws)
+    NB_CHECK((pad_y == 0 || pad_y == ws / 2) && (pad_x == 0 || pad_x == ws / 2), "padding must be 0 or ws / 2");
+    NB_CHECK((H + 2 * pad_y) % ws == 0 && (W + 2 * pad_x) % ws == 0, "padded token grid must be a multiple of the window");
+    NB_CHECK(qkv_bias || (pad_y == 0 && pad_x == 0), "padding needs the qkv bias");
+    NB_CHECK(C % heads == 0, "channels must split evenly into heads");
     const int nwx = (W + 2 * pad_x) / ws, nwy = (H + 2 * pad_y) / ws, hd = C / heads;
     const long long nwin = (long long)B * nwx * nwy;
     if (ws == 3 && hd == 32 && heads == 2) return launch_window_mha<3, 32, 2>(st, qkv, qkv_bias, bias, out, H, W, pad_y, pad_x, nwx, nwy, nwin);
@@ -148,6 +158,11 @@ int window_mha(cudaStream_t st, const __half* qkv, const float* qkv_bias, const 
 }
 
 int reppad1(cudaStream_t st, const __half* x, int B, int H, int W, int C, __half* out) {
+    if (rec_on(REC_AUX)) {
+        char line[96];
+        snprintf(line, sizeof(line), "reppad,%d,%d,%d,%d", B, H, W, C);
+        rec_append(line);
+    }
     NB_CHECK(C % 8 == 0, "channels must be a multiple of 8");
     const long long total = (long long)B * (H + 2) * (W + 2) * (C / 8);
     reppad1_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out), B, H, W, C / 8);
@@ -156,3 +171,15 @@ int reppad1(cudaStream_t st, const __half* x, int B, int H, int W, int C, __half
 }
 
 }  // namespace nb200
+
+// Test entry points of the WABlock kernels (include/nunif_b200.h)
+extern "C" int nb200_window_mha_f16(const void* qkv, const float* qkv_bias, const float* bias, void* out, int B, int H, int W, int C,
+                                    int ws, int heads, int pad_y, int pad_x, void* stream) {
+    NB_CHECK(qkv && bias && out && B > 0 && H > 0 && W > 0 && C > 0 && ws > 0 && heads > 0, "bad arguments");
+    return nb200::window_mha((cudaStream_t)stream, (const __half*)qkv, qkv_bias, bias, (__half*)out, B, H, W, C, ws, heads, pad_y, pad_x);
+}
+
+extern "C" int nb200_reppad1_f16(const void* x, int B, int H, int W, int C, void* out, void* stream) {
+    NB_CHECK(x && out && B > 0 && H > 0 && W > 0 && C > 0, "bad arguments");
+    return nb200::reppad1((cudaStream_t)stream, (const __half*)x, B, H, W, C, (__half*)out);
+}
