@@ -339,6 +339,41 @@ int nb200_ema_scaler_normalize(nb200_ema_scaler* s, const float* frame, int n, i
 /* iw3/mapper.py:29-32 get_mapper("div_*") alone: distance_to_disparity(x, mapper_c); in place allowed. */
 int nb200_depth_mapper(const float* depth, long long n, float mapper_c, float* out, void* stream);
 
+/* Disparity mapper descriptor: iw3/mapper.py:129-151 get_mapper(name) parsed once on the host
+ * (nunif_b200/iw3/mapper.py) into up to NB200_MAPPER_MAX_STAGES chained stages, each one function
+ * (resolve_mapper_function, :64-120) or the blend a(x)*(1-w) + b(x)*w (:136-147).  Every constant
+ * is already rounded to fp32 the way the reference rounds it, so the device evaluates in fp32 in the
+ * reference's op order (csrc/mapper.cuh).  Function kinds and their constants k[]:
+ *   0 none  identity                        1 pow2  x*x
+ *   2 softplus  softplus01_legacy (:7-11)   3 softplus2  its square           k = {min_v, max_v - min_v}
+ *   4 softplus01 (mul_*, :14-19)            k = {bias, scale, min_v, max_v - min_v}
+ *   5 inv_softplus01 (inv_mul_*, :22-26)    k = {bias, scale, min_v, max_v - min_v}  (fp32 tensor values)
+ *   6 distance_to_disparity (div_*, :29-32) k = {c, 1 + c, c / (1 + c), 1 - c / (1 + c)}
+ *   7 shift_relative_depth (shift_*, :39-61) k = {A, B, 1 - min_distance, 1 / 17, 1 - 1 / 17}
+ * n_stages = 0 is "none".  Fixed size: 528 bytes. */
+#define NB200_MAPPER_MAX_STAGES 8
+typedef struct nb200_mapper_fn {
+    int32_t kind;
+    float k[5];
+} nb200_mapper_fn;
+typedef struct nb200_mapper_stage {
+    nb200_mapper_fn a, b;         /* b is read only when blend != 0 */
+    int32_t blend;
+    float one_minus_w, w, pad;
+} nb200_mapper_stage;
+typedef struct nb200_mapper {
+    int32_t n_stages, pad[3];
+    nb200_mapper_stage stage[NB200_MAPPER_MAX_STAGES];
+} nb200_mapper;
+
+/* iw3/utils.py:310 get_mapper(args.mapper)(depth) for any mapper name: out = mapper(depth), n elements;
+ * in place allowed. */
+int nb200_mapper_apply(const float* depth, long long n, const nb200_mapper* mapper_host, float* out, void* stream);
+/* nb200_minmax_map with any mapper: iw3/depth_scaler.py:4-17 per frame, then get_mapper(name)
+ * (iw3/utils.py:310), in one pass (what stereo_sbs runs).  In place allowed. */
+int nb200_minmax_mapper(const float* depth, int B, int n_per_frame, const nb200_mapper* mapper_host,
+                        float* out, float* minmax_out /* [B][2] or NULL */, void* stream);
+
 /* iw3/anaglyph.py:51-92 on already-warped eyes: l,r,out [B][3][H][W] */
 int nb200_anaglyph_dubois(const float* l, const float* r, int B, int H, int W, int clip_before,
                           float* out, void* stream);

@@ -43,6 +43,25 @@ class GemmDesc(ctypes.Structure):
                 + [(n, ctypes.c_int) for n in ("ldr", "res_H", "res_W", "res_cy", "res_cx", "res_before_act", "Cin2", "ld2")])
 
 
+MAPPER_MAX_STAGES = 8
+
+
+class MapperFn(ctypes.Structure):
+    """nb200_mapper_fn: one function of iw3/mapper.py resolve_mapper_function and its fp32 constants."""
+    _fields_ = [("kind", ctypes.c_int32), ("k", ctypes.c_float * 5)]
+
+
+class MapperStage(ctypes.Structure):
+    """nb200_mapper_stage: one function, or the blend a(x) * (1 - w) + b(x) * w."""
+    _fields_ = [("a", MapperFn), ("b", MapperFn), ("blend", ctypes.c_int32), ("one_minus_w", ctypes.c_float),
+                ("w", ctypes.c_float), ("pad", ctypes.c_float)]
+
+
+class Mapper(ctypes.Structure):
+    """nb200_mapper: a parsed get_mapper(name) chain (nunif_b200/iw3/mapper.py builds it)."""
+    _fields_ = [("n_stages", ctypes.c_int32), ("pad", ctypes.c_int32 * 3), ("stage", MapperStage * MAPPER_MAX_STAGES)]
+
+
 # name -> (restype, argtypes).  Must list every symbol declared in include/nunif_b200.h
 # (tests/test_abi.py parses the header and checks this table and the .so against it).
 SIGNATURES = {
@@ -119,6 +138,8 @@ SIGNATURES = {
     "nb200_ema_scaler_update": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(c_int), c_void_p]),
     "nb200_ema_scaler_normalize": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
     "nb200_depth_mapper": (c_int, [c_void_p, ctypes.c_longlong, c_float, c_void_p, c_void_p]),
+    "nb200_mapper_apply": (c_int, [c_void_p, ctypes.c_longlong, ctypes.POINTER(Mapper), c_void_p, c_void_p]),
+    "nb200_minmax_mapper": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(Mapper), c_void_p, c_void_p, c_void_p]),
     "nb200_anaglyph_dubois": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_conv_gemm_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
                                     c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,

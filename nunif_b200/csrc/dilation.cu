@@ -8,9 +8,10 @@
 //       is monotone in r, so w_min/w_max follow from r_min/r_max: one reduction pass
 //       instead of three.
 //   K3  x' = x*(1-w) + maxpool_k(gauss3x3_replicate(x))*w  (5x5 footprint, fused)
-// and iw3/depth_scaler.py:4-17 + iw3/mapper.py:29-32 with 2 launches.
+// and iw3/depth_scaler.py:4-17 + iw3/mapper.py (any mapper, csrc/mapper.cuh) with 2 launches.
 // These maps are ~1 MB per frame: latency-bound, reported in microseconds.
 #include "common.cuh"
+#include "mapper.cuh"
 #include "../../include/nunif_b200.h"
 
 namespace nb200 {
@@ -164,7 +165,7 @@ __global__ void __launch_bounds__(DL_THREADS) minmax_partial_kernel(const float*
 }
 
 __global__ void __launch_bounds__(DL_THREADS) minmax_apply_kernel(const float* __restrict__ x, const float2* __restrict__ partials,
-                                                                  int nblk, int n, float mapper_c, float* __restrict__ out,
+                                                                  int nblk, int n, const nb200_mapper mapper, float* __restrict__ out,
                                                                   float* __restrict__ minmax_out) {
     const int b = blockIdx.y;
     __shared__ float s_mn, s_mx;
@@ -180,15 +181,11 @@ __global__ void __launch_bounds__(DL_THREADS) minmax_apply_kernel(const float* _
     }
     __syncthreads();
     const float mn = s_mn, scale = s_mx - s_mn;
-    // mapper.py:29-32 distance_to_disparity constants (python doubles -> fp32 scalars)
-    const double c = (double)mapper_c, c1 = 1.0 + c, min_v = c / c1;
-    const float c1f = (float)c1, cf = (float)c, minvf = (float)min_v, denf = (float)(1.0 - min_v);
     for (int i = blockIdx.x * DL_THREADS + threadIdx.x; i < n; i += gridDim.x * DL_THREADS) {
         float v = x[(size_t)b * n + i];
         if (scale > 0.f) v = (v - mn) / scale;  // depth_scaler.py:9-12
         v = clamp01(v);
-        if (mapper_c >= 0.f) v = ((cf / (c1f - v)) - minvf) / denf;
-        out[(size_t)b * n + i] = v;
+        out[(size_t)b * n + i] = mapper_eval(mapper, v);
     }
 }
 
@@ -245,8 +242,8 @@ extern "C" int nb200_dilate_edge(const float* x, int B, int h, int w, int x_iter
     return 0;
 }
 
-extern "C" int nb200_minmax_map(const float* depth, int B, int n_per_frame, float mapper_c, float* out,
-                                float* minmax_out, void* stream) {
+static int minmax_map(const float* depth, int B, int n_per_frame, const nb200_mapper& mapper, float* out,
+                      float* minmax_out, void* stream) {
     NB_CHECK(depth && out, "null pointer");
     cudaStream_t st = (cudaStream_t)stream;
     const int nblk = dl_blocks(n_per_frame);
@@ -255,8 +252,20 @@ extern "C" int nb200_minmax_map(const float* depth, int B, int n_per_frame, floa
     ProfScope ps(st, PC_MINMAX, (double)B * n_per_frame * 4 * 3);
     minmax_partial_kernel<<<dim3(nblk, B), DL_THREADS, 0, st>>>(depth, partials, n_per_frame);
     NB_LAUNCHED();
-    minmax_apply_kernel<<<dim3(nblk, B), DL_THREADS, 0, st>>>(depth, partials, nblk, n_per_frame, mapper_c, out, minmax_out);
+    minmax_apply_kernel<<<dim3(nblk, B), DL_THREADS, 0, st>>>(depth, partials, nblk, n_per_frame, mapper, out, minmax_out);
     NB_LAUNCHED();
     NB_CUDA(cudaFreeAsync(partials, st));
     return 0;
+}
+
+extern "C" int nb200_minmax_map(const float* depth, int B, int n_per_frame, float mapper_c, float* out,
+                                float* minmax_out, void* stream) {
+    return minmax_map(depth, B, n_per_frame, mapper_from_c(mapper_c), out, minmax_out, stream);
+}
+
+extern "C" int nb200_minmax_mapper(const float* depth, int B, int n_per_frame, const nb200_mapper* mapper_host, float* out,
+                                   float* minmax_out, void* stream) {
+    NB_CHECK(mapper_host, "null mapper");
+    NB_CHECK(!*mapper_invalid(*mapper_host), mapper_invalid(*mapper_host));
+    return minmax_map(depth, B, n_per_frame, *mapper_host, out, minmax_out, stream);
 }

@@ -5,10 +5,11 @@
 //   ema_step_kernel       MinMaxBuffer.add (:46-58: the first add fills every slot, later adds are ring writes), ring
 //                         amin/amax (:63-64), EMA update min = decay*min + (1-decay)*new (:108-113, fp32 like torch)
 //   ema_normalize_kernel  (x - min) / (max - min) clamp[0,1] (:4-17) or x / max (:20-31) with the DEVICE-resident values,
-//                         optionally followed by the disparity mapper (iw3/mapper.py:29-32)
+//                         optionally followed by the disparity mapper (iw3/mapper.py, csrc/mapper.cuh)
 // Whether the look-ahead buffer is filled (and so whether a frame comes out) depends only on call counts: the host
 // mirror (nunif_b200/iw3/depth_scaler.py) tracks that without reading the device.
 #include "common.cuh"
+#include "mapper.cuh"
 #include "../../include/nunif_b200.h"
 
 namespace nb200 {
@@ -78,21 +79,19 @@ __global__ void __launch_bounds__(ER_THREADS) ema_step_kernel(float* __restrict_
 
 // mode 0: minmax_normalize, 1: max_normalize; mm == nullptr: no normalisation (mapper only)
 __global__ void __launch_bounds__(ER_THREADS) ema_normalize_kernel(const float* __restrict__ x, int n, const float* __restrict__ mm, int mode,
-                                                                   float mapper_c, float* __restrict__ out, float* __restrict__ mm_out) {
+                                                                   const nb200_mapper mapper, float* __restrict__ out,
+                                                                   float* __restrict__ mm_out) {
     float mn = 0.f, mx = 0.f;
     if (mm) { mn = mm[0]; mx = mm[1]; }
     if (mm_out && blockIdx.x == 0 && threadIdx.x == 0) { mm_out[0] = mn; mm_out[1] = mx; }
     const float scale = mode == 0 ? mx - mn : mx;
-    const double c = (double)mapper_c, c1 = 1.0 + c, min_v = c / c1;
-    const float c1f = (float)c1, cf = (float)c, minvf = (float)min_v, denf = (float)(1.0 - min_v);
     for (int i = blockIdx.x * ER_THREADS + threadIdx.x; i < n; i += gridDim.x * ER_THREADS) {
         float v = x[i];
         if (mm) {
             if (scale > 0.f) v = mode == 0 ? (v - mn) / scale : v / scale;
             v = clamp01(v);
         }
-        if (mapper_c >= 0.f) v = ((cf / (c1f - v)) - minvf) / denf;
-        out[i] = v;
+        out[i] = mapper_eval(mapper, v);
     }
 }
 
@@ -180,18 +179,30 @@ extern "C" int nb200_ema_scaler_normalize(nb200_ema_scaler* s, const float* fram
     NB_CHECK(from_ring || s->has_value, "the look-ahead buffer is not filled yet");
     cudaStream_t st = (cudaStream_t)stream;
     ProfScope ps(st, PC_MINMAX, (double)n * 8);
-    ema_normalize_kernel<<<er_blocks(n), ER_THREADS, 0, st>>>(frame, n, s->state + (from_ring ? 2 : 0), s->mode, mapper_c, out, minmax_out);
+    ema_normalize_kernel<<<er_blocks(n), ER_THREADS, 0, st>>>(frame, n, s->state + (from_ring ? 2 : 0), s->mode, mapper_from_c(mapper_c),
+                                                              out, minmax_out);
+    NB_LAUNCHED();
+    return 0;
+}
+
+static int mapper_apply(const float* depth, long long n, const nb200_mapper& mapper, float* out, void* stream) {
+    NB_CHECK(depth && out, "null pointer");
+    NB_CHECK(n > 0 && n < (1ll << 31), "bad size");
+    cudaStream_t st = (cudaStream_t)stream;
+    ema_normalize_kernel<<<er_blocks((int)n), ER_THREADS, 0, st>>>(depth, (int)n, nullptr, 0, mapper, out, nullptr);
     NB_LAUNCHED();
     return 0;
 }
 
 // disparity mapper alone (iw3/mapper.py:29-32 div_*: distance_to_disparity(x, c)); in place allowed
 extern "C" int nb200_depth_mapper(const float* depth, long long n, float mapper_c, float* out, void* stream) {
-    NB_CHECK(depth && out, "null pointer");
-    NB_CHECK(n > 0 && n < (1ll << 31), "bad size");
     NB_CHECK(mapper_c >= 0.f, "mapper constant must be >= 0");
-    cudaStream_t st = (cudaStream_t)stream;
-    ema_normalize_kernel<<<er_blocks((int)n), ER_THREADS, 0, st>>>(depth, (int)n, nullptr, 0, mapper_c, out, nullptr);
-    NB_LAUNCHED();
-    return 0;
+    return mapper_apply(depth, n, mapper_from_c(mapper_c), out, stream);
+}
+
+// any mapper alone (iw3/mapper.py:129-151 get_mapper(name)(x)); in place allowed
+extern "C" int nb200_mapper_apply(const float* depth, long long n, const nb200_mapper* mapper_host, float* out, void* stream) {
+    NB_CHECK(mapper_host, "null mapper");
+    NB_CHECK(!*mapper_invalid(*mapper_host), mapper_invalid(*mapper_host));
+    return mapper_apply(depth, n, *mapper_host, out, stream);
 }

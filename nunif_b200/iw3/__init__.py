@@ -10,6 +10,8 @@ from .backward_warp import apply_divergence_grid_sample  # noqa: F401
 from .forward_warp import apply_divergence_forward_warp  # noqa: F401
 from .dilation import dilate_edge, edge_dilation_parse, edge_dilation_is_enabled, mask_closing, dilate_outer, dilate_inner  # noqa: F401
 from .depth_scaler import minmax_normalize, depth_mapper, EMAMinMaxScaler  # noqa: F401
+from .mapper import get_mapper, resolve_mapper_name, get_mapper_levels  # noqa: F401
+from .mapper import METRIC_DIV_MAPPER, RELATIVE_MUL_MAPPER, RELATIVE_SHIFT_MAPPER, LEGACY_MAPPER, MAPPER_ALL  # noqa: F401
 from .base_depth_model import BaseDepthModel  # noqa: F401
 from .anaglyph import apply_anaglyph_redcyan  # noqa: F401
 from .stereo import stereo_sbs  # noqa: F401

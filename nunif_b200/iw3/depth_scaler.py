@@ -1,46 +1,34 @@
 """Mirror of iw3/depth_scaler.py: the stateless per-frame normaliser (:4-17, with the disparity mapper of
-iw3/mapper.py fused into the same pass) and the stateful ``EMAMinMaxScaler`` (:64-142) whose min/max ring and EMA
+iw3/mapper.py, nunif_b200/iw3/mapper.py, fused into the same pass) and the stateful ``EMAMinMaxScaler`` (:64-142) whose min/max ring and EMA
 values live on the device (csrc/ema_scaler.cu) - no host synchronisation per frame."""
 import ctypes
 import torch
 from .. import _lib
 from ._common import prep
-
-_DIV_C = {"div_25": 2.5, "div_10": 1.0, "div_6": 0.6, "div_4": 0.4, "div_2": 0.2, "div_1": 0.1}  # mapper.py:106-113
+from .mapper import descriptor, apply_mapper
 
 
 def minmax_normalize(depth, mapper="none", return_minmax=False):
-    """depth: B,1,h,w (or 1,h,w): per-frame (x-min)/(max-min) clamp[0,1], then mapper
-    ("none" or "div_*").  No host sync (the reference's ``if scale > 0`` syncs)."""
+    """depth: B,1,h,w (or 1,h,w): per-frame (x-min)/(max-min) clamp[0,1], then get_mapper(mapper) (any name of
+    iw3/mapper.py, blends and chains included) in the same pass.  No host sync (the reference's ``if scale > 0``
+    syncs)."""
     squeeze = depth.ndim == 3
     d = prep(depth.unsqueeze(0) if squeeze else depth, "depth")
-    if mapper == "none":
-        c = -1.0
-    elif mapper in _DIV_C:
-        c = _DIV_C[mapper]
-    else:
-        raise NotImplementedError(f"mapper={mapper}")
+    desc = descriptor(mapper)
     B = d.shape[0]
     n = d[0].numel()
     out = torch.empty_like(d)
     mm = torch.empty((B, 2), device=d.device, dtype=torch.float32) if return_minmax else None
     with torch.cuda.device(d.device):
-        _lib.check(_lib.lib().nb200_minmax_map(_lib.ptr(d), B, n, c, _lib.ptr(out), _lib.ptr(mm), _lib.stream_ptr(d.device)))
+        _lib.check(_lib.lib().nb200_minmax_mapper(_lib.ptr(d), B, n, ctypes.byref(desc), _lib.ptr(out), _lib.ptr(mm),
+                                                  _lib.stream_ptr(d.device)))
     out = out[0] if squeeze else out
     return (out, mm) if return_minmax else out
 
 
 def depth_mapper(depth, mapper="none"):
-    """iw3/mapper.py get_mapper(name)(depth) for the names on the hot path ("none", "div_*")."""
-    if mapper == "none":
-        return depth
-    if mapper not in _DIV_C:
-        raise NotImplementedError(f"mapper={mapper}")
-    d = prep(depth, "depth")
-    out = torch.empty_like(d)
-    with torch.cuda.device(d.device):
-        _lib.check(_lib.lib().nb200_depth_mapper(_lib.ptr(d), d.numel(), _DIV_C[mapper], _lib.ptr(out), _lib.stream_ptr(d.device)))
-    return out
+    """iw3/mapper.py get_mapper(mapper)(depth) for any mapper name; an identity mapper returns ``depth`` itself."""
+    return apply_mapper(depth, descriptor(mapper))
 
 
 class EMAMinMaxScaler:

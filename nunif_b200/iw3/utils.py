@@ -4,11 +4,15 @@ layers, which stay in the reference's host code).
 
 ``args`` is the reference's argparse namespace; the fields read here are the ones the reference reads on this path:
 ``method, mapper, convergence, divergence, synthetic_view, warp_steps, preserve_screen_border, stereo_width, disable_amp,
-mask_inner_dilation, mask_outer_dilation, inpaint_max_width, state["convergence_model"]``.  A convergence model must be the
+mask_inner_dilation, mask_outer_dilation, inpaint_max_width, state["convergence_model"]``.  ``mapper`` is any name of
+iw3/mapper.py; build it from ``--foreground-scale`` / ``--mapper-type`` with ``resolve_mapper_name`` as iw3/utils.py:2341-2344
+does.  A convergence model must be the
 engine's ``ConvergenceEstimator`` (``--convergence-mode sod_v1``).  Anything the engine does not implement raises ``NotImplementedError`` - never a silent
 fallback."""
 import torch
 
+from .. import _lib
+from ._common import prep
 from .backward_warp import apply_divergence_grid_sample
 from .forward_warp import apply_divergence_forward_warp
 from .depth_scaler import depth_mapper
@@ -21,6 +25,17 @@ _WARP = {"grid_sample": "backward", "backward": "backward", "forward": "forward"
 
 def _arg(args, name, default=None):
     return getattr(args, name, default)
+
+
+def resize_depth_aa(depth, height, width):
+    """F.interpolate(depth, size=(height, width), mode="bilinear", align_corners=True, antialias=True) for a B,1,h,w
+    depth map (nb200_depth_resize_aa)."""
+    d = prep(depth, "depth")
+    B, C, h, w = d.shape
+    out = torch.empty((B, C, height, width), dtype=torch.float32, device=d.device)
+    with torch.cuda.device(d.device):
+        _lib.check(_lib.lib().nb200_depth_resize_aa(_lib.ptr(d), B * C, h, w, height, width, _lib.ptr(out), _lib.stream_ptr(d.device)))
+    return out
 
 
 def apply_divergence(depth, im, args, side_model, reset_pts=None):
@@ -68,9 +83,12 @@ def apply_divergence(depth, im, args, side_model, reset_pts=None):
                                 enable_amp=True)
     else:
         # the learned warps (row_flow*, mlbw*): apply_divergence_nn_LR with args.side_model (:363-385)
-        stereo_width = _arg(args, "stereo_width", None)
-        if stereo_width is not None and depth.shape[3] != min(im.shape[3], stereo_width):
-            raise NotImplementedError("--stereo-width depth resampling is not implemented by the H100 engine")
+        if _arg(args, "stereo_width", None) is not None:
+            # --stereo-width (:370-379): the warp runs at this width, with the frame's aspect ratio (not the depth's)
+            H, W = im.shape[2:]
+            stereo_width = min(W, args.stereo_width)
+            if depth.shape[3] != stereo_width:
+                depth = resize_depth_aa(depth, int(H * (stereo_width / W)), stereo_width).clamp_(0, 1)
         if side_model is None:
             raise ValueError(f"method {method} needs side_model")
         eyes = apply_divergence_nn_LR(side_model, im, depth, args.divergence, convergence, _arg(args, "warp_steps", None),
