@@ -468,6 +468,37 @@ int nb200_zoe_clb_final_f32(const void* g, int ldg, const float* w2, const float
                             int H, int W, float* depth, void* stream);
 int nb200_zoe_expand_rel_bias_f32(const float* table, int ph, int pw, int heads, float* bias, int ldb, void* stream);
 
+/* The hand-written convolutions of the waifu2x models and the SE block, through the host functions the networks call (so
+ * nb200_tune_set(7, 1) selects their SIMT kernels here too).  w / b / w1 / b1 / w2 / b2 are HOST fp32 tensors in the PyTorch
+ * layout (Conv2d [co][ci][kh][kw], ConvTranspose2d [ci][co][kh][kw], bias [co]), packed by the networks' own packers into a
+ * stream-ordered workspace; activations are device fp16.
+ *   stem: x [n][Hi][Wi][8] (channel 3 must be 0, channels 4..7 are not read), w [cout][3][3][3] -> out [n][Hi-2][Wi-2][ldo],
+ *         LeakyReLU(0.1); channels cout..cout_pad-1 are written as 0, cout_pad..ldo-1 are not written.  cout_pad 32 or 64.
+ *   tail: x [n][Hi][Wi][64]; mode 0: Conv2d(64, 3, 3) valid, mode 1: ConvTranspose2d(64, 3, 4, 2, 3).  epi 0: out NHWC8
+ *         [n][Ho][Wo][8] (3 channels, optional clamp(0, 1), 5 zeros); epi 1 (mode 0 only): out planar [n][3][Ho][Wo] =
+ *         clamp(conv + z1[:, 20:20+Ho, 20:20+Wo, :3]) with z1 NHWC8 [n][z1H][z1W][8].
+ *   head: x [n][Hi][Wi][cin]; mode 0 (cin 128): Conv2d(cin, 3, 3), mode 1 (cin 256): ConvTranspose2d(cin, 3, 4, 2, 3);
+ *         out planar [n][3][Ho][Wo] = clamp(conv, 0, 1).
+ *   se:   x [n][H][W][C] fp16 scaled in place by sigmoid(conv2(relu(conv1(mean over H, W)))); C 64 or 128, conv1 [C/8][C],
+ *         conv2 [C][C/8]. */
+int nb200_stem_conv_f16(const void* x, const float* w, const float* b, int cout, int cout_pad, int n, int Hi, int Wi, void* out,
+                        int ldo, void* stream);
+int nb200_tail_conv_f16(const void* x, const float* w, const float* b, int mode, int epi, int n, int Hi, int Wi, void* out,
+                        const void* z1, int z1H, int z1W, int clip, void* stream);
+int nb200_head_conv_f16(const void* x, const float* w, const float* b, int mode, int cin, int n, int Hi, int Wi, void* out,
+                        void* stream);
+int nb200_se_block_f16(void* x, const float* w1, const float* b1, const float* w2, const float* b2, int n, int H, int W, int C,
+                       void* stream);
+/* SwinUNet's to_image tail: y fp16 [n][Hs][Ws][cs] with channel c*r*r + dy*r + dx (F.pixel_shuffle) -> z planar [n][3][S][S],
+ * S = Hs * r / down; down 1: fp16 clamp(pixel_shuffle(y), 0, 1); down 2 / 4: fp32 clamp(bicubic antialias resize (ATen
+ * upsample_bicubic2d_aa) of that clamp, 0, 1).  Hs == Ws. */
+int nb200_to_image_f16(const void* y, int n, int Hs, int Ws, int cs, int r, int down, void* z, void* stream);
+/* One REBNCONV of iw3.sod_v1 (csrc/sod.cu sod_conv_kernel): out[..., out_off:out_off+cout] = fp16(relu(fp16(fp16(conv3x3(
+ * in[..., in_off:in_off+cin], dilation and padding dil)) + bias)) [+ res[..., :cout]]), NHWC fp16 with pixel strides in_ld /
+ * out_ld / res_ld (res may be NULL).  wt fp16 [cout][9][cin] (k = tap * cin + c), bias fp32; cin % 16 == 0, cout 16 or 64. */
+int nb200_sod_conv_f16(const void* in, int in_ld, int in_off, int cin, const void* wt, const float* bias, int cout, int dil,
+                       void* out, int out_ld, int out_off, const void* res, int res_ld, int B, int H, int W, void* stream);
+
 /* shifted-window attention core between the qkv and proj Linears
  * (torchvision swin_transformer.py:166-221), window 6x6, 6 heads.
  * qkv: three dense planes q | k | v, each [B][H][W][C] fp16 (how the engine's qkv GEMM writes them)
@@ -552,8 +583,9 @@ int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launc
 /* Launch recorder for tests: a non-zero `on` clears the record and appends one CSV line per launch of the kinds its bits
  * select; on = 0 stops.  Bit 0 (on = 1): the implicit GEMM, the ViT attention and the fused Swin-block head and tail (gemm,
  * attn, swin_attn, swin_mlp).  Bit 1 (on = 2): the WABlock core and pad, the ViT add + LayerNorm, the DPT upsample and the
- * ZoeDepth bins head (the other kinds below).  Other bits are refused.  Off by default; recording changes no launch.  Lines
- * (has_* / normed: 0 or 1):
+ * ZoeDepth bins head (wmha .. zrelbias).  Bit 2 (on = 4): the waifu2x stem, tail and head convolutions, the SE block,
+ * to_image and the SOD REBNCONV (stem .. sodconv; path = the kernel the host chose: 0 mma.sync, 1 SIMT).  Other bits are
+ * refused.  Off by default; recording changes no launch.  Lines (has_* / normed: 0 or 1):
  *   gemm,kind,pad,dil,B,Hi,Wi,Ci,Cin,a_row_stride,a_img_stride,a_planes,a_plane_stride,N,act,ldo,out_mode,cout,
  *        split_stride,has_bias,has_res,ldr,res_H,res_W,res_cy,res_cx,res_before_act,has_A2,Cin2,ld2,out_is_res,out_is_A,
  *        block_n,bk,grid
@@ -561,6 +593,8 @@ int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launc
  *   wmha,B,H,W,C,ws,heads,pad_y,pad_x      reppad,B,H,W,C      ln,rows,dim,has_delta,has_out      upbl,B,h,w,C,H,W
  *   zadd_up,B,h,w,C,H,W      zsoftplus,n      zseed,npix,min,max      zattr,B,h,w,H,W,lda,na,normed,min,max,has_sorted
  *   zclb_concat,B,h,w,H,W      zclb_final,B,h,w,H,W,ldg      zrelbias,ph,pw,heads,ldb
+ *   stem,n,Hi,Wi,cout_pad,ldo,path      tail,mode,epi,n,Hi,Wi,z1H,z1W,clip,path      head,mode,cin,n,Hi,Wi,path
+ *   se,n,H,W,C      toimg,n,Hs,Ws,cs,r,down      sodconv,B,H,W,cin,cout,dil,in_ld,in_off,out_ld,out_off,has_res,res_ld
  * (min / max: fp32 depths printed with 9 significant digits, 0 for an unnormed attractor).  recorded_launches copies them (NUL-terminated) like nb200_profile_dump; it fails if cap is too small. */
 int nb200_record_launches(int on);
 int nb200_recorded_launches(char* buf, size_t cap);

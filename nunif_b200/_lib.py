@@ -161,6 +161,13 @@ SIGNATURES = {
     "nb200_zoe_clb_concat_f16": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_void_p]),
     "nb200_zoe_clb_final_f32": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_void_p]),
     "nb200_zoe_expand_rel_bias_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "nb200_stem_conv_f16": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_int, c_void_p]),
+    "nb200_tail_conv_f16": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "nb200_head_conv_f16": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_void_p]),
+    "nb200_se_block_f16": (c_int, [c_void_p] * 5 + [c_int] * 4 + [c_void_p]),
+    "nb200_to_image_f16": (c_int, [c_void_p] + [c_int] * 6 + [c_void_p, c_void_p]),
+    "nb200_sod_conv_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p,
+                                   c_int, c_int, c_int, c_int, c_void_p]),
     "nb200_swin_mlp_fused_y_f16": (c_int, [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "nb200_record_launches": (c_int, [c_int]),

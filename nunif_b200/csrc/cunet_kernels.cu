@@ -93,6 +93,11 @@ __global__ void __launch_bounds__(256) se_scale_kernel(__half* __restrict__ x, c
 
 int se_block(cudaStream_t st, __half* x, int n, int H, int W, int C, const float* w1, const float* b1, const float* w2,
              const float* b2, float* partial, float* scale) {
+    if (rec_on(REC_CONV)) {
+        char line[96];
+        snprintf(line, sizeof(line), "se,%d,%d,%d,%d", n, H, W, C);
+        rec_append(line);
+    }
     const int HW = H * W, nchunks = cdiv(HW, SE_CHUNK);
     ProfScope ps(st, PC_SE, (double)n * HW * C * 2 * 3);
     if (C == 64) {
@@ -331,8 +336,14 @@ int tail_conv(cudaStream_t st, int mode, int epi, const __half* x, const float* 
     const int Ho = mode == 0 ? Hi - 2 : 2 * Hi - 4, Wo = mode == 0 ? Wi - 2 : 2 * Wi - 4;
     const size_t total = (size_t)n * Ho * Wo;
     const unsigned blocks = (unsigned)cdiv64(total, 128);
+    const bool mma = g_tune[7] == 0 && (mode == 0 || Wo % 2 == 0) && n <= 65535;
+    if (rec_on(REC_CONV)) {
+        char line[128];
+        snprintf(line, sizeof(line), "tail,%d,%d,%d,%d,%d,%d,%d,%d,%d", mode, epi, n, Hi, Wi, z1H, z1W, clip, mma ? 0 : 1);
+        rec_append(line);
+    }
     ProfScope ps(st, PC_TAIL, (double)n * Hi * Wi * 128 + (double)total * 16);
-    if (g_tune[7] == 0 && (mode == 0 || Wo % 2 == 0) && n <= 65535) {
+    if (mma) {
         int rc;
         if (mode == 0 && epi == 0) rc = launch_tail_mma<0, 0>(st, x, wt, bias, out, z1, n, Hi, Wi, Ho, Wo, z1H, z1W, clip);
         else if (mode == 0 && epi == 1) rc = launch_tail_mma<0, 1>(st, x, wt, bias, out, z1, n, Hi, Wi, Ho, Wo, z1H, z1W, clip);

@@ -216,10 +216,10 @@ __global__ void __launch_bounds__(256) head_conv_mma_kernel(const __half* __rest
 }
 
 template <int MODE, int CIN>
-static int launch_head(cudaStream_t st, const __half* x, const float* wt, const float* bias, __half* out, int n, int Hi, int Wi,
-                       int Ho, int Wo) {
+static int launch_head(cudaStream_t st, bool mma, const __half* x, const float* wt, const float* bias, __half* out, int n, int Hi,
+                       int Wi, int Ho, int Wo) {
     using Cfg = HeadCfg<MODE>;
-    if (g_tune[7] == 0 && (MODE == 0 || Wo % 2 == 0) && n <= 65535) {
+    if (mma) {
         if (ensure_dyn_smem((const void*)head_conv_mma_kernel<MODE, CIN>, Cfg::SMEM)) return 1;
         const int npx = MODE == 1 ? Wo / 2 : Wo;
         const dim3 grid(cdiv(npx, 64), MODE == 0 ? cdiv(Ho, 2) : cdiv(Ho + 1, 2), n);
@@ -238,10 +238,16 @@ int head_conv(cudaStream_t st, int mode, int cin, const __half* x, const float* 
               int Wi) {
     const int Ho = mode == 0 ? Hi - 2 : 2 * Hi - 4, Wo = mode == 0 ? Wi - 2 : 2 * Wi - 4;
     NB_CHECK(Ho > 0 && Wo > 0, "head_conv: input too small");
+    const bool mma = g_tune[7] == 0 && (mode == 0 || Wo % 2 == 0) && n <= 65535;
+    if (rec_on(REC_CONV)) {
+        char line[96];
+        snprintf(line, sizeof(line), "head,%d,%d,%d,%d,%d,%d", mode, cin, n, Hi, Wi, mma ? 0 : 1);
+        rec_append(line);
+    }
     const double rbytes = (double)n * Hi * Wi * cin * 2, wbytes = (double)n * Ho * Wo * 3 * 2;
     ProfScope ps(st, PC_TAIL, rbytes + wbytes, rbytes, wbytes);
-    if (mode == 0 && cin == 128) return launch_head<0, 128>(st, x, wt, bias, out, n, Hi, Wi, Ho, Wo);
-    if (mode == 1 && cin == 256) return launch_head<1, 256>(st, x, wt, bias, out, n, Hi, Wi, Ho, Wo);
+    if (mode == 0 && cin == 128) return launch_head<0, 128>(st, mma, x, wt, bias, out, n, Hi, Wi, Ho, Wo);
+    if (mode == 1 && cin == 256) return launch_head<1, 256>(st, mma, x, wt, bias, out, n, Hi, Wi, Ho, Wo);
     return fail("head_conv: unsupported (mode, input channels)");
 }
 

@@ -164,15 +164,11 @@ static Lin pack_convT2(Packer& pk, const std::string& name, int cin, int cout) {
     l.b = pk.add_f32(bv);
     return l;
 }
-// first 3x3 conv from 3 channels, fp32 [27][cout_pad] with k = (ky*3+kx)*3 + ci
-static Lin pack_stem(Packer& pk, const std::string& name, int cout, int cout_pad) {
-    Lin l;
-    l.N = cout_pad;
-    l.K = 27;
-    const float* w = pk.get(name + ".weight", (int64_t)cout * 27);
-    const float* b = pk.get(name + ".bias", cout);
-    if (!w || !b) return l;
-    std::vector<float> wv((size_t)27 * cout_pad, 0.f), bv(cout_pad, 0.f);
+// first 3x3 conv from 3 channels: Conv2d weight [cout][3][3][3] and bias [cout] -> wv = fp32 [27][cout_pad] with
+// k = (ky*3+kx)*3 + ci, then the mma.sync B fragments; bv = bias [cout_pad] (both zero padded)
+static void pack_stem_w(const float* w, const float* b, int cout, int cout_pad, std::vector<float>& wv, std::vector<float>& bv) {
+    wv.assign((size_t)27 * cout_pad, 0.f);
+    bv.assign(cout_pad, 0.f);
     for (int co = 0; co < cout; ++co)
         for (int ci = 0; ci < 3; ++ci)
             for (int k = 0; k < 9; ++k) {
@@ -194,6 +190,16 @@ static Lin pack_stem(Packer& pk, const std::string& name, int cout, int cout_pad
                     const float v = (tap < 9 && ci < 3) ? wv[(size_t)(tap * 3 + ci) * cout_pad + nt * 8 + nn] : 0.f;
                     frag[(((size_t)ks * (cout_pad / 8) + nt) * 8 + nn) * 16 + k] = __float2half_rn(v);
                 }
+}
+static Lin pack_stem(Packer& pk, const std::string& name, int cout, int cout_pad) {
+    Lin l;
+    l.N = cout_pad;
+    l.K = 27;
+    const float* w = pk.get(name + ".weight", (int64_t)cout * 27);
+    const float* b = pk.get(name + ".bias", cout);
+    if (!w || !b) return l;
+    std::vector<float> wv, bv;
+    pack_stem_w(w, b, cout, cout_pad, wv, bv);
     l.w = pk.add_f32(wv);
     l.b = pk.add_f32(bv);
     return l;
@@ -905,4 +911,92 @@ extern "C" int nb200_light_inpaint(nb200_model* m, const float* x, const float* 
     NB_CHECK(m->kind == NB200_MODEL_LIGHT_INPAINT_V1 && m->inp, "model is not inpaint.light_inpaint_v1");
     NB_CHECK(B > 0 && H > 0 && W > 0, "empty input");
     return light_inpaint_forward(m, (cudaStream_t)stream, x, mask, B, H, W, mirror, out);
+}
+
+// ---- test entry points of the waifu2x convolutions and the SE block: the weights are host fp32 tensors in the PyTorch layout,
+// packed by the network's own packers and copied to a stream-ordered workspace that is freed behind the launch
+static int upload_f32(cudaStream_t st, const std::vector<const std::vector<float>*>& parts, float** dev, std::vector<const float*>& ptrs) {
+    std::vector<float> all;
+    std::vector<size_t> off;
+    for (const std::vector<float>* p : parts) {
+        off.push_back(all.size());
+        all.insert(all.end(), p->begin(), p->end());
+        all.resize((all.size() + 63) & ~(size_t)63, 0.f);   // every part 256-byte aligned
+    }
+    NB_CUDA(cudaMallocAsync((void**)dev, all.size() * 4, st));
+    const cudaError_t e = cudaMemcpyAsync(*dev, all.data(), all.size() * 4, cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) {
+        cudaFreeAsync(*dev, st);
+        return fail(std::string("upload_f32: ") + cudaGetErrorString(e));
+    }
+    ptrs.clear();
+    for (size_t o : off) ptrs.push_back(*dev + o);
+    return 0;
+}
+
+extern "C" int nb200_stem_conv_f16(const void* x, const float* w, const float* b, int cout, int cout_pad, int n, int Hi, int Wi,
+                                   void* out, int ldo, void* stream) {
+    NB_CHECK(x && w && b && out, "null pointer");
+    NB_CHECK(cout > 0 && cout <= cout_pad && (cout_pad == 32 || cout_pad == 64), "cout_pad must be 32 or 64, cout at most cout_pad");
+    NB_CHECK(n > 0 && Hi > 2 && Wi > 2, "input too small");
+    std::vector<float> wv, bv;
+    pack_stem_w(w, b, cout, cout_pad, wv, bv);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&wv, &bv}, &ws, p)) return 1;
+    const int rc = stem_conv3x3(st, (const __half*)x, p[0], p[1], (__half*)out, n, Hi, Wi, cout_pad, ldo);
+    cudaFreeAsync(ws, st);
+    return rc;
+}
+
+extern "C" int nb200_tail_conv_f16(const void* x, const float* w, const float* b, int mode, int epi, int n, int Hi, int Wi, void* out,
+                                   const void* z1, int z1H, int z1W, int clip, void* stream) {
+    NB_CHECK(x && w && b && out && (epi == 0 || z1), "null pointer");
+    NB_CHECK((mode == 0 && (epi == 0 || epi == 1)) || (mode == 1 && epi == 0), "unsupported (mode, epilogue)");
+    const int Ho = mode == 0 ? Hi - 2 : 2 * Hi - 4, Wo = mode == 0 ? Wi - 2 : 2 * Wi - 4;
+    NB_CHECK(n > 0 && Ho > 0 && Wo > 0, "input too small");
+    NB_CHECK(epi == 0 || (z1H >= Ho + 40 && z1W >= Wo + 40), "z1 smaller than the output plus its 20-pixel crop");
+    const std::vector<float> wv = pack_tail_w(w, mode == 1), bv(b, b + 3);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&wv, &bv}, &ws, p)) return 1;
+    const int rc = tail_conv(st, mode, epi, (const __half*)x, p[0], p[1], (__half*)out, (const __half*)z1, n, Hi, Wi, z1H, z1W, clip);
+    cudaFreeAsync(ws, st);
+    return rc;
+}
+
+extern "C" int nb200_head_conv_f16(const void* x, const float* w, const float* b, int mode, int cin, int n, int Hi, int Wi, void* out,
+                                   void* stream) {
+    NB_CHECK(x && w && b && out, "null pointer");
+    NB_CHECK((mode == 0 && cin == 128) || (mode == 1 && cin == 256), "unsupported (mode, input channels)");
+    NB_CHECK(n > 0, "empty batch");
+    const std::vector<float> wv = pack_head_w(w, mode == 1, cin), bv(b, b + 3);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&wv, &bv}, &ws, p)) return 1;
+    const int rc = head_conv(st, mode, cin, (const __half*)x, p[0], p[1], (__half*)out, n, Hi, Wi);
+    cudaFreeAsync(ws, st);
+    return rc;
+}
+
+extern "C" int nb200_se_block_f16(void* x, const float* w1, const float* b1, const float* w2, const float* b2, int n, int H, int W, int C,
+                                  void* stream) {
+    NB_CHECK(x && w1 && b1 && w2 && b2, "null pointer");
+    NB_CHECK(C == 64 || C == 128, "channels must be 64 or 128");
+    NB_CHECK(n > 0 && n <= 65535 && H > 0 && W > 0, "bad geometry");
+    const int R = C / 8;
+    const std::vector<float> W1 = pack_se_w(w1, (size_t)R * C), B1 = pack_se_w(b1, R), W2 = pack_se_w(w2, (size_t)C * R),
+                             B2 = pack_se_w(b2, C);
+    const std::vector<float> scratch(se_partial_floats(n, H, W, C) + (size_t)n * C);   // partial sums, then the scales
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&W1, &B1, &W2, &B2, &scratch}, &ws, p)) return 1;
+    float* partial = const_cast<float*>(p[4]);
+    const int rc = se_block(st, (__half*)x, n, H, W, C, p[0], p[1], p[2], p[3], partial, partial + se_partial_floats(n, H, W, C));
+    cudaFreeAsync(ws, st);
+    return rc;
 }

@@ -182,6 +182,35 @@ __global__ void __launch_bounds__(128) sod_conv_kernel(SodConvArgs a) {
     }
 }
 
+// one REBNCONV launch over B images (the network's layers and nb200_sod_conv_f16)
+int sod_conv(cudaStream_t st, const SodConvArgs& a, int cout, int B) {
+    if (rec_on(REC_CONV)) {
+        char line[160];
+        snprintf(line, sizeof(line), "sodconv,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d", B, a.H, a.W, a.cin, cout, a.dil, a.in_ld,
+                 a.in_off, a.out_ld, a.out_off, a.res ? 1 : 0, a.res_ld);
+        rec_append(line);
+    }
+    NB_CHECK(cout == 16 || cout == 64, "output channels must be 16 or 64");
+    NB_CHECK(a.cin > 0 && a.cin % 16 == 0 && a.in_ld % 8 == 0 && a.in_off % 8 == 0 && a.in_off + a.cin <= a.in_ld,
+             "input channels must be a multiple of 16 inside a 16-byte aligned slice");
+    NB_CHECK(a.out_ld % 2 == 0 && a.out_off % 2 == 0 && a.out_off + cout <= a.out_ld, "bad output slice");
+    NB_CHECK(!a.res || (a.res_ld % 2 == 0 && a.res_off % 2 == 0 && a.res_off + cout <= a.res_ld), "bad residual slice");
+    NB_CHECK(a.dil >= 1 && a.H > 0 && a.W > 0 && B > 0 && B <= 65535, "bad geometry");
+    const int d = a.dil;
+    const size_t smem = ((size_t)(SC_TH + 2 * d) * (SC_TW + 2 * d) * SC_PX + (size_t)cout * SC_WROW) * sizeof(__half);
+    const dim3 grid(cdiv(a.W, SC_TW), cdiv(a.H, SC_TH), B);
+    ProfScope ps(st, PC_OTHER, 2.0 * B * a.H * a.W * cout * 9.0 * a.cin);
+    if (cout == 64) {
+        if (ensure_dyn_smem((const void*)sod_conv_kernel<64>, smem)) return 1;
+        sod_conv_kernel<64><<<grid, 128, smem, st>>>(a);
+    } else {
+        if (ensure_dyn_smem((const void*)sod_conv_kernel<16>, smem)) return 1;
+        sod_conv_kernel<16><<<grid, 128, smem, st>>>(a);
+    }
+    NB_LAUNCHED();
+    return 0;
+}
+
 // MaxPool2d(2, stride 2, ceil_mode=True) at even H, W: in channels [in_off, in_off + C) -> out [H/2][W/2] slice
 __global__ void __launch_bounds__(256) sod_pool_kernel(const __half* __restrict__ in, int in_ld, int in_off, int C, int H, int W,
                                                        __half* __restrict__ out, int out_ld, int out_off, long long total) {
@@ -318,19 +347,7 @@ struct SodRun {
         a.out = out.p; a.out_ld = out.ld; a.out_off = out.off;
         a.res = res; a.res_ld = res_ld; a.res_off = 0;
         a.H = H; a.W = W; a.dil = L.dil;
-        const int d = L.dil;
-        const size_t smem = ((size_t)(SC_TH + 2 * d) * (SC_TW + 2 * d) * SC_PX + (size_t)L.cout * SC_WROW) * sizeof(__half);
-        const dim3 grid(cdiv(W, SC_TW), cdiv(H, SC_TH), B);
-        ProfScope ps(st, PC_OTHER, 2.0 * B * H * W * L.cout * 9.0 * L.cin);
-        if (L.cout == 64) {
-            if (ensure_dyn_smem((const void*)sod_conv_kernel<64>, smem)) return 1;
-            sod_conv_kernel<64><<<grid, 128, smem, st>>>(a);
-        } else {
-            if (ensure_dyn_smem((const void*)sod_conv_kernel<16>, smem)) return 1;
-            sod_conv_kernel<16><<<grid, 128, smem, st>>>(a);
-        }
-        NB_LAUNCHED();
-        return 0;
+        return sod_conv(st, a, L.cout, B);
     }
     int pool(HView in, int C, int H, int W, HView out) {
         const long long total = (long long)B * (H / 2) * (W / 2) * (C / 8);
@@ -572,6 +589,18 @@ extern "C" int nb200_sod_position(const float* saliency, const float* depth, int
     sod_position_kernel<<<B, POS_THREADS, smem, st>>>(saliency, depth, n, (float)(pos - 0.5), out);
     NB_LAUNCHED();
     return 0;
+}
+
+extern "C" int nb200_sod_conv_f16(const void* in, int in_ld, int in_off, int cin, const void* wt, const float* bias, int cout, int dil,
+                                  void* out, int out_ld, int out_off, const void* res, int res_ld, int B, int H, int W, void* stream) {
+    NB_CHECK(in && wt && bias && out, "null pointer");
+    SodConvArgs a;
+    a.in = (const __half*)in; a.in_ld = in_ld; a.in_off = in_off; a.cin = cin;
+    a.wt = (const __half*)wt; a.bias = bias;
+    a.out = (__half*)out; a.out_ld = out_ld; a.out_off = out_off;
+    a.res = (const __half*)res; a.res_ld = res_ld; a.res_off = 0;
+    a.H = H; a.W = W; a.dil = dil;
+    return sod_conv((cudaStream_t)stream, a, cout, B);
 }
 
 extern "C" int nb200_sod_ema(float* state, const float* z, int B, const int* reset_host, double decay, float* out, void* stream) {

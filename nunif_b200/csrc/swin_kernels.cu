@@ -151,7 +151,13 @@ extern int g_tune[16];  // gemm.cu; [7] != 0 selects the SIMT stem / tail kernel
 int stem_conv3x3(cudaStream_t st, const __half* x, const float* wt, const float* bias, __half* out, int n, int Hi, int Wi,
                  int cout_pad, int ldo) {
     NB_CHECK(ldo >= cout_pad && ldo % 8 == 0, "bad output stride");
-    if (g_tune[7] == 0 && n <= 65535 && (cout_pad == 64 || cout_pad == 32)) {
+    const bool mma = g_tune[7] == 0 && n <= 65535 && (cout_pad == 64 || cout_pad == 32);
+    if (rec_on(REC_CONV)) {
+        char line[96];
+        snprintf(line, sizeof(line), "stem,%d,%d,%d,%d,%d,%d", n, Hi, Wi, cout_pad, ldo, mma ? 0 : 1);
+        rec_append(line);
+    }
+    if (mma) {
         const int Ho = Hi - 2, Wo = Wi - 2;
         ProfScope ps(st, PC_STEM, (double)n * Hi * Wi * 16 + (double)n * Ho * Wo * ldo * 2, (double)n * Hi * Wi * 16, (double)n * Ho * Wo * cout_pad * 2);
         const dim3 grid(cdiv(Wo, 64), cdiv(Ho, 2), n);
@@ -327,6 +333,11 @@ __global__ void __launch_bounds__(256) to_image_down_kernel(const __half* __rest
 }
 
 int to_image(cudaStream_t st, const __half* y, void* z, int n, int Hs, int Ws, int cs, int r, int down) {
+    if (rec_on(REC_CONV)) {
+        char line[96];
+        snprintf(line, sizeof(line), "toimg,%d,%d,%d,%d,%d,%d", n, Hs, Ws, cs, r, down);
+        rec_append(line);
+    }
     NB_CHECK(down == 1 || down == 2 || down == 4, "downscale must be 1, 2 or 4");
     NB_CHECK(Hs == Ws && (Hs * r) % down == 0, "bad ToImage geometry");
     const size_t total = (size_t)n * 3 * (Hs * r / down) * (Ws * r / down);
@@ -362,4 +373,10 @@ extern "C" int nb200_window_attention_f16(const void* qkv, const float* bias_tab
     if (!rc) rc = window_attention(st, (const __half*)qkv, frag, (__half*)out, B, H, W, C, shift, (size_t)B * H * W * C);
     cudaFreeAsync(frag, st);
     return rc;
+}
+
+extern "C" int nb200_to_image_f16(const void* y, int n, int Hs, int Ws, int cs, int r, int down, void* z, void* stream) {
+    NB_CHECK(y && z, "null pointer");
+    NB_CHECK(n > 0 && Hs > 0 && r > 0 && cs >= 3 * r * r, "bad ToImage shape");
+    return to_image((cudaStream_t)stream, (const __half*)y, z, n, Hs, Ws, cs, r, down);
 }

@@ -102,12 +102,14 @@ def test_zoe_preprocess_size_host_rule_bit_exact(lib):
         assert (fh + 2 * p_h, fw + 2 * p_w, p_h, p_w) == (int(oh), int(ow), int(ph), int(pw)), (H, W)
 
 
-def test_launch_recorder_mask(lib):
+def test_launch_recorder_mask_bits_0_to_2(lib):
     """nb200_record_launches takes a mask of the recorded kinds (bit 0: GEMM / attention / Swin, bit 1: the kernels between
-    them) and refuses other bits; host only, no device needed."""
-    for on in (1, 2, 3, 0):
+    them, bit 2: the waifu2x stem / tail / head convolutions, SE, to_image and the SOD REBNCONV) and refuses other bits; host
+    only, no device needed."""
+    for on in (1, 2, 3, 4, 7, 0):
         assert lib.nb200_record_launches(on) == 0, on
-    assert lib.nb200_record_launches(4) != 0
-    assert b"unknown recorder bits" in lib.nb200_last_error()
+    for on in (8, 15):
+        assert lib.nb200_record_launches(on) != 0, on
+        assert b"unknown recorder bits" in lib.nb200_last_error()
     buf = ctypes.create_string_buffer(16)
     assert lib.nb200_recorded_launches(buf, 16) == 0 and buf.value == b""
