@@ -217,6 +217,53 @@ def require_cuda(t, name="tensor"):
         raise RuntimeError(f"nunif_b200: {name} must be a CUDA tensor (the engine has no CPU fallback)")
 
 
+# NB200_MODEL_<NAME> -> value: the network kinds nb200_model_create packs.  Must match the enum in include/nunif_b200.h
+# (tests/test_abi.py parses the header and checks this table against it).
+MODEL_KINDS = {
+    "UPCUNET": 1, "CUNET": 2, "SWIN_UNET_1X": 3, "SWIN_UNET_2X": 4, "SWIN_UNET_4X": 5, "DEPTH_ANYTHING_V2_S": 6,
+    "ROW_FLOW_V3": 7, "DEPTH_ANYTHING_V2_B": 8, "DEPTH_ANYTHING_V2_L": 9, "DEPTH_AA": 10, "MLBW": 11, "ZOEDEPTH_N": 12,
+    "UPCONV_7": 13, "VGG_7": 14, "LIGHT_INPAINT_V1": 15, "ROW_FLOW_V2": 16, "SOD_V1": 17, "ZOEDEPTH_ANY_N": 18,
+    "ZOEDEPTH_ANY_K": 19, "DEPTH_ANYTHING_V1_S": 20, "DEPTH_ANYTHING_V1_B": 21, "DEPTH_ANYTHING_V1_L": 22, "TRANSNET_V2": 23,
+}
+
+
+def cuda_device(device):
+    """``torch.device(device)``; raises unless it is a CUDA device."""
+    import torch
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
+    return device
+
+
+class Model:
+    """One packed network (``nb200_model*``) of kind ``MODEL_KINDS[kind]`` on ``device``, built from a state_dict with the
+    reference's key names (strict: a missing or unexpected key raises) and destroyed with this object.  It passes directly as
+    the ``nb200_model*`` argument of the library's entry points (ctypes reads ``_as_parameter_``)."""
+    _as_parameter_ = None
+
+    def __init__(self, kind, state_dict, device, no_clip=False):
+        import torch
+        # the tensors must outlive nb200_model_create: the ctypes arrays hold only their raw pointers
+        items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in state_dict.items()]
+        n = len(items)
+        names = (c_char_p * n)(*[k.encode() for k, _ in items])
+        datas = (c_void_p * n)(*[v.data_ptr() for _, v in items])
+        numels = (ctypes.c_int64 * n)(*[v.numel() for _, v in items])
+        h = c_void_p()
+        with torch.cuda.device(device):
+            check(lib().nb200_model_create(MODEL_KINDS[kind], n, names, datas, numels, 1 if no_clip else 0, ctypes.byref(h)))
+        self._as_parameter_ = h
+
+    def __del__(self):
+        try:
+            if self._as_parameter_:
+                lib().nb200_model_destroy(self._as_parameter_)
+                self._as_parameter_ = None
+        except Exception:
+            pass
+
+
 def stream_ptr(device=None):
     import torch
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)

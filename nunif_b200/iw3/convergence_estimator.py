@@ -10,9 +10,7 @@ import torch
 from .. import _lib
 from ._common import prep
 from .base_depth_model import HUB_MODEL_DIR
-from .row_flow import _create
 
-KIND_SOD_V1 = 17           # NB200_MODEL_SOD_V1
 SOD_SIZE = 192             # SODV1's i2i_in_size
 SOD_NAMES = ("iw3.sod_v1", "iw3.dsod_v1")
 SOD_CHECKPOINT = "iw3_sod_v1_20260125.pth"   # the file name of convergence_estimator.py's SOD_URL
@@ -25,18 +23,8 @@ class SODV1:
     name = "iw3.sod_v1"
 
     def __init__(self, state_dict, device="cuda:0"):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
-        self._h = _create(KIND_SOD_V1, state_dict, self.device)
-
-    def __del__(self):
-        try:
-            if self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        self.device = _lib.cuda_device(device)
+        self._h = _lib.Model("SOD_V1", state_dict, self.device)
 
     def infer(self, rgb, depth):
         rgb = prep(rgb, "rgb")

@@ -2,11 +2,8 @@
 Depth-Anything output when ``depth_aa`` is set (iw3/depth_anything_model.py:153-154, :190-194).
 
 The Linears / 1x1 / 3x3 convolutions run on the wgmma GEMM, everything else in csrc/depth_aa.cu (nb200_depth_aa)."""
-import ctypes
 import torch
 from .. import _lib
-
-KIND_DEPTH_AA = 10     # NB200_MODEL_DEPTH_AA
 
 
 class DepthAA:
@@ -14,26 +11,8 @@ class DepthAA:
     name = "iw3.depth_aa"
 
     def __init__(self, state_dict, device="cuda:0"):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
-        items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in state_dict.items()]
-        n = len(items)
-        names = (ctypes.c_char_p * n)(*[k.encode() for k, _ in items])
-        datas = (ctypes.c_void_p * n)(*[v.data_ptr() for _, v in items])
-        numels = (ctypes.c_int64 * n)(*[v.numel() for _, v in items])
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().nb200_model_create(KIND_DEPTH_AA, n, names, datas, numels, 0, ctypes.byref(h)))
-        self._h = h
-
-    def __del__(self):
-        try:
-            if self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        self.device = _lib.cuda_device(device)
+        self._h = _lib.Model("DEPTH_AA", state_dict, self.device)
 
     def _run(self, x, mode):
         _lib.require_cuda(x, "x")

@@ -7,7 +7,6 @@ packed into the native container (csrc/depth_model.inl) and run as wgmma GEMMs +
 csrc/depth_kernels.cu.  ``infer`` keeps the reference's signature and output convention: depth B,1,h,w (or 1,h,w)
 float32 on ``x.device``, larger = nearer.
 """
-import ctypes
 from os import path
 import torch
 from .. import _lib
@@ -15,10 +14,11 @@ from .base_depth_model import BaseDepthModel, HUB_MODEL_DIR
 from .depth_anything_preprocess import batch_preprocess
 from .dilation import dilate_edge, edge_dilation_is_enabled
 
-# NB200_MODEL_DEPTH_ANYTHING_V2_{S,B,L}, NB200_MODEL_DEPTH_ANYTHING_V1_{S,B,L}; model types as in iw3/depth_anything_model.py
-# NAME_MAP.  V1 is the same network with the hooks on the last four blocks.
-KINDS = {"vits": 6, "vitb": 8, "vitl": 9}
-V1_KINDS = {"vits": 20, "vitb": 21, "vitl": 22}
+# encoder -> the _lib.MODEL_KINDS DEPTH_ANYTHING_V2_{S,B,L} and DEPTH_ANYTHING_V1_{S,B,L}; model types as in
+# iw3/depth_anything_model.py NAME_MAP.  V1 is the same network with the hooks on the last four blocks.
+_SIZE = {"vits": "S", "vitb": "B", "vitl": "L"}
+KINDS = {e: _lib.MODEL_KINDS["DEPTH_ANYTHING_V2_" + s] for e, s in _SIZE.items()}
+V1_KINDS = {e: _lib.MODEL_KINDS["DEPTH_ANYTHING_V1_" + s] for e, s in _SIZE.items()}
 ENCODER_OF = {"Any_V2_S": "vits", "Any_V2_B": "vitb", "Any_V2_L": "vitl", "Any_S": "vits", "Any_B": "vitb", "Any_L": "vitl"}
 V1_MODELS = {"Any_S", "Any_B", "Any_L"}
 AA_SUPPORTED_MODELS = {"Any_V2_S", "Any_V2_B", "Any_V2_L"}   # depth_anything_model.py:61-65
@@ -33,28 +33,10 @@ class DepthAnythingNet:
             raise ValueError(f"encoder: choose from {list(KINDS)}")
         self.encoder = encoder
         self.v1 = v1
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
-        items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in state_dict.items()]
-        n = len(items)
-        names = (ctypes.c_char_p * n)(*[k.encode() for k, _ in items])
-        datas = (ctypes.c_void_p * n)(*[v.data_ptr() for _, v in items])
-        numels = (ctypes.c_int64 * n)(*[v.numel() for _, v in items])
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().nb200_model_create((V1_KINDS if v1 else KINDS)[encoder], n, names, datas, numels, 0, ctypes.byref(h)))
-        self._h = h
+        self.device = _lib.cuda_device(device)
+        self._h = _lib.Model(f"DEPTH_ANYTHING_V{1 if v1 else 2}_{_SIZE[encoder]}", state_dict, self.device)
         self.metric_depth = False
         self.prep_lower_bound = 392
-
-    def __del__(self):
-        try:
-            if self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     def __call__(self, x):
         _lib.require_cuda(x, "x")

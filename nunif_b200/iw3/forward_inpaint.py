@@ -12,9 +12,7 @@ from .. import _lib
 from ._common import prep
 from .base_depth_model import HUB_MODEL_DIR
 from .forward_warp import apply_divergence_forward_warp
-from .row_flow import _create
 
-KIND_LIGHT_INPAINT_V1 = 15   # NB200_MODEL_LIGHT_INPAINT_V1
 MODEL_NAME = "inpaint.light_inpaint_v1"
 CHECKPOINT = "iw3_light_inpaint_v1_20250919.pth"   # iw3/inpaint_utils.py:45
 
@@ -42,20 +40,10 @@ class LightInpaintV1:
     name = MODEL_NAME
 
     def __init__(self, state_dict=None, device="cuda:0"):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
+        self.device = _lib.cuda_device(device)
         if state_dict is None or isinstance(state_dict, (str, os.PathLike)):
             state_dict = load_state_dict(state_dict if state_dict is not None else default_checkpoint())
-        self._h = _create(KIND_LIGHT_INPAINT_V1, state_dict, self.device)
-
-    def __del__(self):
-        try:
-            if self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        self._h = _lib.Model("LIGHT_INPAINT_V1", state_dict, self.device)
 
     def infer(self, x, mask, mirror=False):
         x, mask = prep(x, "x"), prep(mask, "mask")

@@ -8,29 +8,11 @@ The v3 delta network runs as wgmma GEMMs + the kernels in csrc/rowflow_kernels.c
 _f16 / _sym forms).  steps > 1 (iterative re-warping of the depth, :205-226) and preserve_screen_border (:33-47) run the same
 kernels once per step.
 """
-import ctypes
 import os
 import torch
 from .. import _lib
 from . import _common
 from .base_depth_model import HUB_MODEL_DIR
-
-KIND_ROW_FLOW_V3 = 7     # NB200_MODEL_ROW_FLOW_V3
-KIND_MLBW = 11           # NB200_MODEL_MLBW
-KIND_ROW_FLOW_V2 = 16    # NB200_MODEL_ROW_FLOW_V2
-
-
-def _create(kind, state_dict, device):
-    items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in state_dict.items()]
-    n = len(items)
-    names = (ctypes.c_char_p * n)(*[k.encode() for k, _ in items])
-    datas = (ctypes.c_void_p * n)(*[v.data_ptr() for _, v in items])
-    numels = (ctypes.c_int64 * n)(*[v.numel() for _, v in items])
-    h = ctypes.c_void_p()
-    with torch.cuda.device(device):
-        _lib.check(_lib.lib().nb200_model_create(kind, n, names, datas, numels, 0, ctypes.byref(h)))
-    return h
-
 
 class MLBW:
     """Packed `sbs.mlbw` (iw3/models/mlbw.py; methods mlbw_l2 / mlbw_l4 and their `s` variants, and mask_mlbw_l2 with
@@ -41,20 +23,10 @@ class MLBW:
     delta_output = True
 
     def __init__(self, state_dict, device="cuda:0"):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
-        self._h = _create(KIND_MLBW, state_dict, self.device)
+        self.device = _lib.cuda_device(device)
+        self._h = _lib.Model("MLBW", state_dict, self.device)
         self.num_layers = int(_lib.lib().nb200_mlbw_num_layers(self._h))
         self.hole_mask = bool(_lib.lib().nb200_mlbw_has_hole_mask(self._h))
-
-    def __del__(self):
-        try:
-            if self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     def __call__(self, x):
         _lib.require_cuda(x, "x")
@@ -81,22 +53,12 @@ class RowFlowV3:
     name = "sbs.row_flow_v3"
     symmetric = False
     delta_output = True
-    _kind, _entry = KIND_ROW_FLOW_V3, "nb200_row_flow_delta"
+    _kind, _entry = "ROW_FLOW_V3", "nb200_row_flow_delta"
 
     def __init__(self, state_dict, device="cuda:0", symmetric=False):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
+        self.device = _lib.cuda_device(device)
         self.symmetric = bool(symmetric)
-        self._h = _create(self._kind, state_dict, self.device)
-
-    def __del__(self):
-        try:
-            if self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        self._h = _lib.Model(self._kind, state_dict, self.device)
 
     def delta_x(self, x):
         _lib.require_cuda(x, "x")
@@ -119,7 +81,7 @@ class RowFlowV2(RowFlowV3):
     that the reference's ``delta * delta_scale`` is then an fp16 product."""
     name = "sbs.row_flow_v2"
     delta_f16 = True
-    _kind, _entry = KIND_ROW_FLOW_V2, "nb200_row_flow_v2_delta"
+    _kind, _entry = "ROW_FLOW_V2", "nb200_row_flow_v2_delta"
 
     def __init__(self, state_dict, device="cuda:0"):
         super().__init__(state_dict, device)

@@ -9,10 +9,12 @@ ZoeD_N; ZoeD_Any_K the "normed" one (bins bounded to [1e-3, 80], sorted at the l
 ``infer`` are ZoeDepthModel's (the reference uses one class for all ZoeDepth checkpoints).
 """
 from os import path
+from .. import _lib
 from .base_depth_model import HUB_MODEL_DIR
 from .zoedepth_model import ZoeDepthModel, ZoeDepthNet
 
-KINDS = {"ZoeD_Any_N": 18, "ZoeD_Any_K": 19}   # NB200_MODEL_ZOEDEPTH_ANY_{N,K}
+_KIND_KEYS = {"ZoeD_Any_N": "ZOEDEPTH_ANY_N", "ZoeD_Any_K": "ZOEDEPTH_ANY_K"}   # model type -> _lib.MODEL_KINDS key
+KINDS = {t: _lib.MODEL_KINDS[k] for t, k in _KIND_KEYS.items()}
 
 MODEL_FILES = {   # zoedepth_model.py:17-19
     "ZoeD_Any_N": path.join(HUB_MODEL_DIR, "checkpoints", "depth_anything_metric_depth_indoor.pt"),
@@ -28,7 +30,7 @@ class ZoeDepthAnythingNet(ZoeDepthNet):
     def __init__(self, state_dict, device="cuda:0", model_type="ZoeD_Any_N"):
         if model_type not in KINDS:
             raise ValueError(f"model_type: choose from {list(KINDS)}")
-        super().__init__(state_dict, device, kind=KINDS[model_type])
+        super().__init__(state_dict, device, kind=_KIND_KEYS[model_type])
         self.model_type = model_type
         self.prep_mod = 14                      # zoedepth_model.py:190-199
         self.prep_h_height = 392

@@ -12,15 +12,12 @@ Not built: ZoeD_K / ZoeD_NK (two bin heads + the patch-transformer domain classi
 constructor raises.  The Depth-Anything-metric checkpoints ZoeD_Any_N / ZoeD_Any_K run through ZoeDepthAnythingModel
 (zoedepth_any_model.py), a subclass that shares this class's loading and ``infer``.
 """
-import ctypes
 from os import path
 import torch
 from .. import _lib
 from .base_depth_model import BaseDepthModel, HUB_MODEL_DIR
 from .zoedepth_preprocess import batch_preprocess
 from .dilation import dilate_edge, edge_dilation_is_enabled
-
-KIND_ZOEDEPTH_N = 12   # NB200_MODEL_ZOEDEPTH_N
 
 MODEL_FILES = {   # zoedepth_model.py:12-19 (the one checkpoint the engine implements)
     "ZoeD_N": path.join(HUB_MODEL_DIR, "checkpoints", "ZoeD_M12_N.pt"),
@@ -38,32 +35,13 @@ class ZoeDepthNet:
     """The packed network: ``net(x)`` == ``ZoeDepth.forward(x)['metric_depth']`` (x: B,3,H,W normalised, H,W % 32 == 0
     -> B,1,H,W metric depth)."""
 
-    def __init__(self, state_dict, device="cuda:0", kind=KIND_ZOEDEPTH_N):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
-        items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in _strip_checkpoint(state_dict).items()
-                 if torch.is_tensor(v)]
-        n = len(items)
-        names = (ctypes.c_char_p * n)(*[k.encode() for k, _ in items])
-        datas = (ctypes.c_void_p * n)(*[v.data_ptr() for _, v in items])
-        numels = (ctypes.c_int64 * n)(*[v.numel() for _, v in items])
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().nb200_model_create(kind, n, names, datas, numels, 0, ctypes.byref(h)))
-        self._h = h
+    def __init__(self, state_dict, device="cuda:0", kind="ZOEDEPTH_N"):
+        self.device = _lib.cuda_device(device)
+        self._h = _lib.Model(kind, {k: v for k, v in _strip_checkpoint(state_dict).items() if torch.is_tensor(v)}, self.device)
         self.metric_depth = True
         self.prep_mod = 32                      # zoedepth_model.py:172-180
         self.prep_h_height = 384
         self.prep_v_height = 512
-
-    def __del__(self):
-        try:
-            if self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     def __call__(self, x):
         _lib.require_cuda(x, "x")

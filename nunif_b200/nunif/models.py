@@ -8,11 +8,12 @@ import ctypes
 import torch
 from .. import _lib
 
-KINDS = {
-    "waifu2x.upcunet": 1, "waifu2x.cunet": 2,
-    "waifu2x.swin_unet_1x": 3, "waifu2x.swin_unet_2x": 4, "waifu2x.swin_unet_4x": 5,
-    "waifu2x.upconv_7": 13, "waifu2x.vgg_7": 14,
+_KIND_KEYS = {   # model name -> _lib.MODEL_KINDS key
+    "waifu2x.upcunet": "UPCUNET", "waifu2x.cunet": "CUNET",
+    "waifu2x.swin_unet_1x": "SWIN_UNET_1X", "waifu2x.swin_unet_2x": "SWIN_UNET_2X", "waifu2x.swin_unet_4x": "SWIN_UNET_4X",
+    "waifu2x.upconv_7": "UPCONV_7", "waifu2x.vgg_7": "VGG_7",
 }
+KINDS = {name: _lib.MODEL_KINDS[k] for name, k in _KIND_KEYS.items()}
 
 
 def _cunet_validator(size):            # waifu2x/models/cunet.py:124-125
@@ -38,50 +39,26 @@ def _validator_for(name):
 class B200I2IModel:
     """Drop-in for an ``I2IBaseModel`` instance in eval mode."""
 
-    def __init__(self, name, state_dict, device="cuda:0", no_clip=False, _handle=None, _downscale=1, _parent=None):
+    def __init__(self, name, state_dict, device="cuda:0", no_clip=False, _model=None, _downscale=1):
         if name not in KINDS:
             raise ValueError(f"Unknown model name: {name}")          # nunif/models/register.py:22-28
         self.name = name
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
+        self.device = _lib.cuda_device(device)
         self._downscale = _downscale
-        self._parent = _parent  # keeps the shared handle alive (to_2x(shared=True))
         self.training = False
         self.i2i_in_channels = 3
         self.i2i_default_tile_size = 256                              # model.py:69
         self.i2i_default_batch_size = 4
         self._validator = _validator_for(name)
-        lib = _lib.lib()
-        if _handle is not None:
-            self._h = _handle
-            self._own = False
-        else:
-            items = [(k, v.detach().to("cpu", torch.float32).contiguous()) for k, v in state_dict.items()]
-            n = len(items)
-            names = (ctypes.c_char_p * n)(*[k.encode() for k, _ in items])
-            datas = (ctypes.c_void_p * n)(*[v.data_ptr() for _, v in items])
-            numels = (ctypes.c_int64 * n)(*[v.numel() for _, v in items])
-            h = ctypes.c_void_p()
-            with torch.cuda.device(self.device):
-                _lib.check(lib.nb200_model_create(KINDS[name], n, names, datas, numels, 1 if no_clip else 0, ctypes.byref(h)))
-            self._h = h
-            self._own = True
+        # a to_2x / to_1x view shares the 4x model's packed weights, and its reference keeps them alive
+        self._h = _model if _model is not None else _lib.Model(_KIND_KEYS[name], state_dict, self.device, no_clip)
         s, o, b = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        _lib.check(lib.nb200_model_info(self._h, ctypes.byref(s), ctypes.byref(o), ctypes.byref(b)))
+        _lib.check(_lib.lib().nb200_model_info(self._h, ctypes.byref(s), ctypes.byref(o), ctypes.byref(b)))
         if _downscale == 1:
             self.i2i_scale, self.i2i_offset = s.value, o.value
             self.i2i_blend_size = b.value if b.value > 0 else None   # cunet passes blend_size=None
         else:                                                          # swin_unet.py:345-350
             self.i2i_scale, self.i2i_offset, self.i2i_blend_size = 4 // _downscale, 32 // _downscale, 4 * _downscale
-
-    def __del__(self):
-        try:
-            if getattr(self, "_own", False) and self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     # ---- I2IBaseModel surface
     def find_valid_tile_size(self, base_tile_size):
@@ -105,12 +82,12 @@ class B200I2IModel:
         """SwinUNet4x.to_2x (swin_unet.py:289-295): same weights + bicubic-AA /2."""
         if self.name != "waifu2x.swin_unet_4x":
             raise AttributeError("to_2x is defined for waifu2x.swin_unet_4x only")
-        return B200I2IModel(self.name, None, self.device, _handle=self._h, _downscale=2, _parent=self)
+        return B200I2IModel(self.name, None, self.device, _model=self._h, _downscale=2)
 
     def to_1x(self, shared=True):
         if self.name != "waifu2x.swin_unet_4x":
             raise AttributeError("to_1x is defined for waifu2x.swin_unet_4x only")
-        return B200I2IModel(self.name, None, self.device, _handle=self._h, _downscale=4, _parent=self)
+        return B200I2IModel(self.name, None, self.device, _model=self._h, _downscale=4)
 
     def weight_blob(self):
         """(device_ptr, nbytes) of the packed weights, for the one-time NCCL broadcast."""

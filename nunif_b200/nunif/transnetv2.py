@@ -4,9 +4,7 @@ import os
 import torch
 from .. import _lib
 from ..iw3.base_depth_model import HUB_MODEL_DIR
-from ..iw3.row_flow import _create
 
-KIND_TRANSNET_V2 = 23       # NB200_MODEL_TRANSNET_V2
 FRAME_SHAPE = (3, 27, 48)
 CHECKPOINT = "transnetv2-pytorch-weights.pth"   # the file name of TransNetV2.load's URL
 
@@ -22,10 +20,8 @@ class TransNetV2:
     TransNetV2.forward; every window is padded in time on its own, as in the reference."""
 
     def __init__(self, state_dict, device="cuda:0"):
-        self.device = torch.device(device)
-        if self.device.type != "cuda":
-            raise RuntimeError("nunif_b200 models live on a CUDA (sm_90) device; there is no CPU path")
-        self._h = _create(KIND_TRANSNET_V2, state_dict, self.device)
+        self.device = _lib.cuda_device(device)
+        self._h = _lib.Model("TRANSNET_V2", state_dict, self.device)
 
     @classmethod
     def load(cls, device="cuda:0", path=None):
@@ -35,14 +31,6 @@ class TransNetV2:
             raise FileNotFoundError(f"{path}: the TransNetV2 checkpoint of --scene-detect is missing "
                                     "(the engine does not download models)")
         return cls(torch.load(path, map_location="cpu", weights_only=True), device)
-
-    def __del__(self):
-        try:
-            if self._h:
-                _lib.lib().nb200_model_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
 
     def eval(self):
         return self

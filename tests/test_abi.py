@@ -33,6 +33,15 @@ def test_header_symbols_exported(lib):
         assert s in syms, f"{s} bound in _lib.py but not declared in the header"
 
 
+def test_model_kinds_match_header():
+    """_lib.MODEL_KINDS is the header's NB200_MODEL_* enum, name for name and value for value."""
+    from nunif_b200 import _lib
+    src = open(os.path.join(ROOT, "include", "nunif_b200.h")).read()
+    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+    declared = {name: int(v) for name, v in re.findall(r"\bNB200_MODEL_([A-Z0-9_]+)\s*=\s*(\d+)", src)}
+    assert declared == _lib.MODEL_KINDS
+
+
 def test_abi_version(lib):
     assert lib.nb200_abi_version() == 1
 

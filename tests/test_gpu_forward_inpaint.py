@@ -178,13 +178,12 @@ def test_apply_divergence_forward_inpaint(model):
     assert torch.equal(left, l2[0]) and torch.equal(right, r2[0])
 
 
-def test_strict_keys(sd):
-    from nunif_b200.iw3.row_flow import _create
+def test_lib_model_strict_keys(sd):
     bad = dict(sd)
     bad.pop("enc2.3.norm2.weight")
     with pytest.raises(RuntimeError, match="missing key"):
-        _create(15, bad, torch.device(DEV))
+        _lib.Model("LIGHT_INPAINT_V1", bad, torch.device(DEV))
     bad = dict(sd)
     bad["extra"] = torch.zeros(1)
     with pytest.raises(RuntimeError, match="unexpected key"):
-        _create(15, bad, torch.device(DEV))
+        _lib.Model("LIGHT_INPAINT_V1", bad, torch.device(DEV))

@@ -99,14 +99,13 @@ def test_delta_entry_point_refuses_hole_model(mm):
         _lib.check(_lib.lib().nb200_mlbw_delta(mm._h, _lib.ptr(x), 1, 8, 32, _lib.ptr(d), _lib.ptr(lw), _lib.stream_ptr()))
 
 
-def test_pack_rejects_odd_lv1_out(sd):
+def test_lib_model_rejects_odd_lv1_out(sd):
     """Only the 5-output hole head (num_layers 2) exists upstream: a 7-element lv1_out bias is refused with a clear error."""
-    from nunif_b200.iw3.row_flow import _create
     bad = dict(sd)
     bad["lv1_out.1.weight"] = torch.cat([sd["lv1_out.1.weight"], sd["lv1_out.1.weight"][:2]])
     bad["lv1_out.1.bias"] = torch.cat([sd["lv1_out.1.bias"], sd["lv1_out.1.bias"][:2]])
     with pytest.raises(RuntimeError, match="lv1_out.1.bias"):
-        _create(11, bad, torch.device(DEV))
+        _lib.Model("MLBW", bad, torch.device(DEV))
 
 
 def _pp_case(g, i):
