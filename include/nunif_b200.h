@@ -561,6 +561,34 @@ int nb200_anaglyph(const float* l, const float* r, int B, int H, int W, int type
  * max-output-size resize of postprocess_image, iw3/utils.py:445-485); clamp01_out applies the following clamp. */
 int nb200_resize_bicubic_aa(const float* x, int planes, int H, int W, int oh, int ow, int clamp01_out,
                             float* out, void* stream);
+/* The same resize with F.interpolate's align_corners flag (preprocess_image's --max-output-height resize,
+ * iw3/utils.py:247-271, uses align_corners=True): ATen's scale becomes (in - 1) / (out - 1); align_corners = 0 is
+ * nb200_resize_bicubic_aa. */
+int nb200_resize_bicubic_aa_ac(const float* x, int planes, int H, int W, int oh, int ow, int clamp01_out,
+                               int align_corners, float* out, void* stream);
+
+/* torch.rot90(x, k, (-2, -1)) of `planes` fp32 H x W planes (--rotate-left k = 1, --rotate-right k = 3,
+ * iw3/utils.py:247-252): x [planes][H][W] -> out [planes][W][H], bit-exact.  out must not alias x. */
+int nb200_rot90(const float* x, int planes, int H, int W, int k, float* out, void* stream);
+
+/* The autocrop detector (nunif/utils/autocrop.py:6-207) on x [B][3][H][W] fp32, one frame at a time as the reference's
+ * detect_tb / detect_lr:  Y = r*0.299 + g*0.587 + b*0.114 (fp32, no contraction).
+ *   black != 0 (black, black_tb, black_lr): Y clamped to [16/255, 235/255]; a line is a bar when its mean <= 32/255 and
+ *     max|Y - mean| < 16/255 (mean = sum * fl(1/n) as ATen's CUDA mean; the summation order is the kernel's own).
+ *   black == 0 (flat, flat_tb, flat_lr): a line is a bar when fl(count(|Y - median| < 16/255) * fl(1/n)) > 0.99, median
+ *     the exact lower median (torch.median).
+ * axes: bit 0 rows (detect_tb), bit 1 columns (detect_lr).  Every output may be NULL: mask_tb [B][H] / mask_lr [B][W]
+ * (uint8 0 / 1), count_tb [H] / count_lr [W] int32 (+= the mask, summed over the B frames: AutoCropDetector.update),
+ * stat_tb [B][H] / stat_lr [B][W] (black: the mean, flat: the median).  Makes no host synchronisation.
+ * Rows in flat mode need W <= 12544, columns need H <= 6144 (shared-memory staging). */
+int nb200_autocrop_detect(const float* x, int B, int H, int W, int black, int axes, unsigned char* mask_tb,
+                          unsigned char* mask_lr, int* count_tb, int* count_lr, float* stat_tb, float* stat_lr,
+                          void* stream);
+/* AutoCropDetector.get_crop (:47-69) on the device: bar_i = fl(count_i * fl(1 / frame_count)) >= threshold (ATen's
+ * CUDA division by a host scalar); out[0], out[1] = first / last non-bar row, out[2], out[3] = first / last non-bar
+ * column, -1 when there is none or the counts are NULL.  out: 4 int32 on the device. */
+int nb200_autocrop_bounds(const int* count_tb, int H, const int* count_lr, int W, int frame_count, float threshold,
+                          int* out, void* stream);
 
 /* VR180 output (iw3/equirectangular.py:7-40; iw3/utils.py:441-443): zero-pad to 1.5 x the longer edge, bicubic grid_sample
  * (zeros, align_corners=True) through x' = k tan(az), y' = k tan(el)/cos(az), clamp [0,1].

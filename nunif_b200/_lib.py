@@ -113,6 +113,10 @@ SIGNATURES = {
     "nb200_zoe_preprocess": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_anaglyph": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_resize_bicubic_aa": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "nb200_resize_bicubic_aa_ac": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "nb200_rot90": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "nb200_autocrop_detect": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int] + [c_void_p] * 7),
+    "nb200_autocrop_bounds": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p]),
     "nb200_equirectangular_size": (c_int, [c_int, c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),
     "nb200_equirectangular": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_backward_warp": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_double, c_int, c_int,

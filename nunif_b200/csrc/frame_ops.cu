@@ -95,9 +95,44 @@ __global__ void __launch_bounds__(128) da_preprocess_kernel(DaPrepParams p) {
     }
 }
 
+// torch.rot90(x, k, (-2, -1)) of one H x W plane per blockIdx.z -> W x H.  k = 1: out[i][j] = x[j][W-1-i];
+// k = 3: out[i][j] = x[H-1-j][i].  A 32 x 32 tile goes through shared memory so that reads and writes are both coalesced.
+__global__ void __launch_bounds__(256) rot90_kernel(const float* __restrict__ x, float* __restrict__ out, int H, int W, int k) {
+    __shared__ float tile[32][33];
+    const int x0 = blockIdx.x * 32, y0 = blockIdx.y * 32, tx = threadIdx.x, ty = threadIdx.y;
+    const size_t plane = (size_t)H * W;
+    const float* src = x + blockIdx.z * plane;
+    float* dst = out + blockIdx.z * plane;
+    for (int r = ty; r < 32; r += 8) {
+        const int yy = y0 + r, xx = x0 + tx;
+        if (yy < H && xx < W) tile[r][tx] = src[(size_t)yy * W + xx];
+    }
+    __syncthreads();
+    // thread (tx, r) writes the element that came from input (y0 + tx, x0 + r)
+    const int yy = y0 + tx;
+    if (yy >= H) return;
+    for (int r = ty; r < 32; r += 8) {
+        const int xx = x0 + r;
+        if (xx >= W) break;
+        const size_t o = k == 1 ? (size_t)(W - 1 - xx) * H + yy : (size_t)xx * H + (H - 1 - yy);
+        dst[o] = tile[tx][r];
+    }
+}
+
 }  // namespace nb200
 
 using namespace nb200;
+
+extern "C" int nb200_rot90(const float* x, int planes, int H, int W, int k, float* out, void* stream) {
+    NB_CHECK(x && out && x != out, "null or aliased pointer");
+    NB_CHECK(planes > 0 && planes <= 65535 && H > 0 && W > 0, "bad shape");
+    NB_CHECK(k == 1 || k == 3, "k must be 1 or 3");
+    cudaStream_t st = (cudaStream_t)stream;
+    ProfScope ps(st, PC_OTHER, (double)planes * H * W * 8);
+    rot90_kernel<<<dim3(cdiv(W, 32), cdiv(H, 32), planes), dim3(32, 8), 0, st>>>(x, out, H, W, k);
+    NB_LAUNCHED();
+    return 0;
+}
 
 extern "C" int nb200_hwc_to_chw_f32(const void* x, int bits, int B, int H, int W, float* out, void* stream) {
     NB_CHECK(x && out, "null pointer");

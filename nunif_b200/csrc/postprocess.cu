@@ -2,7 +2,8 @@
 //   * the whole red-cyan anaglyph family (iw3/anaglyph.py:4-110): color, gray, half-color, wimmer, wimmer2 (dubois lives
 //     in warp_backward.cu),
 //   * torchvision TF.resize(..., BICUBIC, antialias=True) on fp32 planes = ATen _upsample_bicubic2d_aa
-//     (align_corners=False, A = -0.5): half-SBS / half-TB squeeze and the max-output-size resize.
+//     (align_corners=False, A = -0.5): half-SBS / half-TB squeeze and the max-output-size resize; with align_corners=True
+//     (F.interpolate) the --max-output-height pre-resize of preprocess_image.
 // HBM-bound elementwise / small-stencil kernels.
 #include "common.cuh"
 #include "../../include/nunif_b200.h"
@@ -60,27 +61,50 @@ __device__ __forceinline__ float cubic_aa_w(float x) {
 struct ResizeParams {
     const float* x;
     float* out;
-    int planes, H, W, oh, ow, clamp;
+    int planes, H, W, oh, ow, clamp, align_corners;
     float sy, sx, supy, supx, invy, invx;
 };
+
+// Tap window [lo, lo + size) and the filter argument of tap j (aa_arg).  align_corners = 0 keeps the
+// fp32-rounded centre (bit-exact to ATen's CPU kernel).  align_corners = 1 follows ATen's CUDA kernel, whose centre
+// scale * (i + 0.5) is contracted into each use (one FMA, never rounded on its own): with the inexact scales of
+// (in - 1) / (out - 1) a rounded centre moves the 4K -> 1080 output by up to 2e-5.
+struct AaSpan { int lo, size; float off; };
+__device__ __forceinline__ AaSpan aa_span(int i, float s, float sup, int n, int align_corners) {
+    AaSpan a;
+    const float t = (float)i + 0.5f;
+    if (align_corners) {
+        a.lo = max(0, (int)(fmaf(s, t, -sup) + 0.5f));
+        a.size = min(n, (int)(fmaf(s, t, sup) + 0.5f)) - a.lo;
+        a.off = fmaf(-s, t, (float)a.lo);   // xmin - centre
+    } else {
+        const float c = __fmul_rn(s, t);
+        a.lo = max(0, (int)(c - sup + 0.5f));
+        a.size = min(n, (int)(c + sup + 0.5f)) - a.lo;
+        a.off = -c;      // arg = (j + lo) - c + 0.5, as before
+    }
+    return a;
+}
+__device__ __forceinline__ float aa_arg(const AaSpan& a, int j, float inv, int align_corners) {
+    return align_corners ? __fmul_rn(__fadd_rn(__fadd_rn((float)j, a.off), 0.5f), inv) : ((float)(j + a.lo) + a.off + 0.5f) * inv;
+}
 
 // one thread per output pixel; horizontal pass inside the vertical loop (ATen order: horizontal first, fp32)
 __global__ void __launch_bounds__(128) resize_bicubic_aa_kernel(ResizeParams p) {
     const int ox = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y, pl = blockIdx.z;
     if (ox >= p.ow) return;
-    const float cy = __fmul_rn(p.sy, (float)oy + 0.5f), cx = __fmul_rn(p.sx, (float)ox + 0.5f);
-    const int ymin = max(0, (int)(cy - p.supy + 0.5f)), ysize = min(p.H, (int)(cy + p.supy + 0.5f)) - ymin;
-    const int xmin = max(0, (int)(cx - p.supx + 0.5f)), xsize = min(p.W, (int)(cx + p.supx + 0.5f)) - xmin;
+    const AaSpan sy = aa_span(oy, p.sy, p.supy, p.H, p.align_corners), sx = aa_span(ox, p.sx, p.supx, p.W, p.align_corners);
+    const int ymin = sy.lo, ysize = sy.size, xmin = sx.lo, xsize = sx.size;
     float wxs = 0.f, wys = 0.f;
-    for (int j = 0; j < xsize; ++j) wxs += cubic_aa_w(((float)(j + xmin) - cx + 0.5f) * p.invx);
-    for (int j = 0; j < ysize; ++j) wys += cubic_aa_w(((float)(j + ymin) - cy + 0.5f) * p.invy);
+    for (int j = 0; j < xsize; ++j) wxs += cubic_aa_w(aa_arg(sx, j, p.invx, p.align_corners));
+    for (int j = 0; j < ysize; ++j) wys += cubic_aa_w(aa_arg(sy, j, p.invy, p.align_corners));
     const float* src = p.x + (size_t)pl * p.H * p.W;
     float acc = 0.f;
     for (int jy = 0; jy < ysize; ++jy) {
-        const float wy = cubic_aa_w(((float)(jy + ymin) - cy + 0.5f) * p.invy) / wys;
+        const float wy = cubic_aa_w(aa_arg(sy, jy, p.invy, p.align_corners)) / wys;
         const float* row = src + (size_t)(ymin + jy) * p.W + xmin;
         float h = 0.f;
-        for (int jx = 0; jx < xsize; ++jx) h += cubic_aa_w(((float)(jx + xmin) - cx + 0.5f) * p.invx) / wxs * __ldg(row + jx);
+        for (int jx = 0; jx < xsize; ++jx) h += cubic_aa_w(aa_arg(sx, jx, p.invx, p.align_corners)) / wxs * __ldg(row + jx);
         acc += wy * h;
     }
     p.out[((size_t)pl * p.oh + oy) * p.ow + ox] = p.clamp ? clamp01(acc) : acc;
@@ -154,11 +178,24 @@ extern "C" int nb200_anaglyph(const float* l, const float* r, int B, int H, int 
 
 extern "C" int nb200_resize_bicubic_aa(const float* x, int planes, int H, int W, int oh, int ow, int clamp01_out, float* out,
                                        void* stream) {
+    return nb200_resize_bicubic_aa_ac(x, planes, H, W, oh, ow, clamp01_out, 0, out, stream);
+}
+
+// ATen upsample_gen2d_aa: align_corners enters through area_pixel_compute_scale only ((in - 1) / (out - 1), 0 for a
+// 1-pixel output); the centre stays scale * (i + 0.5) and the support and weights follow from that scale as before.
+extern "C" int nb200_resize_bicubic_aa_ac(const float* x, int planes, int H, int W, int oh, int ow, int clamp01_out,
+                                          int align_corners, float* out, void* stream) {
     NB_CHECK(x && out, "null pointer");
     NB_CHECK(planes > 0 && planes <= 65535 && H > 0 && W > 0 && oh > 0 && ow > 0, "bad shape");
     ResizeParams p;
     p.x = x; p.out = out; p.planes = planes; p.H = H; p.W = W; p.oh = oh; p.ow = ow; p.clamp = clamp01_out;
-    p.sy = (float)H / (float)oh; p.sx = (float)W / (float)ow;
+    p.align_corners = align_corners ? 1 : 0;
+    if (align_corners) {
+        p.sy = oh > 1 ? (float)(H - 1) / (float)(oh - 1) : 0.f;
+        p.sx = ow > 1 ? (float)(W - 1) / (float)(ow - 1) : 0.f;
+    } else {
+        p.sy = (float)H / (float)oh; p.sx = (float)W / (float)ow;
+    }
     p.supy = p.sy >= 1.f ? 2.f * p.sy : 2.f; p.supx = p.sx >= 1.f ? 2.f * p.sx : 2.f;
     p.invy = p.sy >= 1.f ? 1.f / p.sy : 1.f; p.invx = p.sx >= 1.f ? 1.f / p.sx : 1.f;
     cudaStream_t st = (cudaStream_t)stream;

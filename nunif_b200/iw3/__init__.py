@@ -26,8 +26,8 @@ from .row_flow import RowFlowV3, MLBW, apply_divergence_nn_LR, apply_divergence_
 from .row_flow import RowFlowV2, apply_divergence_nn_symmetric, load_row_flow_model  # noqa: F401
 from .row_flow import postprocess_hole_mask  # noqa: F401
 from .depth_aa import DepthAA  # noqa: F401
-from .postprocess import postprocess_image, postprocess_padding, resize_bicubic_aa, equirectangular_projection  # noqa: F401
+from .postprocess import postprocess_image, postprocess_padding, resize_bicubic_aa, rot90, equirectangular_projection  # noqa: F401
 from .forward_inpaint import ForwardInpaint, LightInpaintV1  # noqa: F401
 from .mlbw_inpaint import MLBWInpaint  # noqa: F401
 from .convergence_estimator import ConvergenceEstimator, SODV1  # noqa: F401
-from .utils import apply_divergence, process_image  # noqa: F401
+from .utils import apply_divergence, process_image, preprocess_image, apply_rgbd, debug_depth_image  # noqa: F401

@@ -8,8 +8,9 @@ from .. import _lib
 from .anaglyph import apply_anaglyph_redcyan
 
 
-def resize_bicubic_aa(x, size, clamp=False):
-    """TF.resize(x, size, interpolation=BICUBIC, antialias=True) for a CHW / BCHW float tensor (csrc/postprocess.cu)."""
+def resize_bicubic_aa(x, size, clamp=False, align_corners=False):
+    """TF.resize(x, size, interpolation=BICUBIC, antialias=True) for a CHW / BCHW float tensor (csrc/postprocess.cu);
+    ``align_corners=True`` is F.interpolate(..., mode="bicubic", antialias=True, align_corners=True)."""
     _lib.require_cuda(x, "x")
     xf = x.float().contiguous()
     H, W = xf.shape[-2:]
@@ -17,8 +18,19 @@ def resize_bicubic_aa(x, size, clamp=False):
     planes = xf.numel() // (H * W)
     out = torch.empty(xf.shape[:-2] + (oh, ow), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
-        _lib.check(_lib.lib().nb200_resize_bicubic_aa(_lib.ptr(xf), planes, H, W, oh, ow, 1 if clamp else 0, _lib.ptr(out),
-                                                      _lib.stream_ptr(x.device)))
+        _lib.check(_lib.lib().nb200_resize_bicubic_aa_ac(_lib.ptr(xf), planes, H, W, oh, ow, 1 if clamp else 0,
+                                                         1 if align_corners else 0, _lib.ptr(out), _lib.stream_ptr(x.device)))
+    return out
+
+
+def rot90(x, k):
+    """torch.rot90(x, k, (-2, -1)) for k = 1 or 3 on a CHW / BCHW float tensor (csrc/frame_ops.cu), bit-exact."""
+    _lib.require_cuda(x, "x")
+    xf = x.float().contiguous()
+    H, W = xf.shape[-2:]
+    out = torch.empty(xf.shape[:-2] + (W, H), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.lib().nb200_rot90(_lib.ptr(xf), xf.numel() // (H * W), H, W, k, _lib.ptr(out), _lib.stream_ptr(x.device)))
     return out
 
 
@@ -35,9 +47,10 @@ def equirectangular_projection(c, device=None):
     return out
 
 
-def _pad(x, left, top, right, bottom):
-    # TF.pad(..., padding_mode="constant"): a zero-filled copy (layout plumbing, only with --ipd-offset / --pad options)
-    return F.pad(x, (left, right, top, bottom), mode="constant", value=0.0)
+def _pad(x, left, top, right, bottom, value=0.0):
+    # TF.pad(..., padding_mode="constant"): a constant-filled copy (layout plumbing, only with --ipd-offset / --pad options and
+    # the autocrop uncrop)
+    return F.pad(x, (left, right, top, bottom), mode="constant", value=value)
 
 
 def postprocess_padding(left_eye, right_eye, pad, pad_mode):

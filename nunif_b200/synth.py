@@ -207,6 +207,32 @@ def synth_image(seed, c, h, w, smooth=True):
     return x
 
 
+def letterbox_frame(seed, h, w, top=0, bottom=0, left=0, right=0, bar="black"):
+    """RGB frame [3][h][w] in [0,1] for the autocrop detector: uniform-noise content framed by bars ``top`` / ``bottom`` rows
+    and ``left`` / ``right`` columns wide.  ``bar``: "black" (exact 0), "tv" (near-black noise in [0, 20/255]: a bar in
+    every mode), "grey" (0.5: flat but not dark), "dark_texture" (16/255 with 80/255 on every 7th diagonal: dark on
+    average but neither black nor flat)."""
+    g = _gen(seed)
+    x = torch.rand((3, h, w), generator=g, dtype=torch.float32)
+    if bar == "black":
+        b = torch.zeros((3, h, w))
+    elif bar == "tv":
+        b = torch.rand((3, h, w), generator=g, dtype=torch.float32) * (20 / 255)
+    elif bar == "grey":
+        b = torch.full((3, h, w), 0.5)
+    elif bar == "dark_texture":
+        diag = (torch.arange(h).view(h, 1) + torch.arange(w).view(1, w)) % 7 == 0
+        b = torch.where(diag, torch.tensor(80 / 255), torch.tensor(16 / 255)).expand(3, h, w)
+    else:
+        raise ValueError(bar)
+    m = torch.zeros((h, w), dtype=torch.bool)
+    m[:top] = True
+    m[h - bottom:] = bottom > 0         # (an empty slice when bottom == 0)
+    m[:, :left] = True
+    m[:, w - right:] = right > 0
+    return torch.where(m, b, x).contiguous()
+
+
 def synth_depth(seed, b, h, w, boxes=True):
     """Smooth depth in [0,1] plus the reference _bench box pattern
     (iw3/forward_warp.py:311-316) so holes/layered holes occur."""
