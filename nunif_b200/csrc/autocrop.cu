@@ -38,14 +38,6 @@ __device__ __forceinline__ float luma(const float* p, size_t plane, const Autocr
     return a.black ? fminf(fmaxf(y, a.lo), a.hi) : y;
 }
 
-__device__ __forceinline__ unsigned float_key(float f) {
-    const unsigned u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_float(unsigned k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 // element k of the sorted v[0..n) (one warp; hist: 256 words of this warp's shared memory)
 __device__ float warp_select(const float* v, int n, unsigned k, unsigned* hist) {
     const int lane = threadIdx.x & 31;
@@ -57,7 +49,7 @@ __device__ float warp_select(const float* v, int n, unsigned k, unsigned* hist) 
             const int i = base + lane;
             unsigned digit = 256u;                       // no bin
             if (i < n) {
-                const unsigned key = float_key(v[i]);
+                const unsigned key = order_key(v[i]);
                 if ((key & mask) == prefix) digit = (key >> shift) & 255u;
             }
             // equal digits are frequent (a bar is one value): one shared atomic per distinct digit
@@ -91,28 +83,7 @@ __device__ float warp_select(const float* v, int n, unsigned k, unsigned* hist) 
         mask |= 255u << shift;
         __syncwarp();
     }
-    return key_float(prefix);
-}
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-__device__ __forceinline__ float warp_min(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ int warp_isum(int v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
+    return order_key_inv(prefix);
 }
 
 // black-mode decision from the line's sum, min and max
@@ -130,7 +101,7 @@ __device__ __forceinline__ bool flat_bar(const float* v, int n, float factor, un
     *median_out = med;
     int cnt = 0;
     for (int i = lane; i < n; i += 32) cnt += fabsf(__fsub_rn(v[i], med)) < (float)(16.0 / 255.0) ? 1 : 0;
-    cnt = warp_isum(cnt);
+    cnt = warp_sum(cnt);
     // (diff < t).float().mean(): an exact count times fl(1/n) (ATen's CUDA mean), compared with fl(0.99)
     return __fmul_rn((float)cnt, factor) > 0.99f;
 }

@@ -88,4 +88,42 @@ inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
 __device__ __forceinline__ float clamp01(float v) { return fminf(fmaxf(v, 0.f), 1.f); }
 
+// full-warp xor butterflies: every lane gets the reduction over all 32 lanes
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+__device__ __forceinline__ float warp_min(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+
+// v rounded to fp16 and back: where the reference stores an fp16 tensor
+__host__ __device__ __forceinline__ float round_f16(float v) { return __half2float(__float2half_rn(v)); }
+
+// order-preserving float -> uint key (unsigned order = float order for non-NaN values, -0 below +0; every such key > 0)
+// and its inverse
+__device__ __forceinline__ uint32_t order_key(float f) {
+    const uint32_t u = __float_as_uint(f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float order_key_inv(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
+// bicubic weight with A = -0.5 (ATen's antialiased bicubic filter)
+__device__ __forceinline__ float cubic_aa(float x) {
+    const float a = -0.5f;
+    x = fabsf(x);
+    if (x < 1.f) return ((a + 2.f) * x - (a + 3.f)) * x * x + 1.f;
+    if (x < 2.f) return (((x - 5.f) * x + 8.f) * x - 4.f) * a;
+    return 0.f;
+}
+
 }  // namespace nb200

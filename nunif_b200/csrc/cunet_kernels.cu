@@ -5,6 +5,7 @@
 //   fused with the cascade's clamp / crop-add (cunet.py:149-163).
 #include "common.cuh"
 #include "cunet_kernels.h"
+#include "ptx.cuh"
 
 namespace nb200 {
 
@@ -281,12 +282,9 @@ __global__ void __launch_bounds__(256) tail_conv_mma_kernel(const __half* __rest
         const __half* wb = sB + tap * 512 + g * 16 + 2 * t4;
 #pragma unroll
         for (int kc = 0; kc < 4; ++kc) {
-            const uint32_t a0 = *reinterpret_cast<const uint32_t*>(p0 + kc * 16), a1 = *reinterpret_cast<const uint32_t*>(p1 + kc * 16);
-            const uint32_t a2 = *reinterpret_cast<const uint32_t*>(p0 + kc * 16 + 8), a3 = *reinterpret_cast<const uint32_t*>(p1 + kc * 16 + 8);
-            const uint32_t b0 = *reinterpret_cast<const uint32_t*>(wb + kc * 128), b1 = *reinterpret_cast<const uint32_t*>(wb + kc * 128 + 8);
-            asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                         : "+f"(acc[0]), "+f"(acc[1]), "+f"(acc[2]), "+f"(acc[3])
-                         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+            const uint32_t a[4] = {*reinterpret_cast<const uint32_t*>(p0 + kc * 16), *reinterpret_cast<const uint32_t*>(p1 + kc * 16),
+                                   *reinterpret_cast<const uint32_t*>(p0 + kc * 16 + 8), *reinterpret_cast<const uint32_t*>(p1 + kc * 16 + 8)};
+            mma16816(acc, a, *reinterpret_cast<const uint32_t*>(wb + kc * 128), *reinterpret_cast<const uint32_t*>(wb + kc * 128 + 8));
         }
     }
     // accumulator layout: acc[0..1] = row g, channels 2*t4, 2*t4+1; acc[2..3] = row g+8.  Channels 0,1 live in t4 == 0,

@@ -5,35 +5,12 @@
 // softmax in fp32, and the residual stream stays fp32 (cat with the fp32 cls token promotes it) - mirrored here.
 // Restated architecture: oracle/depth_anything.py (upstream dinov2 vision_transformer.py, Depth-Anything-V2 dpt.py).
 #include "depth_kernels.h"
+#include "ptx.cuh"
 
 namespace nb200 {
 
 namespace {
 constexpr int PATCH = 14;
-
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, const void* smem_row) {
-    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(smem_row);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr));
-}
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
-    const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gmem_src) : "memory");
-}
-__device__ __forceinline__ float ex2(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
 }  // namespace
 
 // ------------------------------------------------------------------------------------------ patch embedding
@@ -95,8 +72,7 @@ __global__ void __launch_bounds__(256) add_layernorm_kernel(float* __restrict__ 
         }
         sum += (v[k][0] + v[k][1]) + (v[k][2] + v[k][3]);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    sum = warp_sum(sum);
     const float mean = sum * (1.f / DIM);
     float sq = 0.f;
 #pragma unroll
@@ -106,8 +82,7 @@ __global__ void __launch_bounds__(256) add_layernorm_kernel(float* __restrict__ 
             const float d = v[k][j] - mean;
             sq += d * d;
         }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+    sq = warp_sum(sq);
     const float rstd = rsqrtf(sq * (1.f / DIM) + 1e-6f);
     if (!out) return;
 #pragma unroll
@@ -153,7 +128,7 @@ __global__ void __launch_bounds__(128) flash_attention_kernel(const __half* __re
     };
     for (int r = rr; r < FA_BM; r += 16) cp_async16(sq + r * FA_LD + vv * 8, base + (size_t)min(q0 + r, N - 1) * ld + vv * 8);
     load_kv(0, 0);
-    asm volatile("cp.async.commit_group;" ::: "memory");
+    cp_async_commit();
 
     const int nblk = (N + FA_BN - 1) / FA_BN;
     const float sl2 = 0.125f * 1.4426950408889634f;   // head_dim**-0.5 * log2(e)
@@ -167,8 +142,8 @@ __global__ void __launch_bounds__(128) flash_attention_kernel(const __half* __re
     for (int blk = 0; blk < nblk; ++blk) {
         const int st = blk & 1;
         if (blk + 1 < nblk) load_kv(blk + 1, st ^ 1);
-        asm volatile("cp.async.commit_group;" ::: "memory");
-        asm volatile("cp.async.wait_group 1;" ::: "memory");
+        cp_async_commit();
+        cp_async_wait<1>();
         __syncthreads();
         if (blk == 0) {
 #pragma unroll
@@ -246,9 +221,9 @@ __global__ void __launch_bounds__(128) flash_attention_kernel(const __half* __re
             const __half* pv = vb + (kt * 16 + (lane & 15)) * FA_LD;
 #pragma unroll
             for (int nt = 0; nt < 8; ++nt) {
-                uint32_t b0, b1;
-                ldmatrix_x2_trans(b0, b1, pv + nt * 8);
-                mma16816(o[nt], a, b0, b1);
+                uint32_t b[2];
+                ldmatrix_x2_trans(b, smem_u32(pv + nt * 8));
+                mma16816(o[nt], a, b[0], b[1]);
             }
         }
         __syncthreads();   // everyone is done with stage `st` before the next iteration's prefetch overwrites it
@@ -388,7 +363,7 @@ __global__ void __launch_bounds__(256) head_final_kernel(const __half* __restric
         }
     }
     // the reference's conv output is fp16 under autocast, then ReLU, then .float()
-    depth[i] = fmaxf(__half2float(__float2half_rn(acc + bias)), 0.f);
+    depth[i] = fmaxf(round_f16(acc + bias), 0.f);
 }
 
 // ------------------------------------------------------------------------------------------ host wrappers

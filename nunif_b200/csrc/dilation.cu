@@ -24,19 +24,6 @@ struct DlPartial {
     float mn, mx;
 };
 
-__device__ __forceinline__ float warp_min(float v) {
-    for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ float warp_max(float v) {
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ double warp_sum(double v) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // K1: grid (nblk, B).  Each block strides over the image.
 __global__ void __launch_bounds__(DL_THREADS) range_stats_kernel(const float* __restrict__ x, float* __restrict__ range,
                                                                  DlPartial* __restrict__ partials, int h, int w) {

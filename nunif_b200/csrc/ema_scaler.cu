@@ -17,18 +17,15 @@ namespace {
 
 constexpr int ER_THREADS = 256, ER_MAX_BLOCKS = 256;
 
-__device__ __forceinline__ float wmin(float v) { for (int o = 16; o; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o)); return v; }
-__device__ __forceinline__ float wmax(float v) { for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o)); return v; }
-
 __device__ __forceinline__ void block_minmax(float& mn, float& mx) {
     __shared__ float s_mn[ER_THREADS / 32], s_mx[ER_THREADS / 32];
-    mn = wmin(mn); mx = wmax(mx);
+    mn = warp_min(mn); mx = warp_max(mx);
     if ((threadIdx.x & 31) == 0) { s_mn[threadIdx.x >> 5] = mn; s_mx[threadIdx.x >> 5] = mx; }
     __syncthreads();
     if (threadIdx.x < 32) {
         mn = threadIdx.x < ER_THREADS / 32 ? s_mn[threadIdx.x] : __int_as_float(0x7f800000);
         mx = threadIdx.x < ER_THREADS / 32 ? s_mx[threadIdx.x] : __int_as_float(0xff800000);
-        mn = wmin(mn); mx = wmax(mx);
+        mn = warp_min(mn); mx = warp_max(mx);
     }
     __syncthreads();
 }

@@ -20,6 +20,7 @@
 // co-resident per SM, which overlaps one tile's epilogue with the next tile's loads.
 #pragma once
 #include "common.cuh"
+#include "ptx.cuh"
 #include <cuda.h>
 
 namespace nb200 {
@@ -56,10 +57,8 @@ struct GemmMaps {
 };
 
 // ---------------------------------------------------------------------------------------------
-// PTX wrappers
+// mbarrier and TMA wrappers (smem_u32 and the other generic PTX wrappers: ptx.cuh)
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
@@ -218,8 +217,7 @@ __device__ __forceinline__ float gelu_erf(float x) {
     q = fmaf(q, a, 5.21468017e-02f);
     q = fmaf(q, a, 4.59595724e-01f);
     q = fmaf(q, a, 1.15100057e+00f);
-    float e;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(fmaf(-q, a, -1.0f)));   // Phi(-|x|) = erfc(|x|/sqrt2)/2: one MUFU.EX2
+    const float e = ex2(fmaf(-q, a, -1.0f));   // Phi(-|x|) = erfc(|x|/sqrt2)/2: one MUFU.EX2
     // x*Phi(x) = max(x, 0) - |x|*Phi(-|x|) on both sides of zero: no select, 9 instructions per value
     return fmaxf(x, 0.f) - a * e;
 }

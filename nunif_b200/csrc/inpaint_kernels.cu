@@ -2,6 +2,7 @@
 // (iw3/dilation.py, iw3/forward_inpaint.py:18-40) that are not convolutions.  The convolutions and Linears run on the wgmma
 // implicit GEMM (gemm.cu); the sequence is in inpaint_model.inl.
 #include "inpaint_kernels.h"
+#include "ptx.cuh"
 #include <cmath>
 
 namespace nb200 {
@@ -159,7 +160,7 @@ __global__ void __launch_bounds__(128) inpaint_stem_kernel(const float* __restri
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
                 const float v = x[((size_t)bi * 3 + c) * plane + p] * keep;
-                in[c * 16 + dy * 4 + dx] = __half2float(__float2half_rn((v - 0.5f) / 0.5f));
+                in[c * 16 + dy * 4 + dx] = round_f16((v - 0.5f) / 0.5f);
             }
         }
     uint4* dst = reinterpret_cast<uint4*>(out + tok * 96);
@@ -230,8 +231,7 @@ __global__ void __launch_bounds__(256) ln_pad_kernel(__half* __restrict__ x, con
         v[i] = lane + 32 * i < C2 ? __half22float2(xp[lane + 32 * i]) : make_float2(0.f, 0.f);
         s += v[i].x + v[i].y;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    s = warp_sum(s);
     const float mean = s / C;
     float s2 = 0.f;
 #pragma unroll
@@ -240,8 +240,7 @@ __global__ void __launch_bounds__(256) ln_pad_kernel(__half* __restrict__ x, con
         const float a = v[i].x - mean, b = v[i].y - mean;
         s2 += a * a + b * b;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    s2 = warp_sum(s2);
     const float rstd = rsqrtf(s2 / C + 1e-5f);
 #pragma unroll
     for (int i = 0; i < PER; ++i) {
@@ -293,16 +292,14 @@ __device__ __forceinline__ void mix_load(MixSmem<N>& s, const __half* __restrict
             const float2 f = __half22float2(vp[i]);
             sum += f.x + f.y;
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        sum = warp_sum(sum);
         const float mean = sum / (2 * C);
         float s2 = 0.f;
         for (int i = lane; i < C; i += 32) {
             const float2 f = __half22float2(vp[i]);
             s2 += (f.x - mean) * (f.x - mean) + (f.y - mean) * (f.y - mean);
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+        s2 = warp_sum(s2);
         if (lane == 0) {
             s.mean[n] = mean;
             s.rstd[n] = rsqrtf(s2 / (2 * C) + 1e-5f);
@@ -337,7 +334,7 @@ __global__ void __launch_bounds__(N) token_mix_mma_kernel(__half* __restrict__ u
         for (int b = 0; b < 8; ++b)
 #pragma unroll
             for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
-    const uint32_t sv = (uint32_t)__cvta_generic_to_shared(s.v);
+    const uint32_t sv = smem_u32(s.v);
 #pragma unroll 2
     for (int kt = 0; kt < N / 16; ++kt) {
         uint4 af[2];
@@ -347,18 +344,13 @@ __global__ void __launch_bounds__(N) token_mix_mma_kernel(__half* __restrict__ u
 #pragma unroll
         for (int np = 0; np < 4; ++np) {
             const int chunk = (np * 2 + (lane >> 4)) ^ (row & 7);
-            uint32_t b0, b1, b2, b3;
-            asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-                         : "=r"(b0), "=r"(b1), "=r"(b2), "=r"(b3) : "r"(sv + (uint32_t)(row * 64 + chunk * 8) * 2));
+            uint32_t b[4];
+            ldmatrix_x4_trans(b, sv + (uint32_t)(row * 64 + chunk * 8) * 2);
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
-                asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                             : "+f"(acc[mt][2 * np][0]), "+f"(acc[mt][2 * np][1]), "+f"(acc[mt][2 * np][2]), "+f"(acc[mt][2 * np][3])
-                             : "r"(af[mt].x), "r"(af[mt].y), "r"(af[mt].z), "r"(af[mt].w), "r"(b0), "r"(b1));
-                asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                             : "+f"(acc[mt][2 * np + 1][0]), "+f"(acc[mt][2 * np + 1][1]), "+f"(acc[mt][2 * np + 1][2]),
-                               "+f"(acc[mt][2 * np + 1][3])
-                             : "r"(af[mt].x), "r"(af[mt].y), "r"(af[mt].z), "r"(af[mt].w), "r"(b2), "r"(b3));
+                const uint32_t a[4] = {af[mt].x, af[mt].y, af[mt].z, af[mt].w};
+                mma16816(acc[mt][2 * np], a, b[0], b[1]);
+                mma16816(acc[mt][2 * np + 1], a, b[2], b[3]);
             }
         }
     }

@@ -10,6 +10,7 @@
 // does not grow with CIN, and the fp32 accumulators carry across chunks.
 #include "common.cuh"
 #include "legacy_kernels.h"
+#include "ptx.cuh"
 
 namespace nb200 {
 
@@ -85,20 +86,6 @@ struct HeadCfg {
     static constexpr size_t SMEM = (size_t)2 * STAGE_HALVES * sizeof(__half);
 };
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, int src_bytes) {
-    const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(s), "l"(gmem), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ void mma16816(float* acc, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(acc[0]), "+f"(acc[1]), "+f"(acc[2]), "+f"(acc[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
 template <int MODE, int CIN>
 __global__ void __launch_bounds__(256) head_conv_mma_kernel(const __half* __restrict__ x, const __half* __restrict__ frag,
                                                             const float* __restrict__ bias, __half* __restrict__ out, int Hi,
@@ -157,9 +144,9 @@ __global__ void __launch_bounds__(256) head_conv_mma_kernel(const __half* __rest
                 const __half* wb = sB + t * 512 + g * 16 + 2 * t4;
 #pragma unroll
                 for (int kc = 0; kc < 4; ++kc) {
-                    mma16816(acc[0], *reinterpret_cast<const uint32_t*>(p0 + kc * 16), *reinterpret_cast<const uint32_t*>(p1 + kc * 16),
-                             *reinterpret_cast<const uint32_t*>(p0 + kc * 16 + 8), *reinterpret_cast<const uint32_t*>(p1 + kc * 16 + 8),
-                             *reinterpret_cast<const uint32_t*>(wb + kc * 128), *reinterpret_cast<const uint32_t*>(wb + kc * 128 + 8));
+                    const uint32_t a[4] = {*reinterpret_cast<const uint32_t*>(p0 + kc * 16), *reinterpret_cast<const uint32_t*>(p1 + kc * 16),
+                                           *reinterpret_cast<const uint32_t*>(p0 + kc * 16 + 8), *reinterpret_cast<const uint32_t*>(p1 + kc * 16 + 8)};
+                    mma16816(acc[0], a, *reinterpret_cast<const uint32_t*>(wb + kc * 128), *reinterpret_cast<const uint32_t*>(wb + kc * 128 + 8));
                 }
             }
         } else {
@@ -178,11 +165,11 @@ __global__ void __launch_bounds__(256) head_conv_mma_kernel(const __half* __rest
                     const __half* wb1 = sB + ((3 - 2 * dr) * 4 + kx) * 512 + g * 16 + 2 * t4;
 #pragma unroll
                     for (int kc = 0; kc < 4; ++kc) {
-                        const uint32_t a0 = *reinterpret_cast<const uint32_t*>(p0 + kc * 16), a1 = *reinterpret_cast<const uint32_t*>(p1 + kc * 16);
-                        const uint32_t a2 = *reinterpret_cast<const uint32_t*>(p0 + kc * 16 + 8), a3 = *reinterpret_cast<const uint32_t*>(p1 + kc * 16 + 8);
-                        mma16816(acc[0], a0, a1, a2, a3, *reinterpret_cast<const uint32_t*>(wb0 + kc * 128),
-                                 *reinterpret_cast<const uint32_t*>(wb0 + kc * 128 + 8));
-                        mma16816(acc[ROWS - 1], a0, a1, a2, a3, *reinterpret_cast<const uint32_t*>(wb1 + kc * 128),
+                        const uint32_t a[4] = {*reinterpret_cast<const uint32_t*>(p0 + kc * 16), *reinterpret_cast<const uint32_t*>(p1 + kc * 16),
+                                               *reinterpret_cast<const uint32_t*>(p0 + kc * 16 + 8),
+                                               *reinterpret_cast<const uint32_t*>(p1 + kc * 16 + 8)};
+                        mma16816(acc[0], a, *reinterpret_cast<const uint32_t*>(wb0 + kc * 128), *reinterpret_cast<const uint32_t*>(wb0 + kc * 128 + 8));
+                        mma16816(acc[ROWS - 1], a, *reinterpret_cast<const uint32_t*>(wb1 + kc * 128),
                                  *reinterpret_cast<const uint32_t*>(wb1 + kc * 128 + 8));
                     }
                 }

@@ -74,17 +74,17 @@ __global__ void __launch_bounds__(256) mlbw_out_kernel(const __half* __restrict_
         const size_t base = (rowtok + (qx >> 3)) * (size_t)(8 * C1) + (qx & 7);
         for (int c = 0; c < C1; ++c) {
             // pixel_shuffle (1, 8): S[c][y][x] = token(y, x / 8)[c * 8 + x % 8]; x + x1 is rounded to fp16 like the reference's tensor
-            const float v = __half2float(__float2half_rn(__half2float(t[base + c * 8]) + __half2float(t0[base + c * 8])));
+            const float v = round_f16(__half2float(t[base + c * 8]) + __half2float(t0[base + c * 8]));
 #pragma unroll
             for (int o = 0; o < NO; ++o) acc[o] = fmaf(sw[(o * C1 + c) * 9 + tap], v, acc[o]);
         }
     }
-    if (HOLE) hole[(size_t)b * H * W + (size_t)Y * W + X] = __half2float(__float2half_rn(acc[2 * L]));   // .float() of the fp16 logit
+    if (HOLE) hole[(size_t)b * H * W + (size_t)Y * W + X] = round_f16(acc[2 * L]);   // .float() of the fp16 logit
     float lg[L], mx = -1e30f;
 #pragma unroll
     for (int l = 0; l < L; ++l) {
-        delta[((size_t)b * L + l) * H * W + (size_t)Y * W + X] = __half2float(__float2half_rn(acc[l]));   // conv output is fp16 under autocast
-        lg[l] = __half2float(__float2half_rn(acc[L + l]));
+        delta[((size_t)b * L + l) * H * W + (size_t)Y * W + X] = round_f16(acc[l]);   // conv output is fp16 under autocast
+        lg[l] = round_f16(acc[L + l]);
         mx = fmaxf(mx, lg[l]);
     }
     float sum = 0.f;

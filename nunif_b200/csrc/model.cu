@@ -174,7 +174,7 @@ static void pack_stem_w(const float* w, const float* b, int cout, int cout_pad, 
             for (int k = 0; k < 9; ++k) {
                 // the stem reads fp16 inputs and the reference runs this conv in fp16 with fp32 accumulate:
                 // keep the weights at fp16 precision
-                wv[(size_t)(k * 3 + ci) * cout_pad + co] = __half2float(__float2half_rn(w[((size_t)co * 3 + ci) * 9 + k]));
+                wv[(size_t)(k * 3 + ci) * cout_pad + co] = round_f16(w[((size_t)co * 3 + ci) * 9 + k]);
             }
     memcpy(bv.data(), b, (size_t)cout * 4);
     // ... followed by the same weights as fp16 mma.sync B fragments for stem_conv_mma_kernel:
@@ -679,7 +679,6 @@ extern "C" int nb200_tiled_render(nb200_model* m, const float* x, int C, int H, 
     NB_CHECK(batch_size > 0, "batch_size must be positive");
     int scale, offset, blend, S;
     if (model_out_geometry(m, tile_size, downscale, &scale, &offset, &blend, &S)) return 1;
-    cudaStream_t st = (cudaStream_t)stream;
     nb200_tile_config cfg;
     if (nb200_tile_config_create(H, W, scale, offset, tile_size, blend, &cfg)) return 1;
     const int ntiles = cfg.h_blocks * cfg.w_blocks;

@@ -50,14 +50,6 @@ __global__ void __launch_bounds__(256) anaglyph_mix_kernel(const float* __restri
     op[0] = o0; op[plane] = o1; op[2 * plane] = o2;
 }
 
-__device__ __forceinline__ float cubic_aa_w(float x) {
-    const float a = -0.5f;
-    x = fabsf(x);
-    if (x < 1.f) return ((a + 2.f) * x - (a + 3.f)) * x * x + 1.f;
-    if (x < 2.f) return (((x - 5.f) * x + 8.f) * x - 4.f) * a;
-    return 0.f;
-}
-
 struct ResizeParams {
     const float* x;
     float* out;
@@ -96,15 +88,15 @@ __global__ void __launch_bounds__(128) resize_bicubic_aa_kernel(ResizeParams p) 
     const AaSpan sy = aa_span(oy, p.sy, p.supy, p.H, p.align_corners), sx = aa_span(ox, p.sx, p.supx, p.W, p.align_corners);
     const int ymin = sy.lo, ysize = sy.size, xmin = sx.lo, xsize = sx.size;
     float wxs = 0.f, wys = 0.f;
-    for (int j = 0; j < xsize; ++j) wxs += cubic_aa_w(aa_arg(sx, j, p.invx, p.align_corners));
-    for (int j = 0; j < ysize; ++j) wys += cubic_aa_w(aa_arg(sy, j, p.invy, p.align_corners));
+    for (int j = 0; j < xsize; ++j) wxs += cubic_aa(aa_arg(sx, j, p.invx, p.align_corners));
+    for (int j = 0; j < ysize; ++j) wys += cubic_aa(aa_arg(sy, j, p.invy, p.align_corners));
     const float* src = p.x + (size_t)pl * p.H * p.W;
     float acc = 0.f;
     for (int jy = 0; jy < ysize; ++jy) {
-        const float wy = cubic_aa_w(aa_arg(sy, jy, p.invy, p.align_corners)) / wys;
+        const float wy = cubic_aa(aa_arg(sy, jy, p.invy, p.align_corners)) / wys;
         const float* row = src + (size_t)(ymin + jy) * p.W + xmin;
         float h = 0.f;
-        for (int jx = 0; jx < xsize; ++jx) h += cubic_aa_w(aa_arg(sx, jx, p.invx, p.align_corners)) / wxs * __ldg(row + jx);
+        for (int jx = 0; jx < xsize; ++jx) h += cubic_aa(aa_arg(sx, jx, p.invx, p.align_corners)) / wxs * __ldg(row + jx);
         acc += wy * h;
     }
     p.out[((size_t)pl * p.oh + oy) * p.ow + ox] = p.clamp ? clamp01(acc) : acc;

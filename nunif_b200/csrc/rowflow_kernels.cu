@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(256) rf_last_conv_kernel(const __half* __restr
             for (int oc = 0; oc < 8; ++oc) acc = fmaf(__half2float(tp[oc * 8]), sw[oc * 9 + ky * 3 + kx], acc);
         }
     }
-    delta[i] = __half2float(__float2half_rn(acc));   // the reference's conv output is fp16 under autocast, then .float()
+    delta[i] = round_f16(acc);   // the reference's conv output is fp16 under autocast, then .float()
 }
 
 int rf_prep(cudaStream_t st, const float* x, int B, int h, int w, int Hp, int Wt, __half* out) {

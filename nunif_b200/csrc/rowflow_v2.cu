@@ -22,6 +22,7 @@
 // fp16 add), ReLU on fp16, and non_overlap + overlap_residual is an fp16 add.
 #include "common.cuh"
 #include "rowflow_kernels.h"
+#include "ptx.cuh"
 
 namespace nb200 {
 
@@ -42,20 +43,6 @@ constexpr int OFF_NOV = OFF_C3 + 3 * BW * S32 * 2;
 constexpr int SMEM_BYTES = OFF_NOV + 3 * NC * 4;
 static_assert(RF2_PARAM_BYTES % 16 == 0 && OFF_C3 % 16 == 0 && OFF_NOV % 16 == 0, "16-byte aligned smem regions");
 
-__device__ __forceinline__ float r16(float v) { return __half2float(__float2half_rn(v)); }
-
-__device__ __forceinline__ void ldsm_x4(uint32_t (&a)[4], const __half* p) {
-    const uint32_t s = (uint32_t)__cvta_generic_to_shared(p);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
-                 : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]) : "r"(s));
-}
-
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint2 b) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b.x), "r"(b.y));
-}
-
 // One warp, two m16 tiles (columns m0 .. m0 + 15 and m0 + 64 .. m0 + 79): acc[mt][nt] += sum over the k-steps of
 // A[col][k] * B[k][n], k-step ks = (row * TAPS + tap) * CIN/16 + chunk reading channels chunk*16 .. +15 of column col + tap of
 // src[row].  The weights are B fragments in lane order, [ks][nt][lane] (rf2 packing in rowflow_v2_model.inl).
@@ -71,13 +58,13 @@ __device__ __forceinline__ void conv_mma(float (&acc)[2][NT][4], const __half* c
             for (int ch = 0; ch < CIN / 16; ++ch) {
                 const int ks = (ry * TAPS + tap) * (CIN / 16) + ch;
                 uint32_t a0[4], a1[4];
-                ldsm_x4(a0, src[ry] + (prow + tap) * stride + ch * 16 + koff);
-                ldsm_x4(a1, src[ry] + (prow + 64 + tap) * stride + ch * 16 + koff);
+                ldmatrix_x4(a0, smem_u32(src[ry] + (prow + tap) * stride + ch * 16 + koff));
+                ldmatrix_x4(a1, smem_u32(src[ry] + (prow + 64 + tap) * stride + ch * 16 + koff));
 #pragma unroll
                 for (int nt = 0; nt < NT; ++nt) {
                     const uint2 b = frag[(ks * NT + nt) * 32 + lane];
-                    mma16816(acc[0][nt], a0, b);
-                    mma16816(acc[1][nt], a1, b);
+                    mma16816(acc[0][nt], a0, b.x, b.y);
+                    mma16816(acc[1][nt], a1, b.x, b.y);
                 }
             }
 }
@@ -95,9 +82,9 @@ __device__ __forceinline__ void store_relu(const float (&acc)[2][NT][4], const f
             const float b0 = bias[n], b1 = bias[n + 1];
             const float* c = acc[mt][nt];
             *reinterpret_cast<__half2*>(dst + col * stride + n) =
-                __floats2half2_rn(fmaxf(r16(c[0]) + b0, 0.f), fmaxf(r16(c[1]) + b1, 0.f));
+                __floats2half2_rn(fmaxf(round_f16(c[0]) + b0, 0.f), fmaxf(round_f16(c[1]) + b1, 0.f));
             *reinterpret_cast<__half2*>(dst + (col + 8) * stride + n) =
-                __floats2half2_rn(fmaxf(r16(c[2]) + b0, 0.f), fmaxf(r16(c[3]) + b1, 0.f));
+                __floats2half2_rn(fmaxf(round_f16(c[2]) + b0, 0.f), fmaxf(round_f16(c[3]) + b1, 0.f));
         }
 }
 
@@ -151,7 +138,7 @@ __global__ void __launch_bounds__(THREADS, 2) rf2_kernel(const float* __restrict
             for (int k = 0; k < 3; ++k) {
                 const int xx = min(max(x0 - 14 + j + k, 0), w - 1);
 #pragma unroll
-                for (int ci = 0; ci < 3; ++ci) in[ci][k] = r16(__ldg(xb + ci * plane + (size_t)ry * w + xx));
+                for (int ci = 0; ci < 3; ++ci) in[ci][k] = round_f16(__ldg(xb + ci * plane + (size_t)ry * w + xx));
             }
             __align__(16) __half o[16];
 #pragma unroll
@@ -161,7 +148,7 @@ __global__ void __launch_bounds__(THREADS, 2) rf2_kernel(const float* __restrict
                 for (int ci = 0; ci < 3; ++ci)
 #pragma unroll
                     for (int k = 0; k < 3; ++k) acc = fmaf(in[ci][k], fw[(oc * 3 + ci) * 3 + k], acc);
-                o[oc] = __float2half_rn(fmaxf(r16(acc) + fb[oc], 0.f));
+                o[oc] = __float2half_rn(fmaxf(round_f16(acc) + fb[oc], 0.f));
             }
             uint4* dst = reinterpret_cast<uint4*>(bufF + j * S16);
             dst[0] = reinterpret_cast<const uint4*>(o)[0];
@@ -174,7 +161,7 @@ __global__ void __launch_bounds__(THREADS, 2) rf2_kernel(const float* __restrict
             float acc = 0.f;
 #pragma unroll
             for (int c = 0; c < 16; ++c) acc = fmaf(__half2float(f[c]), hw[c], acc);
-            nov[slot * NC + tid] = r16(r16(acc) + hb);
+            nov[slot * NC + tid] = round_f16(round_f16(acc) + hb);
         }
         {
             float acc[2][2][4];
@@ -215,8 +202,8 @@ __global__ void __launch_bounds__(THREADS, 2) rf2_kernel(const float* __restrict
                     for (int hi = 0; hi < 2; ++hi) {
                         const int j = m0 + mt * 64 + (lane >> 2) + hi * 8;
                         if (j < RF2_T && x0 + j < w) {
-                            const float res = r16(r16(acc[mt][0][hi * 2]) + b4);
-                            drow[x0 + j] = r16(nv[j] + res);
+                            const float res = round_f16(round_f16(acc[mt][0][hi * 2]) + b4);
+                            drow[x0 + j] = round_f16(nv[j] + res);
                         }
                     }
             }

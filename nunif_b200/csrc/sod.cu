@@ -13,6 +13,7 @@
 //   * sod_position_kernel: ConvergenceEstimator.depth_position_from_ratio, one CTA per image (mask, the two torch.quantile
 //     values by radix select, the branch, the clamp).  sod_ema_kernel: the EMA recurrence over the batch.
 #include "sod_kernels.h"
+#include "ptx.cuh"
 #include "../../include/nunif_b200.h"
 #include <cmath>
 
@@ -41,8 +42,6 @@ __device__ __forceinline__ BilTap bil_tap(float scale, int dst, int in_size) {
 __device__ __forceinline__ float bil_mix(const BilTap& ty, const BilTap& tx, float v00, float v01, float v10, float v11) {
     return fmaf(ty.l0, fmaf(tx.l0, v00, tx.l1 * v01), ty.l1 * fmaf(tx.l0, v10, tx.l1 * v11));
 }
-
-__device__ __forceinline__ float round_h(float v) { return __half2float(__float2half_rn(v)); }
 
 // rgb [B][3][H][W], depth [B][1][h][w] -> x [B][192][192][16] fp16 (r, g, b, d, sqrt(d), d*d, 0 ...), depth192 fp32
 __global__ void __launch_bounds__(256) sod_prep_kernel(const float* __restrict__ rgb, int H, int W, const float* __restrict__ depth,
@@ -91,12 +90,6 @@ struct SodConvArgs {
 };
 
 constexpr int SC_TH = 8, SC_TW = 16, SC_PX = 24, SC_WROW = 152;   // tile rows / cols; smem halves per pixel / per weight row
-
-__device__ __forceinline__ void mma16816(float* c, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
 
 template <int COUT>
 __global__ void __launch_bounds__(128) sod_conv_kernel(SodConvArgs a) {
@@ -147,12 +140,10 @@ __global__ void __launch_bounds__(128) sod_conv_kernel(SodConvArgs a) {
             for (int m = 0; m < 2; ++m) {
                 const int r = warp * 2 + m + dy;
                 const __half* ap = s_in + (r * tw + g + dx) * SC_PX + 2 * t;
-                const uint32_t a0 = *reinterpret_cast<const uint32_t*>(ap);
-                const uint32_t a1 = *reinterpret_cast<const uint32_t*>(ap + 8 * SC_PX);
-                const uint32_t a2 = *reinterpret_cast<const uint32_t*>(ap + 8);
-                const uint32_t a3 = *reinterpret_cast<const uint32_t*>(ap + 8 * SC_PX + 8);
+                const uint32_t af[4] = {*reinterpret_cast<const uint32_t*>(ap), *reinterpret_cast<const uint32_t*>(ap + 8 * SC_PX),
+                                        *reinterpret_cast<const uint32_t*>(ap + 8), *reinterpret_cast<const uint32_t*>(ap + 8 * SC_PX + 8)};
 #pragma unroll
-                for (int n = 0; n < NT; ++n) mma16816(acc[m][n], a0, a1, a2, a3, bf[n][0], bf[n][1]);
+                for (int n = 0; n < NT; ++n) mma16816(acc[m][n], af, bf[n][0], bf[n][1]);
             }
         }
     }
@@ -169,8 +160,8 @@ __global__ void __launch_bounds__(128) sod_conv_kernel(SodConvArgs a) {
 #pragma unroll
             for (int n = 0; n < NT; ++n) {
                 const int co = n * 8 + 2 * t;
-                float v0 = fmaxf(round_h(round_h(acc[m][n][hh * 2]) + a.bias[co]), 0.f);
-                float v1 = fmaxf(round_h(round_h(acc[m][n][hh * 2 + 1]) + a.bias[co + 1]), 0.f);
+                float v0 = fmaxf(round_f16(round_f16(acc[m][n][hh * 2]) + a.bias[co]), 0.f);
+                float v1 = fmaxf(round_f16(round_f16(acc[m][n][hh * 2 + 1]) + a.bias[co + 1]), 0.f);
                 if (a.res) {
                     const __half2 r = *reinterpret_cast<const __half2*>(a.res + px * a.res_ld + a.res_off + co);
                     v0 += __low2float(r);
@@ -186,7 +177,7 @@ __global__ void __launch_bounds__(128) sod_conv_kernel(SodConvArgs a) {
 int sod_conv(cudaStream_t st, const SodConvArgs& a, int cout, int B) {
     if (rec_on(REC_CONV)) {
         char line[160];
-        snprintf(line, sizeof(line), "sodconv,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d", B, a.H, a.W, a.cin, cout, a.dil, a.in_ld,
+        snprintf(line, sizeof(line), "sodconv,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d", B, a.H, a.W, a.cin, cout, a.dil, a.in_ld,
                  a.in_off, a.out_ld, a.out_off, a.res ? 1 : 0, a.res_ld);
         rec_append(line);
     }
@@ -298,7 +289,7 @@ __global__ void __launch_bounds__(256) sod_side_kernel(SodSideArgs a) {
             }
         }
     }
-    ol[(size_t)b * s * s + i] = round_h(round_h(acc) + a.w[6 * 9 * 64 + l]);
+    ol[(size_t)b * s * s + i] = round_f16(round_f16(acc) + a.w[6 * 9 * 64 + l]);
 }
 
 // d2..d6 upsampled to 192 (fp16), outconv (1x1, 6 -> 1) and the sigmoid, all rounded to fp16 as under autocast
@@ -313,12 +304,12 @@ __global__ void __launch_bounds__(256) sod_head_kernel(SodSideArgs a, const floa
         const int s = S >> l;
         const BilTap ty = bil_tap((float)s / (float)S, y, s), tx = bil_tap((float)s / (float)S, x, s);
         const float* p = a.out[l] + (size_t)b * s * s;
-        const float d = round_h(bil_mix(ty, tx, __ldg(p + ty.i0 * s + tx.i0), __ldg(p + ty.i0 * s + tx.i1),
+        const float d = round_f16(bil_mix(ty, tx, __ldg(p + ty.i0 * s + tx.i0), __ldg(p + ty.i0 * s + tx.i1),
                                         __ldg(p + ty.i1 * s + tx.i0), __ldg(p + ty.i1 * s + tx.i1)));
         acc = fmaf(d, hw[l], acc);
     }
-    const float d0 = round_h(round_h(acc) + hw[6]);
-    sal[(size_t)b * S * S + i] = round_h(1.f / (1.f + expf(-d0)));
+    const float d0 = round_f16(round_f16(acc) + hw[6]);
+    sal[(size_t)b * S * S + i] = round_f16(1.f / (1.f + expf(-d0)));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -480,12 +471,6 @@ int sod_forward(cudaStream_t st, const uint8_t* blob, const SodW& w, const float
 // ---------------------------------------------------------------------------------------------
 constexpr int POS_THREADS = 1024;
 
-__device__ __forceinline__ uint32_t f2key(float f) {
-    const uint32_t u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key2f(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
-
 // k-th smallest (0-based) of keys[0, n) by 4 radix passes of 8 bits
 __device__ float select_kth(const uint32_t* keys, int n, int k, uint32_t* hist, uint32_t* sel) {
     uint32_t prefix = 0, mask = 0;
@@ -512,7 +497,7 @@ __device__ float select_kth(const uint32_t* keys, int n, int k, uint32_t* hist, 
         k -= (int)sel[1];
         __syncthreads();
     }
-    return key2f(prefix);
+    return order_key_inv(prefix);
 }
 
 // torch.quantile(d, q), linear interpolation: rank = q * (n - 1) in fp32, ATen's lerp (two FMA forms)
@@ -536,7 +521,7 @@ __global__ void __launch_bounds__(POS_THREADS) sod_position_kernel(const float* 
     const float* s = sal + (size_t)b * n;
     const float* d = depth + (size_t)b * n;
     for (int i = threadIdx.x; i < n; i += POS_THREADS)
-        if (__ldg(s + i) > 0.5f) pos_keys[atomicAdd(&cnt, 1u)] = f2key(__ldg(d + i));
+        if (__ldg(s + i) > 0.5f) pos_keys[atomicAdd(&cnt, 1u)] = order_key(__ldg(d + i));
     __syncthreads();
     const int m = (int)cnt;
     float r;

@@ -27,40 +27,9 @@ extern int g_tune[16];  // gemm.cu (nb200_tune_set)
 
 namespace {
 constexpr int WS = 6, WTOK = 36, WPAD = 48, HEADS = 6;
-
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, const void* smem_row) {
-    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(smem_row);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr));
-}
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
 }  // namespace
 
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
-    const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gmem_src) : "memory");
-}
-
 constexpr int NKT = 5;   // key tiles of 8 columns covering the 36 keys (columns 36..39 are masked by the bias table)
-
-__device__ __forceinline__ void mma1688(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t b0) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k8.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-        : "r"(a0), "r"(a1), "r"(b0));
-}
-__device__ __forceinline__ void ldmatrix_x1_trans(uint32_t& r0, const void* smem_row) {
-    const uint32_t addr = (uint32_t)__cvta_generic_to_shared(smem_row);
-    asm volatile("ldmatrix.sync.aligned.m8n8.x1.trans.shared.b16 {%0}, [%1];" : "=r"(r0) : "r"(addr));
-}
 
 template <int D>
 struct AttnCtx {
@@ -141,9 +110,7 @@ __device__ __forceinline__ void attn_mtile(const AttnCtx<D>& cx, int mt) {
         for (int nt = 0; nt < NKT; ++nt)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                float pe;
-                asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(pe) : "f"(s[nt][2 * hlf + e] - mx));
-                s[nt][2 * hlf + e] = pe;
+                s[nt][2 * hlf + e] = ex2(s[nt][2 * hlf + e] - mx);
             }
     }
     if (LAST) {
@@ -166,9 +133,9 @@ __device__ __forceinline__ void attn_mtile(const AttnCtx<D>& cx, int mt) {
         mma16816(osum, a, ONES, ONES);
 #pragma unroll
         for (int nt = 0; nt < D / 8; ++nt) {
-            uint32_t b0, b1;
-            ldmatrix_x2_trans(b0, b1, cx.vbase[kt] + nt * 8);
-            mma16816(o[nt], a, b0, b1);
+            uint32_t b[2];
+            ldmatrix_x2_trans(b, smem_u32(cx.vbase[kt] + nt * 8));
+            mma16816(o[nt], a, b[0], b[1]);
         }
     }
     {
@@ -176,9 +143,7 @@ __device__ __forceinline__ void attn_mtile(const AttnCtx<D>& cx, int mt) {
         mma1688(osum, a0, a1, ONES);
 #pragma unroll
         for (int nt = 0; nt < D / 8; ++nt) {
-            uint32_t b0;
-            ldmatrix_x1_trans(b0, cx.vbase[2] + nt * 8);
-            mma1688(o[nt], a0, a1, b0);
+            mma1688(o[nt], a0, a1, ldmatrix_x1_trans(smem_u32(cx.vbase[2] + nt * 8)));
         }
     }
     const float inv0 = __fdividef(1.f, osum[0]);
@@ -238,8 +203,8 @@ __global__ void __launch_bounds__(192, D == 16 ? 6 : 4) window_attention_mma_ker
         cp_async16(dst + WTOK * LD, src + plane);
         cp_async16(dst + 2 * WTOK * LD, src + 2 * plane);
     }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    cp_async_commit();
+    cp_async_wait<0>();
     __syncthreads();
 
     const int head = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
@@ -441,8 +406,8 @@ __global__ void __launch_bounds__(FA_THREADS, 2) swin_attn_fused_kernel(const __
         if (tok >= 0) cp_async16(dst, x + (size_t)tok * C + u * 8);
         else *reinterpret_cast<uint4*>(dst) = make_uint4(0u, 0u, 0u, 0u);
     }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    cp_async_commit();
+    cp_async_wait<0>();
     fence_async_smem();   // generic-proxy writes of the A tile -> visible to wgmma
     consumer_bar_sync();
 

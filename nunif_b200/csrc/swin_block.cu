@@ -254,8 +254,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
             for (int q = 0; q < 4; ++q) {
                 const int j = 2 * kk + (q >> 1), i = q & 1;
                 const float2 bq = __ldg(reinterpret_cast<const float2*>(b1 + 64 * hc + 8 * j + cq));
-                const __half2 h = __floats2half2_rn(gelu_erf(hacc[buf][4 * j + 2 * i] + bq.x), gelu_erf(hacc[buf][4 * j + 2 * i + 1] + bq.y));
-                af[kk][q] = *reinterpret_cast<const uint32_t*>(&h);
+                af[kk][q] = pack_half2(gelu_erf(hacc[buf][4 * j + 2 * i] + bq.x), gelu_erf(hacc[buf][4 * j + 2 * i + 1] + bq.y));
             }
         // out += hidden_chunk W2[:, 64 hc : 64 hc + 64]^T
         const uint32_t bb = take();

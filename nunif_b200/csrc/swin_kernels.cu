@@ -5,6 +5,7 @@
 //                           (swin_unet.py:108-115, :366-379)
 #include "common.cuh"
 #include "swin_kernels.h"
+#include "ptx.cuh"
 
 namespace nb200 {
 
@@ -120,10 +121,7 @@ __global__ void __launch_bounds__(256) stem_conv_mma_kernel(const __half* __rest
         const __half* wb = sB + ks * NT * 128 + g * 16 + 2 * t4;
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt) {
-            const uint32_t b0 = *reinterpret_cast<const uint32_t*>(wb + nt * 128), b1 = *reinterpret_cast<const uint32_t*>(wb + nt * 128 + 8);
-            asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                         : "+f"(acc[nt][0]), "+f"(acc[nt][1]), "+f"(acc[nt][2]), "+f"(acc[nt][3])
-                         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+            mma16816(acc[nt], a, *reinterpret_cast<const uint32_t*>(wb + nt * 128), *reinterpret_cast<const uint32_t*>(wb + nt * 128 + 8));
         }
     }
     // bias + LeakyReLU(0.1) -> fp16, staged per warp, then 16-byte stores (one output pixel row = COUT_PAD*2 bytes)
@@ -180,14 +178,6 @@ int stem_conv3x3(cudaStream_t st, const __half* x, const float* wt, const float*
 // ToImage tail: y [n][Hs][Ws][cs] fp16 with channel = c*r*r + dy*r + dx (F.pixel_shuffle) ->
 // z planar fp16 [n][3][S][S], S = Hs*r/down.  down>1: clamp, bicubic antialias (A=-0.5) resize, clamp.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ float cubic_aa(float x) {
-    const float a = -0.5f;
-    x = fabsf(x);
-    if (x < 1.f) return ((a + 2.f) * x - (a + 3.f)) * x * x + 1.f;
-    if (x < 2.f) return (((x - 5.f) * x + 8.f) * x - 4.f) * a;
-    return 0.f;
-}
-
 __device__ __forceinline__ float shuffled_px(const __half* __restrict__ yb, int Ws, int cs, int r, int c, int Y, int X) {
     const int ty = Y / r, dy = Y - ty * r, tx = X / r, dx = X - tx * r;
     return __half2float(yb[((size_t)ty * Ws + tx) * cs + c * r * r + dy * r + dx]);

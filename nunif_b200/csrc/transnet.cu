@@ -101,8 +101,7 @@ __global__ void __launch_bounds__(TN_SIM) tn_project_kernel(const float* __restr
     const float* wr = w + (size_t)j * TN_FEAT;
     for (int k = 0; k < TN_FEAT; ++k) acc = fmaf(__ldg(wr + k), xs[k], acc);
     float ss = acc * acc;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    ss = warp_sum(ss);
     if ((j & 31) == 0) red[j >> 5] = ss;
     __syncthreads();
     const float norm = sqrtf(red[0] + red[1] + red[2] + red[3]);

@@ -243,8 +243,8 @@ __global__ void __launch_bounds__(256) backward_warp_row_kernel(BwParams p, int 
         const float is1 = __fsub_rn(__fmul_rn(__ldg(dep + (size_t)i1 * p.w + jj), p.shift), shift_conv);
         float d0 = __fmul_rn(is0, p.delta_scale), d1 = __fmul_rn(is1, p.delta_scale);
         if (F16_PRODUCT) {
-            d0 = __half2float(__float2half_rn(d0));
-            d1 = __half2float(__float2half_rn(d1));
+            d0 = round_f16(d0);
+            d1 = round_f16(d1);
         }
         GridTab t;
         t.l0 = __fsub_rn(lx, d0); t.r0 = __fadd_rn(lx, d0);
@@ -452,7 +452,7 @@ static int backward_warp_delta(const float* c, const float* delta, int B, int H,
     p.shift = 1.0f; p.shift_conv = 0.0f;
     // an fp16 tensor times the 0-dim fp32 CUDA tensor delta_scale: ATen's mul loads both operands as fp16
     // (opmath_symmetric_gpu_kernel_with_scalars -> BinaryFunctor<Half, Half, Half>, ATen/native/cuda/Loops.cuh)
-    p.delta_scale = f16 ? __half2float(__float2half_rn((float)delta_scale)) : (float)delta_scale;
+    p.delta_scale = f16 ? round_f16((float)delta_scale) : (float)delta_scale;
     p.sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
     p.sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
     p.step_x = w > 1 ? 2.0f / (float)(w - 1) : 0.f;

@@ -46,11 +46,6 @@ struct FwParams {
     const float4* coltab;    // per output column: {xmin (as int bits), w0, w1, w2} of the AA resize (upsampling only), or null
 };
 
-__device__ __forceinline__ unsigned depth_key(float d) {
-    unsigned u = __float_as_uint(d);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);  // order-preserving, > 0 for every non-NaN
-}
-
 __device__ __forceinline__ float tri(float x) {
     x = fabsf(x);
     return x < 1.f ? 1.f - x : 0.f;
@@ -177,7 +172,7 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
             float is = __fsub_rn(__fmul_rn(d, p.shift_size), conv_term);
             float fi = fminf(fmaxf(__fadd_rn((float)xp, sg * is), 0.f), (float)(Wp - 1));
             int fl = (int)floorf(fi), ce = (int)ceilf(fi);
-            unsigned key = depth_key(d);
+            unsigned key = order_key(d);
             atomicMax(&ZF[fl], key);
             atomicMax(&ZC[ce], key);
         }
@@ -188,7 +183,7 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
             float is = __fsub_rn(__fmul_rn(d, p.shift_size), conv_term);
             float fi = fminf(fmaxf(__fadd_rn((float)xp, sg * is), 0.f), (float)(Wp - 1));
             int fl = (int)floorf(fi), ce = (int)ceilf(fi);
-            unsigned key = depth_key(d);
+            unsigned key = order_key(d);
             if (ZF[fl] == key) SF[fl] = xp;
             if (ZC[ce] == key) SC[ce] = xp;
         }

@@ -193,10 +193,8 @@ __global__ void __launch_bounds__(256) zoe_seed_normed_kernel(const __half* __re
     const int lane = threadIdx.x & 31;
     if (pix >= npix) return;
     const float2 r = __half22float2(__ldg(reinterpret_cast<const __half2*>(s + (size_t)pix * NBINS) + lane));
-    const float w0 = __half2float(__float2half_rn(r.x + 1e-3f)), w1 = __half2float(__float2half_rn(r.y + 1e-3f));
-    float sum = w0 + w1;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    const float w0 = round_f16(r.x + 1e-3f), w1 = round_f16(r.y + 1e-3f);
+    const float sum = warp_sum(w0 + w1);
     const float b0 = span * (w0 / sum), b1 = span * (w1 / sum);
     float incl = b0 + b1;                          // inclusive scan of the pair widths over the lanes
 #pragma unroll
@@ -236,7 +234,7 @@ __global__ void __launch_bounds__(256) zoe_attractor_normed_kernel(const __half*
     const __half* ap = apre + (size_t)pix * lda;
     float d0 = 0.f, d1 = 0.f;
     for (int j = 0; j < na; ++j) {
-        const float a = __half2float(__float2half_rn(__half2float(__ldg(ap + 2 * j)) + 1e-3f));
+        const float a = round_f16(__half2float(__ldg(ap + 2 * j)) + 1e-3f);
         const float x0 = a - v[0], x1 = a - v[1];
         d0 += x0 / (1.f + 300.f * (x0 * x0));       // inv_attractor with its default alpha = 300, gamma = 2 (upstream quirk)
         d1 += x1 / (1.f + 300.f * (x1 * x1));
@@ -341,8 +339,7 @@ __global__ void __launch_bounds__(256) zoe_clb_final_kernel(const __half* __rest
     }
 #pragma unroll
     for (int o = 0; o < 4; ++o) {
-#pragma unroll
-        for (int s = 16; s > 0; s >>= 1) acc[o] += __shfl_xor_sync(0xffffffffu, acc[o], s);
+        acc[o] = warp_sum(acc[o]);
         // (the reference's conv output is an fp16 tensor under autocast; the fp32 sum is kept here: these 4 values are
         // amplified by up to 63 / min_temp ~ 3000 in the logits below, so their rounding dominates the output error)
         acc[o] = softplus(acc[o] + sw[320 + o]) + 1e-4f;
@@ -357,9 +354,7 @@ __global__ void __launch_bounds__(256) zoe_clb_final_kernel(const __half* __rest
         const float k = (float)(lane + 32 * j);
         y[j] = (slb[lane + 32 * j] + k * lp + (63.f - k) * lq) / temp;
     }
-    float mx = fmaxf(y[0], y[1]);
-#pragma unroll
-    for (int s = 16; s > 0; s >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, s));
+    const float mx = warp_max(fmaxf(y[0], y[1]));
     const float e0 = expf(y[0] - mx), e1 = expf(y[1] - mx);
     // bin centres at this pixel
     const int X = (int)(pix % W);

@@ -56,6 +56,7 @@ def read_records():
     recs = []
     for line in buf.value.decode().splitlines():
         kind, *vals = line.split(",")
+        assert len(vals) == len(FIELDS[kind]), line
         recs.append((kind, dict(zip(FIELDS[kind], (int(v) for v in vals)))))
     return recs
 

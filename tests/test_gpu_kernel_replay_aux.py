@@ -64,6 +64,7 @@ def recorded_aux(fn):
     recs = []
     for line in buf.value.decode().splitlines():
         kind, *vals = line.split(",")
+        assert len(vals) == len(AUX_FIELDS[kind]), line
         recs.append((kind, dict(zip(AUX_FIELDS[kind], (_num(v) for v in vals)))))
     return recs
 

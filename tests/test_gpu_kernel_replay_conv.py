@@ -69,6 +69,7 @@ def recorded_conv(fn):
     recs = []
     for line in buf.value.decode().splitlines():
         kind, *vals = line.split(",")
+        assert len(vals) == len(CONV_FIELDS[kind]), line
         recs.append((kind, dict(zip(CONV_FIELDS[kind], (_num(v) for v in vals)))))
     return recs
 
