@@ -68,27 +68,21 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// cold path of mbar_wait, kept out of line so that the many call sites of a warp-specialised kernel stay small
-static __device__ __noinline__ void mbar_timeout() {
-    printf("nb200: mbarrier wait timed out (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y, threadIdx.x);
-    __trap();
-}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     const uint32_t addr = smem_u32(bar);
     uint32_t done = 0;
     // try_wait WITH a suspend-time hint: the thread sleeps in hardware until the phase completes (or 20 us pass) instead of
     // re-issuing the instruction, so waiting warps do not take issue slots from the working ones.  Bounded: a protocol bug
-    // traps instead of hanging the GPU.
+    // traps instead of hanging the GPU.  The trap is inline and there is no diagnostic printf: a function call inside a wgmma
+    // pipeline (between a wgmma and the wait_group that retires it) makes ptxas serialise every wgmma of the kernel (C7510).
 #pragma unroll 1
-    for (uint32_t it = 0; it < (1u << 18); ++it) {     // (unroll 1: otherwise the loop is unrolled at every call site)
+    for (uint32_t it = 0; it < (1u << 18) && !done; ++it)     // (unroll 1: otherwise the loop is unrolled at every call site)
         asm volatile(
             "{\n\t.reg .pred p;\n\t"
             "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
             "selp.u32 %0, 1, 0, p;\n\t}"
             : "=r"(done) : "r"(addr), "r"(parity), "r"(20000u) : "memory");
-        if (done) return;
-    }
-    mbar_timeout();
+    if (!done) __trap();
 }
 __device__ __forceinline__ void fence_barrier_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");

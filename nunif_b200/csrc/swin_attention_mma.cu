@@ -308,184 +308,304 @@ int window_attention(cudaStream_t st, const __half* qkv, const float* bias_frag_
 
 // ---------------------------------------------------------------------------------------------
 // Fused block head: att = window_attention_core(x . Wqkv^T + bqkv), q/k/v never leave shared memory.
-// One CTA = 3 windows = 108 tokens (+20 zero rows) = the 128 rows of two wgmma warpgroups.
+// The unit of work is a tile of 3 windows = 108 tokens (+20 zero rows) = the 128 rows of two wgmma warpgroups.
 // q|k|v is computed head-major in C/32 chunks of 96 columns: chunk c holds columns [32c, 32c+32) of q, of k and of v, i.e.
 // head c (d = 32) or heads 2c, 2c+1 (d = 16), so it is complete input of the attention core for those heads.
-//   warp 8    : TMA producer of the weight blocks: per (chunk c, K-block) the rows 32c, C + 32c and 2C + 32c of Wqkv as three
-//               [32][32] boxes (64B swizzle) stacked into one [96][32] operand, C/32 chunks x C/32 K-blocks
-//   warps 0-7 : gather the rolled window tokens into a swizzled [128][C] A tile (cp.async); per chunk one wgmma
-//               accumulation (M = 64 per warpgroup), bias, fp16 into the chunk's per-window q/k/v tiles; then the chunk's
-//               (window, head, m-tile) items of the mma.sync attention core (attn_mtile, the same code as
-//               window_attention_mma_kernel) on the 8 warps, each warp writing its un-rolled output rows back to HBM.
-// Only one chunk of q/k/v is resident (25 KB instead of 127 KB for all heads at C = 192), so two CTAs share an SM at both C
-// and one CTA's GEMM overlaps the other's attention.
+//
+// Persistent and warp-specialised: one CTA per SM takes tiles blockIdx.x + k gridDim.x, and its three roles run concurrently
+// through double-buffered shared memory.  20 warps: 5 per SM sub-partition share its 64 KB register file, 96 registers each
+// (21 warps would put 6 on one sub-partition and cap every thread at 80).
+//   warp 8      : producer (one lane).  Streams Wqkv through a 4-stage ring, tile after tile.  A stage is 3 K-blocks of one
+//                 chunk; per K-block the rows 32c, C + 32c and 2C + 32c of chunk c as three [32][32] boxes (64B swizzle)
+//                 stacked into one [96][32] operand.
+//   warps 0-7   : two MMA warpgroups (64 rows each).  Per chunk the wgmma K loop into acc[48], then bias + fp16 into chunk
+//                 buffer g & 1 (g counts chunks across tiles) as per-window q/k/v tiles.
+//   warps 9-19  : 11 attention warps.  Items (window, head, m-tile) run in one sequence over all of the CTA's tiles,
+//                 chunk-major and m-tile-major within a chunk (54 per tile at both C); item n goes to attention warp n mod 11
+//                 and is attn_mtile (the same code as window_attention_mma_kernel) plus the un-rolled store of its output rows.
+//                 A warp may start on chunk g + 1 while others finish chunk g.  The attention warps also gather the NEXT tile's
+//                 rolled window rows into the other A buffer (16-byte cp.async, zeros for missing windows; rows >= 108 are
+//                 zeroed once at start-up): each warp issues its share at its first item of tile k and signals it at its
+//                 second.  They wait on q|k|v most of the time, and a single producer warp issuing both the weights and the
+//                 gather could not keep the MMA warps fed.
+//
+// Barriers (k: the CTA's tile counter, g: its chunk counter, q: its weight-stage counter; the parity of use u is u & 1):
+//   barrier        count            arrivals                                             waiters
+//   full[s]        1 (+ tx bytes)   producer expect_tx; TMA completes it                MMA warps, stage q: (q / 4) & 1
+//   empty[s]       2                thread 0 of each MMA warpgroup once the stage's      producer before stage q:
+//                                   wgmma group retired                                  ((q / 4) & 1) ^ 1
+//   afull[b]       32 x 11          every attention lane after its cp.async.wait_all     MMA warps, tile k (b = k & 1):
+//                                   and fence.proxy.async (wgmma reads the async proxy)  (k / 2) & 1
+//   aempty[b]      2                thread 0 of each MMA warpgroup after the tile's      attention warps before gathering
+//                                   last wgmma retired                                   tile k into b: ((k / 2) & 1) ^ 1
+//   cfull[b]       8                lane 0 of each MMA warp after its epilogue stores   attention warps, chunk g (b = g & 1):
+//                                                                                        (g / 2) & 1
+//   cempty[b]      items per chunk  lane 0 of the warp that ran an item of the chunk     MMA warps before the epilogue of
+//                  (9 or 18)        (items of windows past nwin arrive too)              chunk g: ((g / 2) & 1) ^ 1
+// A parity wait is exact only if the waiter is at most one phase ahead.  The producer and the MMA warps wait on every phase
+// of their barriers, and every attention warp gathers (waits on aempty) once per tile.  An attention warp waits only on the
+// chunks of its own items, which are 11 apart in the sequence, so at most 2 chunks apart: when it waits for chunk g, either
+// it waited for chunk g - 2 itself or it waited for chunk g - 1, which the MMA warps filled after chunk g - 2; and chunk
+// g + 2 cannot be filled before its own item of chunk g is done.  No wait can deadlock: a warp's first two items of tile k
+// lie in chunks the MMA warps fill from tile k alone, and at its first one the MMA warps have finished reading tile k - 1.
+// The window tables are not per tile: the region pattern of a window (the shift mask) depends only on whether it is in the
+// last window row and/or column, so the 4 patterns are built once; the token of a row is recomputed from the window index
+// where it is needed (the gather, the output stores).  So nothing per tile outlives its A buffer.
 // ---------------------------------------------------------------------------------------------
-constexpr int FA_ROWS = 128, FA_WIN = 3, FA_THREADS = GEMM_CONSUMER_THREADS + 32, FA_SLOT = 96 * 64, FA_STAGES = 4;
+constexpr int FA_ROWS = 128, FA_WIN = 3, FA_SLOT = 96 * 64, FA_KPS = 3, FA_STAGES = 4;
+constexpr int FA_MMA_THREADS = GEMM_CONSUMER_THREADS, FA_PRODUCER_WARP = FA_MMA_THREADS / 32, FA_ATTN_WARPS = 11;
+constexpr int FA_THREADS = FA_MMA_THREADS + 32 + 32 * FA_ATTN_WARPS;   // 640
 constexpr int FA_LD = 32 + 8;   // chunk tile row: 80 B = 20 words, so fragment loads and ldmatrix rows are conflict-free
 constexpr int FA_CHUNK_BYTES = FA_WIN * 3 * WTOK * FA_LD * 2;
+constexpr int FA_STAGE = FA_KPS * FA_SLOT;   // a ring stage: FA_KPS K-blocks of one chunk's [96][32] weight operand
 
 template <int C>
 struct FaCfg {
     static constexpr int X_BYTES = FA_ROWS * C * 2;
-    static constexpr int SMEM = X_BYTES + FA_STAGES * FA_SLOT + FA_CHUNK_BYTES + FA_WIN * (WTOK + WPAD) * 4 + 2 * FA_STAGES * 8 + 1024;
+    static constexpr int SMEM = 2 * X_BYTES + FA_STAGES * FA_STAGE + 2 * FA_CHUNK_BYTES + 4 * WPAD * 4 + (2 * FA_STAGES + 8) * 8 + 1024;
 };
 
+// token of row t of window (b, wy, wx) (torch.roll(-shift) :166-167); shift < H, W
+__device__ __forceinline__ int fa_token(int b, int wy, int wx, int t, int H, int W, int shift) {
+    int y = wy * WS + t / WS + shift, xx = wx * WS + t % WS + shift;
+    if (y >= H) y -= H;
+    if (xx >= W) xx -= W;
+    return (b * H + y) * W + xx;
+}
+
 template <int C>
-__global__ void __launch_bounds__(FA_THREADS, 2) swin_attn_fused_kernel(const __grid_constant__ CUtensorMap wmap,
+__global__ void __launch_bounds__(FA_THREADS, 1) swin_attn_fused_kernel(const __grid_constant__ CUtensorMap wmap,
                                                                         const __half* __restrict__ x, const float* __restrict__ bqkv,
                                                                         const float4* __restrict__ bias_frag, __half* __restrict__ out,
                                                                         int H, int W, int shift, int nwin) {
     using Cfg = FaCfg<C>;
     constexpr int D = C / HEADS, KB = C / 32, NCH = C / 32, HPC = 32 / D;   // HPC: heads per chunk
+    constexpr int IPC = 3 * FA_WIN * HPC, IPT = NCH * IPC;                  // attention items per chunk / per tile
+    constexpr int SPC = KB / FA_KPS;                                        // ring stages per chunk
+    constexpr int VPR = C / 8;                                              // 16-byte pieces per row
+    static_assert(KB % FA_KPS == 0, "a ring stage holds FA_KPS K-blocks of one chunk");
+    static_assert(FA_WIN == 3, "the gather selects among 3 windows");
     extern __shared__ uint8_t smem_dyn[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-    uint8_t* sx = smem;
-    uint8_t* ring = smem + Cfg::X_BYTES;
-    __half* sqkv = reinterpret_cast<__half*>(ring + FA_STAGES * FA_SLOT);   // [window][q|k|v][WTOK][FA_LD], one chunk
-    int* stok = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(sqkv) + FA_CHUNK_BYTES);   // [window][WTOK], -1 = none
-    int* sreg = stok + FA_WIN * WTOK;                                                         // [window][WPAD]
-    uint64_t* full = reinterpret_cast<uint64_t*>(sreg + FA_WIN * WPAD);
+    uint8_t* sx = smem;                                                      // [2][128][C] A tiles
+    uint8_t* ring = smem + 2 * Cfg::X_BYTES;
+    __half* schunk = reinterpret_cast<__half*>(ring + FA_STAGES * FA_STAGE);  // [2][window][q|k|v][WTOK][FA_LD]
+    int* sreg = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(schunk) + 2 * FA_CHUNK_BYTES);  // [last row][last col][WPAD]
+    uint64_t* full = reinterpret_cast<uint64_t*>(sreg + 4 * WPAD);
     uint64_t* empty = full + FA_STAGES;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    uint64_t* afull = empty + FA_STAGES;
+    uint64_t* aempty = afull + 2;
+    uint64_t* cfull = aempty + 2;
+    uint64_t* cempty = cfull + 2;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int nww = W / WS, nwy = H / WS;
-    if (tid < FA_WIN * WPAD) {
-        const int w = tid / WPAD, t = tid % WPAD, gw = blockIdx.x * FA_WIN + w;
+    const int ntiles = (nwin + FA_WIN - 1) / FA_WIN;
+    const int ntl = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // this CTA's tiles (>= 1)
+
+    if (tid < 4 * WPAD) {
+        // region of token t (:193-209) in a window of the last window row (p & 2) and/or column (p & 1); only read when
+        // shift > 0 and the window is in one of them
+        const int p = tid / WPAD, t = tid % WPAD;
         int reg = -1;
         if (t < WTOK) {
-            int tok = -1;
-            if (gw < nwin) {
-                const int b = gw / (nww * nwy), r = gw % (nww * nwy), wy = r / nww, wx = r % nww;
-                const int ry = wy * WS + t / WS, rx = wx * WS + t % WS;       // rolled coordinates
-                const int y = (ry + shift) % H, xx = (rx + shift) % W;        // torch.roll(-shift) :166-167
-                tok = (b * H + y) * W + xx;
-                int hr = 0, wr = 0;
-                if (shift > 0) {
-                    hr = ry < H - WS ? 0 : (ry < H - shift ? 1 : 2);
-                    wr = rx < W - WS ? 0 : (rx < W - shift ? 1 : 2);
-                }
-                reg = hr * 3 + wr;
-            }
-            stok[w * WTOK + t] = tok;
+            const int hr = (p & 2) ? (t / WS < WS - shift ? 1 : 2) : 0;
+            const int wr = (p & 1) ? (t % WS < WS - shift ? 1 : 2) : 0;
+            reg = hr * 3 + wr;
         }
-        sreg[w * WPAD + t] = reg;
+        sreg[tid] = reg;
     }
-    if (tid == GEMM_CONSUMER_THREADS) {
+    // rows 108..127 of both A tiles are zero for good
+    for (int i = tid; i < 2 * (FA_ROWS - FA_WIN * WTOK) * VPR; i += FA_THREADS) {
+        const int bsel = i / ((FA_ROWS - FA_WIN * WTOK) * VPR), j = i % ((FA_ROWS - FA_WIN * WTOK) * VPR);
+        const int r = FA_WIN * WTOK + j / VPR, u = j % VPR;
+        *reinterpret_cast<uint4*>(sx + bsel * Cfg::X_BYTES + (u >> 2) * (FA_ROWS * 64) + stage_off<32>(r, u & 3)) =
+            make_uint4(0u, 0u, 0u, 0u);
+    }
+    if (tid == FA_MMA_THREADS) {
         tma_prefetch_desc(&wmap);
         for (int s = 0; s < FA_STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 2);   // one arrival per consumer warpgroup
+            mbar_init(&empty[s], 2);   // one arrival per MMA warpgroup
+        }
+        for (int b = 0; b < 2; ++b) {
+            mbar_init(&afull[b], 32 * FA_ATTN_WARPS);
+            mbar_init(&aempty[b], 2);
+            mbar_init(&cfull[b], FA_MMA_THREADS / 32);
+            mbar_init(&cempty[b], IPC);
         }
         fence_barrier_init();
     }
+    fence_async_smem();   // the zero rows (generic-proxy writes) -> visible to wgmma
     __syncthreads();
     // the block tail (swin_block.cu, a PDL launch) may start its prologue and weight loads once every CTA of this grid is resident
     if (tid == 0) NB_PDL_TRIGGER();
 
-    if (warp == GEMM_CONSUMER_THREADS / 32) {
-        // ===================== weight producer =====================
+    if (warp == FA_PRODUCER_WARP) {
+        // ===================== producer: the weight ring, tile after tile =====================
         if (elect_one()) {
-            for (int i = 0; i < NCH * KB; ++i) {
-                const int s = i % FA_STAGES, c = i / KB;
-                mbar_wait(&empty[s], ((i / FA_STAGES) & 1) ^ 1);
-                mbar_expect_tx(&full[s], FA_SLOT);
-                // 32-row boxes at 2 KB offsets: the 64B swizzle repeats every 512 B, so the stack is laid out as one 96-row box
+            int q = 0;
+#pragma unroll 1
+            for (int k = 0; k < ntl; ++k) {
+#pragma unroll 1
+                for (int i = 0; i < NCH * SPC; ++i, ++q) {
+                    const int s = q % FA_STAGES, c = i / SPC, kb0 = (i % SPC) * FA_KPS;
+                    mbar_wait(&empty[s], ((q / FA_STAGES) & 1) ^ 1);
+                    mbar_expect_tx(&full[s], FA_STAGE);
+                    // 32-row boxes at 2 KB offsets: the 64B swizzle repeats every 512 B, so the stack is laid out as one 96-row box
 #pragma unroll
-                for (int m = 0; m < 3; ++m)
-                    tma_load_2d(&wmap, &full[s], ring + s * FA_SLOT + m * 32 * 64, (i % KB) * 32, m * C + 32 * c);
+                    for (int kk = 0; kk < FA_KPS; ++kk)
+#pragma unroll
+                        for (int m = 0; m < 3; ++m)
+                            tma_load_2d(&wmap, &full[s], ring + s * FA_STAGE + kk * FA_SLOT + m * 32 * 64, (kb0 + kk) * 32, m * C + 32 * c);
+                }
             }
         }
         return;
     }
 
-    // ===================== gather: row r = window r/36, token r%36; rows >= 108 and missing windows are zero =====================
-    // 16-byte cp.async copies: all of a thread's loads are in flight at once
-    for (int i = tid; i < FA_ROWS * (C / 8); i += GEMM_CONSUMER_THREADS) {
-        const int r = i / (C / 8), u = i % (C / 8);
-        uint8_t* dst = sx + (u >> 2) * (FA_ROWS * 64) + stage_off<32>(r, u & 3);
-        const int tok = r < FA_WIN * WTOK ? stok[r] : -1;
-        if (tok >= 0) cp_async16(dst, x + (size_t)tok * C + u * 8);
-        else *reinterpret_cast<uint4*>(dst) = make_uint4(0u, 0u, 0u, 0u);
+    const float scale = ((D == 16) ? 0.25f : 0.17677669529663687f) * 1.4426950408889634f;  // (C//heads)**-0.5 (:187) * log2(e)
+    const int g = lane >> 2, t4 = lane & 3;
+    if (warp > FA_PRODUCER_WARP) {
+        // ===================== attention: item n of the CTA's sequence on warp 9 + n mod 11 =====================
+        const int aw = warp - FA_PRODUCER_WARP - 1;
+        // this warp's share of the gather of tile `tile` into A tile sa: row r = window r/36, token r%36; 16-byte cp.async
+        auto gather = [&](int tile, uint8_t* sa) {
+            int wb[FA_WIN], wwy[FA_WIN], wwx[FA_WIN];   // (image, window row, window column) of the tile's windows; wb < 0: none
+#pragma unroll
+            for (int w = 0; w < FA_WIN; ++w) {
+                const int gw = tile * FA_WIN + w, b = gw / (nww * nwy), rw = gw - b * (nww * nwy);
+                wb[w] = gw < nwin ? b : -1;
+                wwy[w] = rw / nww;
+                wwx[w] = rw - wwy[w] * nww;
+            }
+            for (int i = aw * 32 + lane; i < FA_WIN * WTOK * VPR; i += 32 * FA_ATTN_WARPS) {
+                const int r = i / VPR, u = i % VPR, w = r / WTOK;
+                const int b = w == 0 ? wb[0] : (w == 1 ? wb[1] : wb[2]);
+                const int wy = w == 0 ? wwy[0] : (w == 1 ? wwy[1] : wwy[2]), wx = w == 0 ? wwx[0] : (w == 1 ? wwx[1] : wwx[2]);
+                uint8_t* dst = sa + (u >> 2) * (FA_ROWS * 64) + stage_off<32>(r, u & 3);
+                if (b >= 0) cp_async16(dst, x + (size_t)fa_token(b, wy, wx, r - w * WTOK, H, W, shift) * C + u * 8);
+                else *reinterpret_cast<uint4*>(dst) = make_uint4(0u, 0u, 0u, 0u);
+            }
+            cp_async_commit();
+        };
+        // the A tile is read by wgmma (the async proxy): every lane fences its own writes before it arrives
+        auto gathered = [&](int kt) {
+            cp_async_wait<0>();
+            fence_async_smem();
+            mbar_arrive(&afull[kt & 1]);
+        };
+        gather(blockIdx.x, sx);
+        gathered(0);
+        int kcur = -1, nth = 0;   // nth: this warp's items so far in tile kcur
+#pragma unroll 1
+        for (int n = aw; n < ntl * IPT; n += FA_ATTN_WARPS) {
+            const int gc = n / IPC, item = n - gc * IPC, c = gc % NCH;   // gc: chunk counter, c: chunk of the tile
+            const int kt = n / IPT, tile = blockIdx.x + kt * gridDim.x;
+            mbar_wait(&cfull[gc & 1], (gc >> 1) & 1);
+            if (kt != kcur) {
+                kcur = kt;
+                nth = 0;
+            }
+            // tile kt + 1 is gathered at this warp's first item of tile kt (chunk gc of tile kt is filled, so the MMA warps
+            // have released A buffer (kt + 1) & 1, tile kt - 1) and signalled at its second (every warp has >= 4 items per
+            // tile, both in the first 3 chunks, which the MMA warps fill without tile kt + 1)
+            if (kt + 1 < ntl && nth == 0) {
+                mbar_wait(&aempty[(kt + 1) & 1], (((kt + 1) >> 1) & 1) ^ 1);
+                gather(tile + gridDim.x, sx + ((kt + 1) & 1) * Cfg::X_BYTES);
+            }
+            if (kt + 1 < ntl && nth == 1) gathered(kt + 1);
+            ++nth;
+            // m-tile-major within the chunk, so that the cheap 4-row tiles come last
+            const int mt = item / (FA_WIN * HPC), pr = item - mt * (FA_WIN * HPC), w = pr / HPC, hh = pr - w * HPC;
+            const int gw = tile * FA_WIN + w;
+            if (gw < nwin) {
+                const int b = gw / (nww * nwy), r = gw % (nww * nwy), wy = r / nww, wx = r % nww, head = c * HPC + hh;
+                const bool lrow = wy == nwy - 1, lcol = wx == nww - 1;
+                __half* sq = schunk + (gc & 1) * (FA_CHUNK_BYTES / 2) + w * 3 * WTOK * FA_LD;
+                __half* sk = sq + WTOK * FA_LD;
+                __half* sv = sk + WTOK * FA_LD;
+                AttnCtx<D> cx;
+                cx.sq = sq; cx.sreg = sreg + (2 * lrow + lcol) * WPAD; cx.bf = bias_frag + (size_t)head * (3 * 6 * 32) + lane;
+                cx.hc = hh * D; cx.g = g; cx.t4 = t4; cx.scale = scale;
+                cx.boundary = shift > 0 && (lrow || lcol);   // only these windows mix mask regions
+#pragma unroll
+                for (int nt = 0; nt < NKT; ++nt) cx.kbase[nt] = sk + min(nt * 8 + g, WTOK - 1) * FA_LD + cx.hc + 2 * t4;
+                cx.vbase[0] = sv + (lane & 15) * FA_LD + cx.hc;
+                cx.vbase[1] = sv + (16 + (lane & 15)) * FA_LD + cx.hc;
+                cx.vbase[2] = sv + min(32 + (lane & 7), WTOK - 1) * FA_LD + cx.hc;
+                if (mt < 2) attn_mtile<D, FA_LD, false>(cx, mt);
+                else attn_mtile<D, FA_LD, true>(cx, 2);
+                // the m-tile's output rows (staged over its own q rows by this warp) -> HBM, D columns = D/8 16-byte pieces per row
+                __syncwarp();
+                const int nrow = mt < 2 ? 16 : WTOK - 32;
+                for (int e = lane; e < nrow * (D / 8); e += 32) {
+                    const int tk = 16 * mt + e / (D / 8), u = e % (D / 8);
+                    *reinterpret_cast<uint4*>(out + (size_t)fa_token(b, wy, wx, tk, H, W, shift) * C + head * D + u * 8) =
+                        *reinterpret_cast<const uint4*>(sq + tk * FA_LD + cx.hc + u * 8);
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&cempty[gc & 1]);
+        }
+        return;
     }
-    cp_async_commit();
-    cp_async_wait<0>();
-    fence_async_smem();   // generic-proxy writes of the A tile -> visible to wgmma
-    consumer_bar_sync();
 
+    // ===================== MMA warps: q | k | v = x Wqkv^T + b, chunk by chunk =====================
     const int wg = tid >> 7, t = tid & 127;
     const int row0 = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
     const int cq = 2 * (t & 3);
-    const uint32_t a_base = smem_u32(sx) + wg * 64 * 64;
-    const int lane = tid & 31, g = lane >> 2, t4 = lane & 3;
-    const float scale = ((D == 16) ? 0.25f : 0.17677669529663687f) * 1.4426950408889634f;  // (C//heads)**-0.5 (:187) * log2(e)
+    int q = 0, gc = 0;
 #pragma unroll 1
-    for (int c = 0; c < NCH; ++c) {
-        // ===================== chunk c of q | k | v = x Wqkv^T + b =====================
-        float acc[48];
-#pragma unroll
-        for (int j = 0; j < 48; ++j) acc[j] = 0.f;
+    for (int k = 0; k < ntl; ++k) {
+        mbar_wait(&afull[k & 1], (k >> 1) & 1);
+        const uint32_t a_base = smem_u32(sx + (k & 1) * Cfg::X_BYTES) + wg * 64 * 64;
 #pragma unroll 1
-        for (int kb = 0; kb < KB; ++kb) {
-            const int it = c * KB + kb, s = it % FA_STAGES;
-            mbar_wait(&full[s], (it / FA_STAGES) & 1);
-            const uint32_t a = a_base + kb * (FA_ROWS * 64), bb = smem_u32(ring + s * FA_SLOT);
-            wgmma_fence();
-            wgmma_f16<96>(acc, make_kmajor_desc<64>(a), make_kmajor_desc<64>(bb), 1u);
-            wgmma_f16<96>(acc, make_kmajor_desc<64>(a + 32), make_kmajor_desc<64>(bb + 32), 1u);
-            wgmma_commit();
-            // keep one group in flight: the stage read by the previous group is released once that group retired
-            wgmma_wait<1>();
-            if (kb > 0 && t == 0) mbar_arrive(&empty[(it - 1) % FA_STAGES]);
-        }
-        wgmma_wait<0>();
-        if (t == 0) mbar_arrive(&empty[(c * KB + KB - 1) % FA_STAGES]);
-        wgmma_fence_operands(acc);
-        consumer_bar_sync();   // every warp is done with the previous chunk's q/k/v
+        for (int c = 0; c < NCH; ++c, ++gc) {
+            float acc[48];
 #pragma unroll
-        for (int j = 0; j < 12; ++j) {
-            const int m = j >> 2, col = 8 * (j & 3) + cq;   // q|k|v, column within the chunk
-            const float2 bq = __ldg(reinterpret_cast<const float2*>(bqkv + m * C + 32 * c + col));
+            for (int j = 0; j < 48; ++j) acc[j] = 0.f;
+#pragma unroll 1
+            for (int j = 0; j < SPC; ++j, ++q) {
+                const int s = q % FA_STAGES;
+                mbar_wait(&full[s], (q / FA_STAGES) & 1);
+                wgmma_fence();
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const int r = row0 + 8 * i;
-                if (r < FA_WIN * WTOK) {
-                    const int w = r / WTOK, tk = r - w * WTOK;
-                    *reinterpret_cast<__half2*>(sqkv + ((w * 3 + m) * WTOK + tk) * FA_LD + col) =
-                        __floats2half2_rn(acc[4 * j + 2 * i] + bq.x, acc[4 * j + 2 * i + 1] + bq.y);
+                for (int kk = 0; kk < FA_KPS; ++kk) {
+                    const uint32_t a = a_base + (j * FA_KPS + kk) * (FA_ROWS * 64), bb = smem_u32(ring + s * FA_STAGE + kk * FA_SLOT);
+                    wgmma_f16<96>(acc, make_kmajor_desc<64>(a), make_kmajor_desc<64>(bb), 1u);
+                    wgmma_f16<96>(acc, make_kmajor_desc<64>(a + 32), make_kmajor_desc<64>(bb + 32), 1u);
+                }
+                wgmma_commit();
+                // keep one group in flight: the stage read by the previous group is released once that group retired
+                wgmma_wait<1>();
+                if (j > 0 && t == 0) mbar_arrive(&empty[(q - 1) % FA_STAGES]);
+            }
+            wgmma_wait<0>();
+            if (t == 0) {
+                mbar_arrive(&empty[(q - 1) % FA_STAGES]);
+                if (c == NCH - 1) mbar_arrive(&aempty[k & 1]);   // the tile's last wgmma has read A
+            }
+            wgmma_fence_operands(acc);
+            mbar_wait(&cempty[gc & 1], ((gc >> 1) & 1) ^ 1);   // every item of chunk gc - 2 is done with the buffer
+            __half* sqkv = schunk + (gc & 1) * (FA_CHUNK_BYTES / 2);
+#pragma unroll
+            for (int j = 0; j < 12; ++j) {
+                const int m = j >> 2, col = 8 * (j & 3) + cq;   // q|k|v, column within the chunk
+                const float2 bq = __ldg(reinterpret_cast<const float2*>(bqkv + m * C + 32 * c + col));
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int r = row0 + 8 * i;
+                    if (r < FA_WIN * WTOK) {
+                        const int w = r / WTOK, tk = r - w * WTOK;
+                        *reinterpret_cast<__half2*>(sqkv + ((w * 3 + m) * WTOK + tk) * FA_LD + col) =
+                            __floats2half2_rn(acc[4 * j + 2 * i] + bq.x, acc[4 * j + 2 * i + 1] + bq.y);
+                    }
                 }
             }
-        }
-        consumer_bar_sync();
-
-        // ===================== attention: the chunk's (window, head, m-tile) items on the 8 consumer warps =====================
-        // m-tile-major order, so that the items left over for a last round are the cheap 4-row tiles
-#pragma unroll 1
-        for (int item = warp; item < 3 * FA_WIN * HPC; item += GEMM_CONSUMER_THREADS / 32) {
-            const int mt = item / (FA_WIN * HPC), pr = item - mt * (FA_WIN * HPC), w = pr / HPC, hh = pr - w * HPC;
-            const int gw = blockIdx.x * FA_WIN + w;
-            if (gw >= nwin) continue;
-            const int r = gw % (nww * nwy), wy = r / nww, wx = r % nww, head = c * HPC + hh;
-            __half* sq = sqkv + w * 3 * WTOK * FA_LD;
-            __half* sk = sq + WTOK * FA_LD;
-            __half* sv = sk + WTOK * FA_LD;
-            AttnCtx<D> cx;
-            cx.sq = sq; cx.sreg = sreg + w * WPAD; cx.bf = bias_frag + (size_t)head * (3 * 6 * 32) + lane;
-            cx.hc = hh * D; cx.g = g; cx.t4 = t4; cx.scale = scale;
-            cx.boundary = shift > 0 && (wy == nwy - 1 || wx == nww - 1);   // only these windows mix mask regions
-#pragma unroll
-            for (int nt = 0; nt < NKT; ++nt) cx.kbase[nt] = sk + min(nt * 8 + g, WTOK - 1) * FA_LD + cx.hc + 2 * t4;
-            cx.vbase[0] = sv + (lane & 15) * FA_LD + cx.hc;
-            cx.vbase[1] = sv + (16 + (lane & 15)) * FA_LD + cx.hc;
-            cx.vbase[2] = sv + min(32 + (lane & 7), WTOK - 1) * FA_LD + cx.hc;
-            if (mt < 2) attn_mtile<D, FA_LD, false>(cx, mt);
-            else attn_mtile<D, FA_LD, true>(cx, 2);
-            // the m-tile's output rows (staged over its own q rows by this warp) -> HBM, D columns = D/8 16-byte pieces per row
+            // one arrival per warp: __syncwarp orders the other lanes' stores before lane 0's (release) arrive; 256 arrivals on
+            // one barrier cost about a microsecond per chunk
             __syncwarp();
-            const int nrow = mt < 2 ? 16 : WTOK - 32;
-            for (int e = lane; e < nrow * (D / 8); e += 32) {
-                const int tk = 16 * mt + e / (D / 8), u = e % (D / 8);
-                *reinterpret_cast<uint4*>(out + (size_t)stok[w * WTOK + tk] * C + head * D + u * 8) =
-                    *reinterpret_cast<const uint4*>(sq + tk * FA_LD + cx.hc + u * 8);
-            }
+            if (lane == 0) mbar_arrive(&cfull[gc & 1]);
         }
     }
 }
@@ -505,7 +625,9 @@ int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const 
     if (encode(&wmap, wqkv, 2, dims, strides, box, 64)) return 1;
     const double T = (double)B * H * W;
     ProfScope ps(st, PC_FUSED_ATTN, T * 3.0 * C * C * 2 + T * C * 36 * 4, T * C * 2, T * C * 2);   // qkv GEMM + QK^T/PV; x in, att out
-    const unsigned grid = (unsigned)((nwin + FA_WIN - 1) / FA_WIN);
+    // persistent: one CTA per SM, each taking every gridDim.x-th tile
+    const long long ntiles = (nwin + FA_WIN - 1) / FA_WIN;
+    const unsigned grid = (unsigned)std::min<long long>(ntiles, device_sm_count());
     if (rec_on()) {
         char line[96];
         snprintf(line, sizeof(line), "swin_attn,%d,%d,%d,%d,%d", B, H, W, C, shift);

@@ -44,21 +44,6 @@ struct FmMaps {
 template <int K>
 __device__ __forceinline__ float (&half96(float (&acc)[K], int h))[48] { return *reinterpret_cast<float(*)[48]>(&acc[48 * h]); }
 
-// mbar_wait without the diagnostic printf of its timeout: a function call inside a wgmma pipeline (between a wgmma and the
-// wait_group that retires it) makes ptxas serialise every wgmma of the kernel.  Still bounded: a protocol bug traps.
-__device__ __forceinline__ void fm_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done = 0;
-#pragma unroll 1
-    for (uint32_t it = 0; it < (1u << 18) && !done; ++it)
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done) : "r"(addr), "r"(parity), "r"(20000u) : "memory");
-    if (!done) __trap();
-}
-
 // wgmma.wait_group 0 or 1, with a count that is a constant after unrolling
 __device__ __forceinline__ void wgmma_wait_n(int n) {
     if (n == 0) wgmma_wait<0>();
@@ -127,7 +112,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
             auto push = [&](const CUtensorMap* m, int k0, int n0, int rows, int nbox) {
                 if (it == FM_STAGES) load_acts();   // the first FM_STAGES stages need no free slot, so cannot wait on consumers
                 const int s = it % FM_STAGES;
-                fm_wait(&empty[s], ((it / FM_STAGES) & 1) ^ 1);
+                mbar_wait(&empty[s], ((it / FM_STAGES) & 1) ^ 1);
                 mbar_expect_tx(&full[s], nbox * rows * 64);
                 for (int b = 0; b < nbox; ++b) tma_load_2d(m, &full[s], ring + s * Cfg::STAGE + b * rows * 64, k0 + 32 * b, n0);
                 ++it;
@@ -156,7 +141,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
     int it = 0, pending = 0;
     auto take = [&]() -> uint32_t {
         const int s = it % FM_STAGES;
-        fm_wait(&full[s], (it / FM_STAGES) & 1);
+        mbar_wait(&full[s], (it / FM_STAGES) & 1);
         return smem_u32(ring + s * Cfg::STAGE);
     };
     auto commit = [&]() {
@@ -183,7 +168,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
         for (int j = 0; j < NP; ++j) {
             const uint32_t bb = take();
 #pragma unroll
-            for (int kb = 2 * j; kb < 2 * j + 2 && kb < KB; ++kb) fm_wait(&abar[kb], 0);
+            for (int kb = 2 * j; kb < 2 * j + 2 && kb < KB; ++kb) mbar_wait(&abar[kb], 0);
             wgmma_fence();
 #pragma unroll
             for (int kb = 2 * j; kb < 2 * j + 2 && kb < KB; ++kb) {
@@ -199,7 +184,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
         }
         retire(0);
         wgmma_fence_operands(acc);
-        fm_wait(xbar, 0);
+        mbar_wait(xbar, 0);
 #pragma unroll
         for (int j = 0; j < C / 8; ++j) {
             const int col = 8 * j + cq;
@@ -214,7 +199,7 @@ __global__ void __launch_bounds__(FM_THREADS, 1) swin_mlp_fused_kernel(const __g
         fence_async_smem();   // x1 (generic-proxy writes) -> A operand of this warpgroup's fc1 wgmma
         asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
     } else {
-        fm_wait(xbar, 0);
+        mbar_wait(xbar, 0);
     }
 
     float oacc[C / 2];

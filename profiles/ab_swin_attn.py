@@ -17,7 +17,8 @@ median ms per call and the max-min spread of each build, the ratio of medians, a
 Also printed: the device, its power limit and SM clocks sampled during the timed region, and per kernel the registers, the
 dynamic shared memory of its launches (from a torch.profiler trace) and the CTAs per SM that
 cuOccupancyMaxActiveBlocksPerMultiprocessor (the driver form of cudaOccupancyMaxActiveBlocksPerMultiprocessor) reports for
-the kernel's cubin at that launch configuration.
+the kernel's cubin at that launch configuration (block size and shared memory as the trace recorded them, so each build is
+queried at its own).
 """
 import argparse
 import ctypes
@@ -35,7 +36,6 @@ SHAPES = [(240, 96), (120, 192), (60, 192), (240, 192)]   # (H = W, C) of the sw
 BATCH = 16
 REPS = 7
 WINDOW_MS = 60.0
-FA_THREADS = 288
 KERNEL = "_ZN5nb20022swin_attn_fused_kernelILi{C}EEEv14CUtensorMap_stPK6__halfPKfPK6float4PS2_iiii"
 
 
@@ -84,7 +84,7 @@ def window_ms(lib, t, shift, n):
 
 
 def launch_smem(libs, dev):
-    """dynamic + static shared memory and registers of each build's swin_attn_fused_kernel<C> launches (torch.profiler trace)."""
+    """shared memory, registers and block size of each build's swin_attn_fused_kernel<C> launches (torch.profiler trace)."""
     import torch
     from torch.profiler import ProfilerActivity, profile
     out = {}
@@ -101,11 +101,12 @@ def launch_smem(libs, dev):
                 ev = [e for e in json.load(open(path))["traceEvents"]
                       if e.get("cat") == "kernel" and "swin_attn_fused_kernel" in e.get("name", "")]
                 a = ev[0]["args"]
-                out[(tag, C)] = {"smem": int(a["shared memory"]), "regs_trace": int(a["registers per thread"])}
+                out[(tag, C)] = {"smem": int(a["shared memory"]), "regs_trace": int(a["registers per thread"]),
+                                 "threads": a["block"][0] * a["block"][1] * a["block"][2]}
     return out
 
 
-def occupancy(so_path, C, smem):
+def occupancy(so_path, C, smem, threads):
     """CTAs per SM of swin_attn_fused_kernel<C> from the build's own cubin, loaded with the driver API into the current context."""
     name = KERNEL.format(C=C)
     cuobjdump = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "cuobjdump")
@@ -124,7 +125,7 @@ def occupancy(so_path, C, smem):
         ck(cu.cuFuncSetAttribute(fn, 8, ctypes.c_int(smem)))   # CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES
         regs, n = ctypes.c_int(), ctypes.c_int()
         ck(cu.cuFuncGetAttribute(ctypes.byref(regs), 4, fn))   # CU_FUNC_ATTRIBUTE_NUM_REGS
-        ck(cu.cuOccupancyMaxActiveBlocksPerMultiprocessor(ctypes.byref(n), fn, FA_THREADS, ctypes.c_size_t(smem)))
+        ck(cu.cuOccupancyMaxActiveBlocksPerMultiprocessor(ctypes.byref(n), fn, threads, ctypes.c_size_t(smem)))
     finally:
         cu.cuModuleUnload(mod)
     return regs.value, n.value
@@ -157,9 +158,10 @@ def main():
     kern = []
     try:
         for (tag, C), s in sorted(launch_smem(libs, dev).items()):
-            regs, ctas = occupancy(paths[tag], C, s["smem"])
-            kern.append({"build": tag, "C": C, "regs": regs, "dyn_smem": s["smem"], "ctas_per_sm": ctas})
-            print(f"# {tag:4s} swin_attn_fused_kernel<{C}>: {regs} registers, {s['smem']} B shared memory/CTA, {ctas} CTA(s)/SM")
+            regs, ctas = occupancy(paths[tag], C, s["smem"], s["threads"])
+            kern.append({"build": tag, "C": C, "regs": regs, "dyn_smem": s["smem"], "threads": s["threads"], "ctas_per_sm": ctas})
+            print(f"# {tag:4s} swin_attn_fused_kernel<{C}>: {s['threads']} threads, {regs} registers, {s['smem']} B shared memory/CTA, "
+                  f"{ctas} CTA(s)/SM")
     except Exception as e:  # noqa: BLE001  (the timing below does not depend on it)
         kern.append({"error": f"{type(e).__name__}: {e}"})
         print(f"# occupancy query failed: {type(e).__name__}: {e}")
