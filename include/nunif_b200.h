@@ -536,6 +536,17 @@ int nb200_swin_attn_fused_f16(const void* x, const void* wqkv, const float* bqkv
 int nb200_hwc_to_chw_f32(const void* x, int bits, int B, int H, int W, float* out, void* stream);
 int nb200_chw_f32_to_hwc(const float* x, int bits, int B, int H, int W, void* out, void* stream);
 
+/* nunif/utils/video.py:309-416 hdr2sdr (steps 1-6), the HDR input stage of input_reformatter (:1025-1041): PQ (HDR10) or
+ * HLG BT.2020 -> Hable tone map -> BT.709 / BT.601 SDR, one fused pass.  x [B][H][W][3] uint16 rgb48, full range;
+ * trc = the stream's color_trc code (16 PQ, 18 HLG); params_host = {pq_exposure, pq_white_point, hlg_exposure,
+ * hlg_white_point, hlg_saturation_gain} as the Python floats (defaults 110, 5, 1.2, 0.8, 0.9).
+ * out_float = 0: out [B][H][W][3] uint16, the rgb48 frame hdr2sdr returns (truncating cast);
+ * out_float = 1: out [B][3][H][W] fp32, that frame / 65535 exactly as nb200_hwc_to_chw_f32 makes it.
+ * Every op rounds to fp32 as ATen's CUDA kernels do; the 3x3 matrix (torch.mm) sums in its own order. */
+enum { NB200_TRC_PQ = 16, NB200_TRC_HLG = 18, NB200_SDR_BT709 = 0, NB200_SDR_BT601 = 1 };
+int nb200_hdr2sdr(const uint16_t* x, int B, int H, int W, int trc, int colorspace, const double* params_host,
+                  int out_float, void* out, void* stream);
+
 /* DepthAnything batch_preprocess (iw3/depth_anything_model.py:69-110): size rule (host,
  * integers) and the fused antialiased-bilinear resize + clamp + ImageNet normalise:
  * x [B][3][H][W] fp32 in [0,1] -> out [B][3][new_h][new_w] fp32. */

@@ -14,10 +14,69 @@ queues directly - no threads, no locks, deterministic ticket order:
 submission order (possibly empty) - the calling convention of ``FrameCallbackPool.__call__``; ``pipeline(None)`` /
 ``finish()`` drains.  ``frame_callback(batch)`` receives B,3,H,W float32 in [0,1] on the GPU and returns B',3,H',W' float
 (B' may differ from B: models with look-ahead buffers emit later), exactly what the reference's batch callbacks do.
+
+``hdr2sdr`` is the reference's HDR input stage (video.py:309-416, applied by input_reformatter :1025-1041 when
+``use_hdr2sdr`` holds): PQ / HLG BT.2020 rgb48 frames tone-mapped to BT.709 / BT.601 SDR by csrc/hdr2sdr.cu.
+``FrameBatchPipeline(..., hdr2sdr=(color_trc, output_colorspace))`` runs it as the uint16 -> float conversion of each batch.
 """
+import ctypes
+
 import torch
 
+from .. import _lib
 from ..iw3.frames import hwc_to_chw_float, chw_float_to_hwc
+
+COLORSPACE_BT2020 = 9
+COLOR_TRC_SMPTE2084 = 16            # PQ (HDR10)
+COLOR_TRC_ARIB_STD_B67 = 18         # HLG
+_HDR2SDR_TARGETS = {"bt709", "bt709-tv", "bt709-pc", "bt601", "bt601-tv", "bt601-pc"}
+_SDR_COLORSPACE = {"bt709": 0, "bt601": 1}   # NB200_SDR_BT709 / NB200_SDR_BT601
+
+
+def use_hdr2sdr(frame_colorspace, color_trc, target_colorspace):
+    """The condition of input_reformatter (video.py:1026-1029): a BT.2020 frame of a PQ or HLG stream, written out as
+    BT.709 / BT.601 (``target_colorspace`` with or without its -tv / -pc suffix)."""
+    return (frame_colorspace == COLORSPACE_BT2020 and color_trc in {COLOR_TRC_SMPTE2084, COLOR_TRC_ARIB_STD_B67}
+            and target_colorspace in _HDR2SDR_TARGETS)
+
+
+def _check_hdr2sdr_args(color_trc, output_colorspace, output="uint16"):
+    if color_trc not in (COLOR_TRC_SMPTE2084, COLOR_TRC_ARIB_STD_B67):
+        raise ValueError(f"color_trc must be {COLOR_TRC_SMPTE2084} (PQ) or {COLOR_TRC_ARIB_STD_B67} (HLG), got {color_trc!r}")
+    if output_colorspace not in _SDR_COLORSPACE:
+        raise ValueError(f"output_colorspace must be 'bt709' or 'bt601', got {output_colorspace!r}")
+    if output not in ("uint16", "float"):
+        raise ValueError(f"output must be 'uint16' or 'float', got {output!r}")
+
+
+def hdr2sdr(x, color_trc, output_colorspace, pq_exposure=110.0, pq_white_point=5.0, hlg_exposure=1.2, hlg_white_point=0.8,
+            hlg_saturation_gain=0.9, output="uint16", device=None):
+    """nunif/utils/video.py:309-416 on rgb48 frames: x uint16 HWC or BHWC, full range, BT.2020 with the PQ (color_trc 16)
+    or HLG (18) transfer, moved to ``device`` (default: x's device, which must be a GPU).
+
+    output="uint16": the tone-mapped rgb48 frame(s) hdr2sdr returns, same shape as x.
+    output="float":  that frame / 65535 as float32 CHW / BCHW - the frame ``to_tensor`` / ``hwc_to_chw_float`` would make of
+                     it, without the intermediate uint16 frame."""
+    _check_hdr2sdr_args(color_trc, output_colorspace, output)
+    if not torch.is_tensor(x) or x.dtype != torch.uint16:
+        raise ValueError("hdr2sdr expects a uint16 (rgb48) tensor")
+    if x.ndim not in (3, 4) or x.shape[-1] != 3:
+        raise ValueError(f"hdr2sdr expects HWC or BHWC frames with 3 channels, got shape {tuple(x.shape)}")
+    dev = torch.device(device) if device is not None else x.device
+    if dev.type != "cuda":
+        raise ValueError("hdr2sdr runs on a CUDA (sm_90) device: pass device= a GPU or a CUDA tensor")
+    xc = x.to(dev).contiguous()
+    B = 1 if x.ndim == 3 else x.shape[0]
+    H, W = x.shape[-3], x.shape[-2]
+    if output == "float":
+        out = torch.empty((B, 3, H, W), dtype=torch.float32, device=xc.device)
+    else:
+        out = torch.empty((B, H, W, 3), dtype=torch.uint16, device=xc.device)
+    params = (ctypes.c_double * 5)(pq_exposure, pq_white_point, hlg_exposure, hlg_white_point, hlg_saturation_gain)
+    with torch.cuda.device(xc.device):
+        _lib.check(_lib.lib().nb200_hdr2sdr(_lib.ptr(xc), B, H, W, int(color_trc), _SDR_COLORSPACE[output_colorspace], params,
+                                            int(output == "float"), _lib.ptr(out), _lib.stream_ptr(xc.device)))
+    return out[0] if x.ndim == 3 else out
 
 
 class _Slot:
@@ -33,8 +92,17 @@ class _Slot:
 
 
 class FrameBatchPipeline:
-    def __init__(self, frame_callback, batch_size, device="cuda:0", depth=3, use_16bit=False, copy_output=True):
+    def __init__(self, frame_callback, batch_size, device="cuda:0", depth=3, use_16bit=False, copy_output=True, hdr2sdr=None):
         assert batch_size > 0 and depth >= 2
+        # (color_trc, output_colorspace): tone-map each uint16 batch to SDR (hdr2sdr(..., output="float")) in place of the
+        # plain uint16 -> float conversion, so the callback receives SDR frames
+        if hdr2sdr is not None:
+            if not use_16bit:
+                raise ValueError("hdr2sdr needs use_16bit=True (rgb48 frames)")
+            color_trc, output_colorspace = hdr2sdr
+            _check_hdr2sdr_args(color_trc, output_colorspace)
+            hdr2sdr = (color_trc, output_colorspace)
+        self.hdr2sdr = hdr2sdr
         self.frame_callback = frame_callback
         self.batch_size = int(batch_size)
         self.device = torch.device(device)
@@ -100,7 +168,10 @@ class FrameBatchPipeline:
         slot.direct = 0
         comp.wait_event(slot.ready)
         with torch.inference_mode():
-            x = hwc_to_chw_float(slot.d_in[:n])
+            if self.hdr2sdr is None:
+                x = hwc_to_chw_float(slot.d_in[:n])
+            else:
+                x = hdr2sdr(slot.d_in[:n], *self.hdr2sdr, output="float")
             y = self.frame_callback(x)
             if y is not None and y.numel() > 0:
                 u = chw_float_to_hwc(y, use_16bit=self.bits == 16)
