@@ -45,8 +45,8 @@ struct AttnCtx {
 
 // One 16-row query tile of one head: S = Q K^T, bias/mask, base-2 softmax numerators, O = P V, normalise, stage.
 // LD: row stride (halves) of the q/k/v tiles.  LAST: query rows 32..35 only (accumulator rows g+8 are padding and are not
-// evaluated).
-template <int D, int LD, bool LAST>
+// evaluated).  BNT: key tiles per m-tile in cx.bf, 6 for the packed table in global memory, NKT for a copy in shared memory.
+template <int D, int LD, bool LAST, int BNT = 6>
 __device__ __forceinline__ void attn_mtile(const AttnCtx<D>& cx, int mt) {
     constexpr uint32_t ONES = 0x3C003C00u;   // half2(1, 1)
     constexpr int HL = LAST ? 1 : 2;         // accumulator row halves in use
@@ -78,7 +78,7 @@ __device__ __forceinline__ void attn_mtile(const AttnCtx<D>& cx, int mt) {
     // scale + bias + key padding is one FMA per element and the softmax runs in base 2.
 #pragma unroll
     for (int nt = 0; nt < NKT; ++nt) {
-        const float4 bv = __ldg(cx.bf + (mt * 6 + nt) * 32);
+        const float4 bv = BNT == 6 ? __ldg(cx.bf + (mt * 6 + nt) * 32) : cx.bf[(mt * BNT + nt) * 32];
         s[nt][0] = fmaf(s[nt][0], cx.scale, bv.x);
         s[nt][1] = fmaf(s[nt][1], cx.scale, bv.y);
         if (!LAST) {
@@ -318,8 +318,9 @@ int window_attention(cudaStream_t st, const __half* qkv, const float* bias_frag_
 //   warp 8      : producer (one lane).  Streams Wqkv through a 4-stage ring, tile after tile.  A stage is 3 K-blocks of one
 //                 chunk; per K-block the rows 32c, C + 32c and 2C + 32c of chunk c as three [32][32] boxes (64B swizzle)
 //                 stacked into one [96][32] operand.
-//   warps 0-7   : two MMA warpgroups (64 rows each).  Per chunk the wgmma K loop into acc[48], then bias + fp16 into chunk
-//                 buffer g & 1 (g counts chunks across tiles) as per-window q/k/v tiles.
+//   warps 0-7   : two MMA warpgroups (64 rows each).  Per chunk the wgmma K loop into acc[48], then bias (bqkv, staged in
+//                 shared memory once per CTA) + fp16 into chunk buffer g & 1 (g counts chunks across tiles) as per-window q/k/v
+//                 tiles.
 //   warps 9-19  : 11 attention warps.  Items (window, head, m-tile) run in one sequence over all of the CTA's tiles,
 //                 chunk-major and m-tile-major within a chunk (54 per tile at both C); item n goes to attention warp n mod 11
 //                 and is attn_mtile (the same code as window_attention_mma_kernel) plus the un-rolled store of its output rows.
@@ -362,7 +363,15 @@ constexpr int FA_STAGE = FA_KPS * FA_SLOT;   // a ring stage: FA_KPS K-blocks of
 template <int C>
 struct FaCfg {
     static constexpr int X_BYTES = FA_ROWS * C * 2;
-    static constexpr int SMEM = 2 * X_BYTES + FA_STAGES * FA_STAGE + 2 * FA_CHUNK_BYTES + 4 * WPAD * 4 + (2 * FA_STAGES + 8) * 8 + 1024;
+    // The attention warps read the relative-position-bias fragments of every item.  Where they fit (C = 96) the NKT key tiles
+    // of each (head, m-tile) are copied to shared memory once per CTA; at C = 192 (4.3 KB left) they are read from L1/L2.
+    static constexpr bool SBF = C == 96;
+    static constexpr int SBF_BYTES = SBF ? HEADS * 3 * NKT * 32 * 16 : 0;
+    static constexpr int SBF_OFF = 2 * X_BYTES + FA_STAGES * FA_STAGE + 2 * FA_CHUNK_BYTES + 4 * WPAD * 4 + (2 * FA_STAGES + 8) * 8 +
+                                   3 * C * 4;
+    static constexpr int SMEM = SBF_OFF + SBF_BYTES + 1024;
+    static_assert(SBF_OFF % 16 == 0, "float4 bias fragments");
+    static_assert(SMEM <= 232448, "over the 227 KB opt-in shared memory of an H100 CTA");
 };
 
 // token of row t of window (b, wy, wx) (torch.roll(-shift) :166-167); shift < H, W
@@ -386,7 +395,9 @@ __global__ void __launch_bounds__(FA_THREADS, 1) swin_attn_fused_kernel(const __
     static_assert(KB % FA_KPS == 0, "a ring stage holds FA_KPS K-blocks of one chunk");
     static_assert(FA_WIN == 3, "the gather selects among 3 windows");
     extern __shared__ uint8_t smem_dyn[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+    // aligned by an offset from smem_dyn, not by integer arithmetic on its address: the compiler then knows every pointer
+    // below is a shared-memory one and emits LDS/STS instead of generic loads and stores
+    uint8_t* smem = smem_dyn + ((1024u - (smem_u32(smem_dyn) & 1023u)) & 1023u);
     uint8_t* sx = smem;                                                      // [2][128][C] A tiles
     uint8_t* ring = smem + 2 * Cfg::X_BYTES;
     __half* schunk = reinterpret_cast<__half*>(ring + FA_STAGES * FA_STAGE);  // [2][window][q|k|v][WTOK][FA_LD]
@@ -397,6 +408,8 @@ __global__ void __launch_bounds__(FA_THREADS, 1) swin_attn_fused_kernel(const __
     uint64_t* aempty = afull + 2;
     uint64_t* cfull = aempty + 2;
     uint64_t* cempty = cfull + 2;
+    float* sbias = reinterpret_cast<float*>(cempty + 2);   // [3C] bqkv
+    float4* sbf = reinterpret_cast<float4*>(smem + Cfg::SBF_OFF);   // [head][m-tile][NKT][32] bias fragments (Cfg::SBF)
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int nww = W / WS, nwy = H / WS;
     const int ntiles = (nwin + FA_WIN - 1) / FA_WIN;
@@ -414,6 +427,10 @@ __global__ void __launch_bounds__(FA_THREADS, 1) swin_attn_fused_kernel(const __
         }
         sreg[tid] = reg;
     }
+    for (int i = tid; i < 3 * C; i += FA_THREADS) sbias[i] = bqkv[i];
+    if (Cfg::SBF)   // from the packed [head][m-tile][6][32] table
+        for (int i = tid; i < HEADS * 3 * NKT * 32; i += FA_THREADS)
+            sbf[i] = __ldg(bias_frag + ((i >> 5) / NKT * 6 + (i >> 5) % NKT) * 32 + (i & 31));
     // rows 108..127 of both A tiles are zero for good
     for (int i = tid; i < 2 * (FA_ROWS - FA_WIN * WTOK) * VPR; i += FA_THREADS) {
         const int bsel = i / ((FA_ROWS - FA_WIN * WTOK) * VPR), j = i % ((FA_ROWS - FA_WIN * WTOK) * VPR);
@@ -525,7 +542,8 @@ __global__ void __launch_bounds__(FA_THREADS, 1) swin_attn_fused_kernel(const __
                 __half* sk = sq + WTOK * FA_LD;
                 __half* sv = sk + WTOK * FA_LD;
                 AttnCtx<D> cx;
-                cx.sq = sq; cx.sreg = sreg + (2 * lrow + lcol) * WPAD; cx.bf = bias_frag + (size_t)head * (3 * 6 * 32) + lane;
+                cx.sq = sq; cx.sreg = sreg + (2 * lrow + lcol) * WPAD;
+                cx.bf = Cfg::SBF ? sbf + head * (3 * NKT * 32) + lane : bias_frag + (size_t)head * (3 * 6 * 32) + lane;
                 cx.hc = hh * D; cx.g = g; cx.t4 = t4; cx.scale = scale;
                 cx.boundary = shift > 0 && (lrow || lcol);   // only these windows mix mask regions
 #pragma unroll
@@ -533,8 +551,9 @@ __global__ void __launch_bounds__(FA_THREADS, 1) swin_attn_fused_kernel(const __
                 cx.vbase[0] = sv + (lane & 15) * FA_LD + cx.hc;
                 cx.vbase[1] = sv + (16 + (lane & 15)) * FA_LD + cx.hc;
                 cx.vbase[2] = sv + min(32 + (lane & 7), WTOK - 1) * FA_LD + cx.hc;
-                if (mt < 2) attn_mtile<D, FA_LD, false>(cx, mt);
-                else attn_mtile<D, FA_LD, true>(cx, 2);
+                constexpr int BNT = Cfg::SBF ? NKT : 6;
+                if (mt < 2) attn_mtile<D, FA_LD, false, BNT>(cx, mt);
+                else attn_mtile<D, FA_LD, true, BNT>(cx, 2);
                 // the m-tile's output rows (staged over its own q rows by this warp) -> HBM, D columns = D/8 16-byte pieces per row
                 __syncwarp();
                 const int nrow = mt < 2 ? 16 : WTOK - 32;
@@ -591,7 +610,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1) swin_attn_fused_kernel(const __
 #pragma unroll
             for (int j = 0; j < 12; ++j) {
                 const int m = j >> 2, col = 8 * (j & 3) + cq;   // q|k|v, column within the chunk
-                const float2 bq = __ldg(reinterpret_cast<const float2*>(bqkv + m * C + 32 * c + col));
+                const float2 bq = *reinterpret_cast<const float2*>(sbias + m * C + 32 * c + col);
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
                     const int r = row0 + 8 * i;
