@@ -619,24 +619,20 @@ int nb200_profile_enable(int on);
 int nb200_profile_report(char* buf, size_t cap);
 int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launch: class,ms,work,read_bytes,write_bytes */
 
-/* Launch recorder for tests: a non-zero `on` clears the record and appends one CSV line per launch of the kinds its bits
- * select; on = 0 stops.  Bit 0 (on = 1): the implicit GEMM, the ViT attention and the fused Swin-block head and tail (gemm,
- * attn, swin_attn, swin_mlp).  Bit 1 (on = 2): the WABlock core and pad, the ViT add + LayerNorm, the DPT upsample and the
- * ZoeDepth bins head (wmha .. zrelbias).  Bit 2 (on = 4): the waifu2x stem, tail and head convolutions, the SE block,
- * to_image and the SOD REBNCONV (stem .. sodconv; path = the kernel the host chose: 0 mma.sync, 1 SIMT).  Other bits are
- * refused.  Off by default; recording changes no launch.  Lines (has_* / normed: 0 or 1):
- *   gemm,kind,pad,dil,B,Hi,Wi,Ci,Cin,a_row_stride,a_img_stride,a_planes,a_plane_stride,N,act,ldo,out_mode,cout,
- *        split_stride,has_bias,has_res,ldr,res_H,res_W,res_cy,res_cx,res_before_act,has_A2,Cin2,ld2,out_is_res,out_is_A,
- *        block_n,bk,grid
- *   attn,B,N,heads,has_bias,ldb      swin_attn,B,H,W,C,shift      swin_mlp,T,C,proj,cs
- *   wmha,B,H,W,C,ws,heads,pad_y,pad_x      reppad,B,H,W,C      ln,rows,dim,has_delta,has_out      upbl,B,h,w,C,H,W
- *   zadd_up,B,h,w,C,H,W      zsoftplus,n      zseed,npix,min,max      zattr,B,h,w,H,W,lda,na,normed,min,max,has_sorted
- *   zclb_concat,B,h,w,H,W      zclb_final,B,h,w,H,W,ldg      zrelbias,ph,pw,heads,ldb
- *   stem,n,Hi,Wi,cout_pad,ldo,path      tail,mode,epi,n,Hi,Wi,z1H,z1W,clip,path      head,mode,cin,n,Hi,Wi,path
- *   se,n,H,W,C      toimg,n,Hs,Ws,cs,r,down      sodconv,B,H,W,cin,cout,dil,in_ld,in_off,out_ld,out_off,has_res,res_ld
- * (min / max: fp32 depths printed with 9 significant digits, 0 for an unnormed attractor).  recorded_launches copies them (NUL-terminated) like nb200_profile_dump; it fails if cap is too small. */
+/* Launch recorder for tests: a non-zero `on` clears the record and appends one line per launch of the kinds its bits
+ * select; on = 0 stops.  Off by default; recording changes no launch.  Other bits are refused.
+ *   bit 0 (on = 1): gemm attn swin_attn swin_mlp (the implicit GEMM, the ViT attention, the fused Swin-block head and tail)
+ *   bit 1 (on = 2): wmha reppad ln upbl zadd_up zsoftplus zseed zattr zclb_concat zclb_final zrelbias (the WABlock core and
+ *                   pad, the ViT add + LayerNorm, the DPT upsample and the ZoeDepth bins head)
+ *   bit 2 (on = 4): stem tail head se toimg sodconv (the waifu2x stem, tail and head convolutions, the SE block, to_image
+ *                   and the SOD REBNCONV)
+ * A line is `kind,name=value,name=value,...`: the launch's fields without its pointers, named where the host code writes
+ * them.  Values are integers (flags 0 or 1) or fp32 values printed with 9 significant digits.  recorded_launches_named copies
+ * the lines (NUL-terminated) like nb200_profile_dump; recorded_launches copies them without the names (`kind,value,...`, the
+ * values in the same order).  Both fail if cap is too small. */
 int nb200_record_launches(int on);
 int nb200_recorded_launches(char* buf, size_t cap);
+int nb200_recorded_launches_named(char* buf, size_t cap);
 
 #ifdef __cplusplus
 }

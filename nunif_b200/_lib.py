@@ -177,6 +177,7 @@ SIGNATURES = {
                                            c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "nb200_record_launches": (c_int, [c_int]),
     "nb200_recorded_launches": (c_int, [c_char_p, c_size_t]),
+    "nb200_recorded_launches_named": (c_int, [c_char_p, c_size_t]),
     "nb200_tune_set": (c_int, [c_int, c_int]),
     "nb200_debug_tap": (c_int, [c_int, c_void_p, ctypes.c_size_t]),
     "nb200_profile_enable": (c_int, [c_int]),

@@ -43,10 +43,22 @@ void prof_end(cudaStream_t st) {
 std::atomic<int> g_rec_enabled{0};
 static std::mutex g_rec_mu;
 static std::string g_rec;
-void rec_append(const char* line) {
+RecField::RecField(const char* n, double v) : name(n) {
+    char s[32];
+    snprintf(s, sizeof(s), "%.9g", v);
+    value = s;
+}
+void rec_launch(const char* kind, std::initializer_list<RecField> fields) {
+    std::string line = kind;
+    for (const RecField& f : fields) {
+        line += ',';
+        line += f.name;
+        line += '=';
+        line += f.value;
+    }
+    line += '\n';
     std::lock_guard<std::mutex> lk(g_rec_mu);
     g_rec += line;
-    g_rec += '\n';
 }
 
 static std::mutex g_attr_mu;
@@ -171,11 +183,31 @@ extern "C" int nb200_record_launches(int on) {
     return 0;
 }
 
-// One CSV line per recorded launch; the first field names the kind (gemm, attn, swin_attn, swin_mlp, wmha, ln, z...: see the header).
-extern "C" int nb200_recorded_launches(char* buf, size_t cap) {
+static int copy_record(const std::string& s, char* buf, size_t cap) {
     NB_CHECK(buf && cap > 0, "null buffer");
-    std::lock_guard<std::mutex> lk(g_rec_mu);
-    NB_CHECK(g_rec.size() + 1 <= cap, "buffer too small: " + std::to_string(g_rec.size() + 1) + " bytes needed");
-    memcpy(buf, g_rec.c_str(), g_rec.size() + 1);
+    NB_CHECK(s.size() + 1 <= cap, "buffer too small: " + std::to_string(s.size() + 1) + " bytes needed");
+    memcpy(buf, s.c_str(), s.size() + 1);
     return 0;
+}
+
+// One line per recorded launch, `kind,name=value,...` (the kinds: see the header).
+extern "C" int nb200_recorded_launches_named(char* buf, size_t cap) {
+    std::lock_guard<std::mutex> lk(g_rec_mu);
+    return copy_record(g_rec, buf, cap);
+}
+
+// The same lines without the names, `kind,value,...`: the positional form this entry point has always returned.
+extern "C" int nb200_recorded_launches(char* buf, size_t cap) {
+    std::lock_guard<std::mutex> lk(g_rec_mu);
+    std::string s;
+    bool in_name = false;   // names and values hold neither ',' nor '='
+    for (const char c : g_rec) {
+        if (in_name) {
+            in_name = c != '=';
+            continue;
+        }
+        s += c;
+        in_name = c == ',';
+    }
+    return copy_record(s, buf, cap);
 }

@@ -6,6 +6,8 @@
 #include <stdio.h>
 #include <string>
 #include <atomic>
+#include <initializer_list>
+#include <type_traits>
 
 struct nb200_tile_config;  // include/nunif_b200.h
 
@@ -59,14 +61,23 @@ struct ProfScope {
     }
 };
 
-// ---- optional launch recorder (nb200_record_launches): the host code of the recorded kernels appends one CSV line per launch
+// ---- optional launch recorder (nb200_record_launches): the host code of the recorded kernels appends one line per launch
 // describing it without its pointers, so tests can replay every configuration a network uses.  The recorder's mask selects
 // the kinds: REC_GEMMS the GEMM, ViT attention and fused Swin block; REC_AUX the WABlock core, add + LayerNorm, DPT upsample
 // and ZoeDepth bins head; REC_CONV the waifu2x stem / tail / head convolutions, the SE block, to_image and the SOD REBNCONV.
 enum { REC_GEMMS = 1, REC_AUX = 2, REC_CONV = 4 };
 extern std::atomic<int> g_rec_enabled;
-void rec_append(const char* line);
 inline bool rec_on(int kinds = REC_GEMMS) { return (g_rec_enabled.load(std::memory_order_relaxed) & kinds) != 0; }
+// one field of a recorded line: integers and flags print as integers, floating-point values with 9 significant digits
+struct RecField {
+    const char* name;
+    std::string value;
+    template <typename T, typename std::enable_if<std::is_integral<T>::value, int>::type = 0>
+    RecField(const char* n, T v) : name(n), value(std::to_string(v)) {}
+    RecField(const char* n, double v);
+};
+// appends the line `kind,name=value,...`; the call sites are the record format's only definition
+void rec_launch(const char* kind, std::initializer_list<RecField> fields);
 
 // seam_blend.cu: rows [y0, y1) of the blended output (used by the band-pipelined host render in model.cu)
 int tile_gather_blend_rows(const void* z_all, int z_f32, int C, const ::nb200_tile_config* cfg, int scale, int offset, int tile_size,

@@ -94,11 +94,7 @@ __global__ void __launch_bounds__(256) se_scale_kernel(__half* __restrict__ x, c
 
 int se_block(cudaStream_t st, __half* x, int n, int H, int W, int C, const float* w1, const float* b1, const float* w2,
              const float* b2, float* partial, float* scale) {
-    if (rec_on(REC_CONV)) {
-        char line[96];
-        snprintf(line, sizeof(line), "se,%d,%d,%d,%d", n, H, W, C);
-        rec_append(line);
-    }
+    if (rec_on(REC_CONV)) rec_launch("se", {{"n", n}, {"H", H}, {"W", W}, {"C", C}});
     const int HW = H * W, nchunks = cdiv(HW, SE_CHUNK);
     ProfScope ps(st, PC_SE, (double)n * HW * C * 2 * 3);
     if (C == 64) {
@@ -335,11 +331,9 @@ int tail_conv(cudaStream_t st, int mode, int epi, const __half* x, const float* 
     const size_t total = (size_t)n * Ho * Wo;
     const unsigned blocks = (unsigned)cdiv64(total, 128);
     const bool mma = g_tune[7] == 0 && (mode == 0 || Wo % 2 == 0) && n <= 65535;
-    if (rec_on(REC_CONV)) {
-        char line[128];
-        snprintf(line, sizeof(line), "tail,%d,%d,%d,%d,%d,%d,%d,%d,%d", mode, epi, n, Hi, Wi, z1H, z1W, clip, mma ? 0 : 1);
-        rec_append(line);
-    }
+    if (rec_on(REC_CONV))
+        rec_launch("tail", {{"mode", mode}, {"epi", epi}, {"n", n}, {"Hi", Hi}, {"Wi", Wi}, {"z1H", z1H}, {"z1W", z1W},
+                            {"clip", clip}, {"path", mma ? 0 : 1}});
     ProfScope ps(st, PC_TAIL, (double)n * Hi * Wi * 128 + (double)total * 16);
     if (mma) {
         int rc;

@@ -384,11 +384,7 @@ int da_assemble_tokens(cudaStream_t st, const __half* T, const float* cls, const
 
 int da_add_layernorm(cudaStream_t st, float* X32, const __half* delta, const float* w, const float* b, __half* out, long long rows,
                      int dim) {
-    if (rec_on(REC_AUX)) {
-        char line[96];
-        snprintf(line, sizeof(line), "ln,%lld,%d,%d,%d", rows, dim, delta ? 1 : 0, out ? 1 : 0);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("ln", {{"rows", rows}, {"dim", dim}, {"has_delta", delta ? 1 : 0}, {"has_out", out ? 1 : 0}});
     const unsigned grid = (unsigned)cdiv64(rows, 8);
     switch (dim) {
         case 256: add_layernorm_kernel<256><<<grid, 256, 0, st>>>(X32, delta, w, b, out, rows); break;
@@ -405,11 +401,8 @@ int da_attention(cudaStream_t st, const __half* qkv, __half* out, int B, int N, 
     const size_t smem = (size_t)(FA_BM + 4 * FA_BN) * FA_LD * sizeof(__half);
     const double T = (double)B * N * heads * FA_D;
     ProfScope ps(st, PC_ATTN, 4.0 * T * N, T * 3 * 2 + (bias_log2e ? (double)heads * N * N * 4 : 0.0), T * 2);
-    if (rec_on()) {
-        char line[96];
-        snprintf(line, sizeof(line), "attn,%d,%d,%d,%d,%d", B, N, heads, bias_log2e ? 1 : 0, bias_log2e ? ldb : 0);
-        rec_append(line);
-    }
+    if (rec_on())
+        rec_launch("attn", {{"B", B}, {"N", N}, {"heads", heads}, {"has_bias", bias_log2e ? 1 : 0}, {"ldb", bias_log2e ? ldb : 0}});
     if (bias_log2e) {
         NB_CHECK(ldb % 2 == 0 && ldb >= cdiv(N, FA_BN) * FA_BN, "bias row stride must be even and cover whole 64-key blocks");
         if (ensure_dyn_smem((const void*)flash_attention_kernel<true>, smem)) return 1;
@@ -431,11 +424,7 @@ int da_relu_add(cudaStream_t st, const __half* x, const __half* x0, __half* y, _
 }
 
 int da_upsample_bilinear(cudaStream_t st, const __half* x, int B, int h, int w, int C, __half* out, int H, int W) {
-    if (rec_on(REC_AUX)) {
-        char line[96];
-        snprintf(line, sizeof(line), "upbl,%d,%d,%d,%d,%d,%d", B, h, w, C, H, W);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("upbl", {{"B", B}, {"h", h}, {"w", w}, {"C", C}, {"H", H}, {"W", W}});
     NB_CHECK(C % 8 == 0, "channels must be a multiple of 8");
     const float sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
     const long long total = (long long)B * H * W * (C / 8);

@@ -263,16 +263,17 @@ int conv_gemm(cudaStream_t st, const ConvGemm& g) {
                  in_px * (g.kind == CG_LINEAR_FLAT ? g.Cin * g.a_planes : g.Cin) * 2.0 + (g.res ? Mrows * g.N * 2.0 : 0.0) +
                      4.0 * Mrows * g.Cin2 * (a2 ? 2.0 : 0.0) + (double)g.N * K * 2.0,
                  Mrows * (double)g.N * 2.0);
-    if (rec_on()) {
-        char line[512];
-        snprintf(line, sizeof(line),
-                 "gemm,%d,%d,%d,%d,%d,%d,%d,%d,%lld,%lld,%d,%lld,%d,%d,%d,%d,%d,%lld,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d",
-                 g.kind, g.pad, g.dil, g.B, g.Hi, g.Wi, g.Ci, g.Cin, g.a_row_stride, g.a_img_stride, g.a_planes, g.a_plane_stride,
-                 g.N, g.act, g.ldo, g.out_mode, g.cout, g.split_stride, g.bias ? 1 : 0, g.res ? 1 : 0, g.ldr, g.res_H, g.res_W,
-                 g.res_cy, g.res_cx, g.res_before_act, a2 ? 1 : 0, g.Cin2, g.ld2, g.res && (const void*)g.out == (const void*)g.res,
-                 (const void*)g.out == (const void*)g.A, bn, BK, m_tiles * p.n_tiles);
-        rec_append(line);
-    }
+    if (rec_on())
+        rec_launch("gemm", {{"kind", g.kind}, {"pad", g.pad}, {"dil", g.dil}, {"B", g.B}, {"Hi", g.Hi}, {"Wi", g.Wi}, {"Ci", g.Ci},
+                            {"Cin", g.Cin}, {"a_row_stride", g.a_row_stride}, {"a_img_stride", g.a_img_stride},
+                            {"a_planes", g.a_planes}, {"a_plane_stride", g.a_plane_stride}, {"N", g.N}, {"act", g.act},
+                            {"ldo", g.ldo}, {"out_mode", g.out_mode}, {"cout", g.cout}, {"split_stride", g.split_stride},
+                            {"has_bias", g.bias ? 1 : 0}, {"has_res", g.res ? 1 : 0}, {"ldr", g.ldr}, {"res_H", g.res_H},
+                            {"res_W", g.res_W}, {"res_cy", g.res_cy}, {"res_cx", g.res_cx}, {"res_before_act", g.res_before_act},
+                            {"has_a2", a2 ? 1 : 0}, {"Cin2", g.Cin2}, {"ld2", g.ld2},
+                            {"out_is_res", g.res && (const void*)g.out == (const void*)g.res},
+                            {"out_is_a", (const void*)g.out == (const void*)g.A}, {"block_n", bn}, {"bk", BK},
+                            {"grid", m_tiles * p.n_tiles}});
     return BK == 64 ? launch_bn<64>(bn, st, maps, p, m_tiles, p.n_tiles) : launch_bn<32>(bn, st, maps, p, m_tiles, p.n_tiles);
 }
 

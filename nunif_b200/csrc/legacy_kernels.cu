@@ -226,11 +226,8 @@ int head_conv(cudaStream_t st, int mode, int cin, const __half* x, const float* 
     const int Ho = mode == 0 ? Hi - 2 : 2 * Hi - 4, Wo = mode == 0 ? Wi - 2 : 2 * Wi - 4;
     NB_CHECK(Ho > 0 && Wo > 0, "head_conv: input too small");
     const bool mma = g_tune[7] == 0 && (mode == 0 || Wo % 2 == 0) && n <= 65535;
-    if (rec_on(REC_CONV)) {
-        char line[96];
-        snprintf(line, sizeof(line), "head,%d,%d,%d,%d,%d,%d", mode, cin, n, Hi, Wi, mma ? 0 : 1);
-        rec_append(line);
-    }
+    if (rec_on(REC_CONV))
+        rec_launch("head", {{"mode", mode}, {"cin", cin}, {"n", n}, {"Hi", Hi}, {"Wi", Wi}, {"path", mma ? 0 : 1}});
     const double rbytes = (double)n * Hi * Wi * cin * 2, wbytes = (double)n * Ho * Wo * 3 * 2;
     ProfScope ps(st, PC_TAIL, rbytes + wbytes, rbytes, wbytes);
     if (mode == 0 && cin == 128) return launch_head<0, 128>(st, mma, x, wt, bias, out, n, Hi, Wi, Ho, Wo);

@@ -175,12 +175,10 @@ __global__ void __launch_bounds__(128) sod_conv_kernel(SodConvArgs a) {
 
 // one REBNCONV launch over B images (the network's layers and nb200_sod_conv_f16)
 int sod_conv(cudaStream_t st, const SodConvArgs& a, int cout, int B) {
-    if (rec_on(REC_CONV)) {
-        char line[160];
-        snprintf(line, sizeof(line), "sodconv,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d", B, a.H, a.W, a.cin, cout, a.dil, a.in_ld,
-                 a.in_off, a.out_ld, a.out_off, a.res ? 1 : 0, a.res_ld);
-        rec_append(line);
-    }
+    if (rec_on(REC_CONV))
+        rec_launch("sodconv", {{"B", B}, {"H", a.H}, {"W", a.W}, {"cin", a.cin}, {"cout", cout}, {"dil", a.dil}, {"in_ld", a.in_ld},
+                               {"in_off", a.in_off}, {"out_ld", a.out_ld}, {"out_off", a.out_off}, {"has_res", a.res ? 1 : 0},
+                               {"res_ld", a.res_ld}});
     NB_CHECK(cout == 16 || cout == 64, "output channels must be 16 or 64");
     NB_CHECK(a.cin > 0 && a.cin % 16 == 0 && a.in_ld % 8 == 0 && a.in_off % 8 == 0 && a.in_off + a.cin <= a.in_ld,
              "input channels must be a multiple of 16 inside a 16-byte aligned slice");

@@ -647,11 +647,7 @@ int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const 
     // persistent: one CTA per SM, each taking every gridDim.x-th tile
     const long long ntiles = (nwin + FA_WIN - 1) / FA_WIN;
     const unsigned grid = (unsigned)std::min<long long>(ntiles, device_sm_count());
-    if (rec_on()) {
-        char line[96];
-        snprintf(line, sizeof(line), "swin_attn,%d,%d,%d,%d,%d", B, H, W, C, shift);
-        rec_append(line);
-    }
+    if (rec_on()) rec_launch("swin_attn", {{"B", B}, {"H", H}, {"W", W}, {"C", C}, {"shift", shift}});
     const float4* bf = reinterpret_cast<const float4*>(bias_frag_f);
     if (C == 96) {
         if (ensure_dyn_smem((const void*)swin_attn_fused_kernel<96>, FaCfg<96>::SMEM)) return 1;

@@ -438,11 +438,7 @@ int swin_mlp_fused(cudaStream_t st, __half* x, const __half* att, long long T, i
     ProfScope ps(st, PC_FUSED_MLP, Td * C * 2 * (C * ((att ? 1 : 0) + 4) + (y ? cs : 0)), Td * C * 2 * (att ? 2 : 1),
                  Td * (y ? cs : C) * 2);
     const int ntiles = (int)((T + FM_ROWS - 1) / FM_ROWS);
-    if (rec_on()) {
-        char line[96];
-        snprintf(line, sizeof(line), "swin_mlp,%lld,%d,%d,%d", T, C, att ? 1 : 0, y ? cs : 0);
-        rec_append(line);
-    }
+    if (rec_on()) rec_launch("swin_mlp", {{"T", T}, {"C", C}, {"proj", att ? 1 : 0}, {"cs", y ? cs : 0}});
     if (y) return C == 96 ? launch_mlp<96, true, 16>(st, ntiles, maps, bp, b1, b2, by) : launch_mlp<192, true, 48>(st, ntiles, maps, bp, b1, b2, by);
     if (C == 96) return att ? launch_mlp<96, true>(st, ntiles, maps, bp, b1, b2) : launch_mlp<96, false>(st, ntiles, maps, bp, b1, b2);
     return att ? launch_mlp<192, true>(st, ntiles, maps, bp, b1, b2) : launch_mlp<192, false>(st, ntiles, maps, bp, b1, b2);

@@ -150,11 +150,8 @@ int stem_conv3x3(cudaStream_t st, const __half* x, const float* wt, const float*
                  int cout_pad, int ldo) {
     NB_CHECK(ldo >= cout_pad && ldo % 8 == 0, "bad output stride");
     const bool mma = g_tune[7] == 0 && n <= 65535 && (cout_pad == 64 || cout_pad == 32);
-    if (rec_on(REC_CONV)) {
-        char line[96];
-        snprintf(line, sizeof(line), "stem,%d,%d,%d,%d,%d,%d", n, Hi, Wi, cout_pad, ldo, mma ? 0 : 1);
-        rec_append(line);
-    }
+    if (rec_on(REC_CONV))
+        rec_launch("stem", {{"n", n}, {"Hi", Hi}, {"Wi", Wi}, {"cout_pad", cout_pad}, {"ldo", ldo}, {"path", mma ? 0 : 1}});
     if (mma) {
         const int Ho = Hi - 2, Wo = Wi - 2;
         ProfScope ps(st, PC_STEM, (double)n * Hi * Wi * 16 + (double)n * Ho * Wo * ldo * 2, (double)n * Hi * Wi * 16, (double)n * Ho * Wo * cout_pad * 2);
@@ -323,11 +320,7 @@ __global__ void __launch_bounds__(256) to_image_down_kernel(const __half* __rest
 }
 
 int to_image(cudaStream_t st, const __half* y, void* z, int n, int Hs, int Ws, int cs, int r, int down) {
-    if (rec_on(REC_CONV)) {
-        char line[96];
-        snprintf(line, sizeof(line), "toimg,%d,%d,%d,%d,%d,%d", n, Hs, Ws, cs, r, down);
-        rec_append(line);
-    }
+    if (rec_on(REC_CONV)) rec_launch("toimg", {{"n", n}, {"Hs", Hs}, {"Ws", Ws}, {"cs", cs}, {"r", r}, {"down", down}});
     NB_CHECK(down == 1 || down == 2 || down == 4, "downscale must be 1, 2 or 4");
     NB_CHECK(Hs == Ws && (Hs * r) % down == 0, "bad ToImage geometry");
     const size_t total = (size_t)n * 3 * (Hs * r / down) * (Ws * r / down);

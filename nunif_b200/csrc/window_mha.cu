@@ -136,11 +136,9 @@ __global__ void __launch_bounds__(256) reppad1_kernel(const uint4* __restrict__ 
 
 int window_mha(cudaStream_t st, const __half* qkv, const float* qkv_bias, const float* bias, __half* out, int B, int H, int W, int C,
                int ws, int heads, int pad_y, int pad_x) {
-    if (rec_on(REC_AUX)) {
-        char line[128];
-        snprintf(line, sizeof(line), "wmha,%d,%d,%d,%d,%d,%d,%d,%d", B, H, W, C, ws, heads, pad_y, pad_x);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX))
+        rec_launch("wmha", {{"B", B}, {"H", H}, {"W", W}, {"C", C}, {"ws", ws}, {"heads", heads}, {"pad_y", pad_y},
+                            {"pad_x", pad_x}});
     NB_CHECK(H % ws == 0 && W % ws == 0, "token grid must be a multiple of the window");
     // a shifted direction pads ws / 2 on both sides; the padded grid must still tile into whole windows (not so for odd ws)
     NB_CHECK((pad_y == 0 || pad_y == ws / 2) && (pad_x == 0 || pad_x == ws / 2), "padding must be 0 or ws / 2");
@@ -158,11 +156,7 @@ int window_mha(cudaStream_t st, const __half* qkv, const float* qkv_bias, const 
 }
 
 int reppad1(cudaStream_t st, const __half* x, int B, int H, int W, int C, __half* out) {
-    if (rec_on(REC_AUX)) {
-        char line[96];
-        snprintf(line, sizeof(line), "reppad,%d,%d,%d,%d", B, H, W, C);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("reppad", {{"B", B}, {"H", H}, {"W", W}, {"C", C}});
     NB_CHECK(C % 8 == 0, "channels must be a multiple of 8");
     const long long total = (long long)B * (H + 2) * (W + 2) * (C / 8);
     reppad1_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out), B, H, W, C / 8);

@@ -407,11 +407,7 @@ int zoe_add_cast(cudaStream_t st, float* X32, const __half* delta, __half* out, 
 
 int zoe_expand_rel_bias(cudaStream_t st, const float* table, int ph, int pw, int heads, float* bias, int ldb) {
     const long long N = (long long)ph * pw + 1, total = (long long)heads * N * N;
-    if (rec_on(REC_AUX)) {
-        char line[160];
-        snprintf(line, sizeof(line), "zrelbias,%d,%d,%d,%d", ph, pw, heads, ldb);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("zrelbias", {{"ph", ph}, {"pw", pw}, {"heads", heads}, {"ldb", ldb}});
     NB_CHECK(ldb >= N, "bias row stride too small");
     zoe_expand_rel_bias_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(table, ph, pw, heads, bias, ldb);
     NB_LAUNCHED();
@@ -428,11 +424,7 @@ int zoe_readout_concat(cudaStream_t st, const __half* F, int B, int P, int dim, 
 }
 
 int zoe_add_upsampled(cudaStream_t st, const __half* e, const __half* prev, int B, int h, int w, int C, int H, int W, __half* y) {
-    if (rec_on(REC_AUX)) {
-        char line[160];
-        snprintf(line, sizeof(line), "zadd_up,%d,%d,%d,%d,%d,%d", B, h, w, C, H, W);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("zadd_up", {{"B", B}, {"h", h}, {"w", w}, {"C", C}, {"H", H}, {"W", W}});
     NB_CHECK(C % 8 == 0, "channels must be a multiple of 8");
     const long long total = (long long)B * H * W * (C / 8);
     zoe_add_upsampled_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(e, prev, B, h, w, C / 8, H, W, ac_scale(h, H), ac_scale(w, W), y);
@@ -441,11 +433,7 @@ int zoe_add_upsampled(cudaStream_t st, const __half* e, const __half* prev, int 
 }
 
 int zoe_softplus(cudaStream_t st, const __half* x, float* out, long long n) {
-    if (rec_on(REC_AUX)) {
-        char line[160];
-        snprintf(line, sizeof(line), "zsoftplus,%lld", n);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("zsoftplus", {{"n", n}});
     zoe_softplus_kernel<<<(unsigned)cdiv64(n, 256), 256, 0, st>>>(x, out, n);
     NB_LAUNCHED();
     return 0;
@@ -453,11 +441,9 @@ int zoe_softplus(cudaStream_t st, const __half* x, float* out, long long n) {
 
 int zoe_attractor(cudaStream_t st, const __half* apre, int lda, int na, const float* prev_bin, int B, int h, int w, int H, int W,
                   float* out) {
-    if (rec_on(REC_AUX)) {
-        char line[160];
-        snprintf(line, sizeof(line), "zattr,%d,%d,%d,%d,%d,%d,%d,0,0,0,0", B, h, w, H, W, lda, na);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX))
+        rec_launch("zattr", {{"B", B}, {"h", h}, {"w", w}, {"H", H}, {"W", W}, {"lda", lda}, {"na", na}, {"normed", 0}, {"min", 0},
+                             {"max", 0}, {"has_sorted", 0}});
     NB_CHECK(na >= 1 && na <= lda, "bad attractor count");
     const long long total = (long long)B * H * W * NBINS;
     zoe_attractor_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(apre, lda, na, prev_bin, B, h, w, H, W, ac_scale(h, H), ac_scale(w, W), out);
@@ -466,11 +452,7 @@ int zoe_attractor(cudaStream_t st, const __half* apre, int lda, int na, const fl
 }
 
 int zoe_seed_normed(cudaStream_t st, const __half* s, long long npix, float min_depth, float max_depth, float* out) {
-    if (rec_on(REC_AUX)) {
-        char line[160];
-        snprintf(line, sizeof(line), "zseed,%lld,%.9g,%.9g", npix, min_depth, max_depth);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("zseed", {{"npix", npix}, {"min", min_depth}, {"max", max_depth}});
     NB_CHECK(max_depth > min_depth, "max_depth must exceed min_depth");
     zoe_seed_normed_kernel<<<(unsigned)cdiv64(npix * 32, 256), 256, 0, st>>>(s, npix, min_depth, max_depth - min_depth, out);
     NB_LAUNCHED();
@@ -479,11 +461,9 @@ int zoe_seed_normed(cudaStream_t st, const __half* s, long long npix, float min_
 
 int zoe_attractor_normed(cudaStream_t st, const __half* apre, int lda, int na, const float* prev_bin, int B, int h, int w, int H, int W,
                          float min_depth, float max_depth, float* out, float* sorted) {
-    if (rec_on(REC_AUX)) {
-        char line[160];
-        snprintf(line, sizeof(line), "zattr,%d,%d,%d,%d,%d,%d,%d,1,%.9g,%.9g,%d", B, h, w, H, W, lda, na, min_depth, max_depth, sorted ? 1 : 0);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX))
+        rec_launch("zattr", {{"B", B}, {"h", h}, {"w", w}, {"H", H}, {"W", W}, {"lda", lda}, {"na", na}, {"normed", 1},
+                             {"min", min_depth}, {"max", max_depth}, {"has_sorted", sorted ? 1 : 0}});
     NB_CHECK(na >= 1 && 2 * na <= lda, "bad attractor count");
     NB_CHECK(max_depth > min_depth, "max_depth must exceed min_depth");
     const long long npix = (long long)B * H * W;
@@ -494,11 +474,7 @@ int zoe_attractor_normed(cudaStream_t st, const __half* apre, int lda, int na, c
 }
 
 int zoe_clb_concat(cudaStream_t st, const __half* act, const float* rel, const __half* emb, int B, int h, int w, int H, int W, __half* A) {
-    if (rec_on(REC_AUX)) {
-        char line[160];
-        snprintf(line, sizeof(line), "zclb_concat,%d,%d,%d,%d,%d", B, h, w, H, W);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("zclb_concat", {{"B", B}, {"h", h}, {"w", w}, {"H", H}, {"W", W}});
     const long long total = (long long)B * H * W * 24;
     zoe_clb_concat_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(act, rel, emb, B, h, w, H, W, ac_scale(h, H), ac_scale(w, W), A);
     NB_LAUNCHED();
@@ -507,11 +483,7 @@ int zoe_clb_concat(cudaStream_t st, const __half* act, const float* rel, const _
 
 int zoe_clb_final(cudaStream_t st, const __half* g, int ldg, const float* w2, const float* b2, const float* bins, int B, int h, int w, int H,
                   int W, float* depth) {
-    if (rec_on(REC_AUX)) {
-        char line[160];
-        snprintf(line, sizeof(line), "zclb_final,%d,%d,%d,%d,%d,%d", B, h, w, H, W, ldg);
-        rec_append(line);
-    }
+    if (rec_on(REC_AUX)) rec_launch("zclb_final", {{"B", B}, {"h", h}, {"w", w}, {"H", H}, {"W", W}, {"ldg", ldg}});
     NB_CHECK(ldg >= 80, "hidden row stride too small");
     const long long npix = (long long)B * H * W;
     const long long blocks = cdiv64(npix, 8), cap = (long long)device_sm_count() * 8;

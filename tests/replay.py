@@ -1,0 +1,320 @@
+"""What the float64 kernel-replay modules (tests/test_gpu_kernel_replay*.py) share: the launch recorder's reader, the networks
+whose launches they record, the deduplication of recorded and synthetic configurations, guarded buffers, the error tally and
+the replay loop.
+
+A recorded line is `kind,name=value,...`, named where the library's host code writes it (include/nunif_b200.h), so a
+configuration here is the dict {name: value} of one line, in the order the line gives.
+"""
+import ctypes
+import math
+import time
+import zlib
+
+import torch
+
+from tests.util import log_metric
+from nunif_b200 import _lib, synth
+
+DEV = "cuda:0"
+SENTINEL = 0x7E5B              # an fp16 NaN payload: fp16 guards keep exactly this bit pattern
+SENTINEL32 = 0x7FC05B5B        # an fp32 NaN payload: fp32 guards keep exactly this bit pattern
+GUARD = 4096                   # guard elements before and after every buffer
+# the host code's choices for a launch (gemm's tile width, K step and grid, the conv kinds' kernel path): recorded, but not
+# part of what identifies a configuration
+HOST_CHOICES = ("block_n", "bk", "grid", "path")
+
+
+# ------------------------------------------------------------------------------------------------------------ recorder
+def _num(v):
+    return int(v) if v.lstrip("-").isdigit() else float(v)
+
+
+def recorded(mask, fn):
+    """Run fn() with the recorder on for the kinds of `mask` (nb200_record_launches bits); -> [(kind, {name: value})] of its
+    launches."""
+    lib = _lib.lib()
+    _lib.check(lib.nb200_record_launches(mask))
+    try:
+        fn()
+        torch.cuda.synchronize()
+    finally:
+        lib.nb200_record_launches(0)
+    cap = 1 << 20
+    while True:
+        buf = ctypes.create_string_buffer(cap)
+        if lib.nb200_recorded_launches_named(buf, cap) == 0:
+            break
+        if b"buffer too small" not in lib.nb200_last_error():
+            _lib.check(1)
+        cap *= 4
+    recs = []
+    for line in buf.value.decode().splitlines():
+        kind, *fields = line.split(",")
+        recs.append((kind, {name: _num(v) for name, v in (f.split("=") for f in fields)}))
+    return recs
+
+
+def record_networks(mask, networks, unique=True):
+    """name -> [(kind, config)] of one forward of each (name, run) of `networks` under the recorder; with `unique`, each
+    recorded (kind, config) once, in the order first recorded."""
+    out = {}
+    for name, fn in networks:
+        t0 = time.time()
+        recs = recorded(mask, fn)
+        torch.cuda.empty_cache()
+        print(f"{name}: {len(recs)} launches recorded in {time.time() - t0:.1f} s")
+        if unique:
+            first = {}
+            for kind, r in recs:
+                first.setdefault((kind, tuple(r.items())), (kind, r))
+            recs = list(first.values())
+        out[name] = recs
+    return out
+
+
+def _key_fields(r):
+    return [f for f in r if f not in HOST_CHOICES]
+
+
+def configurations(production, kind, synthetic=()):
+    """-> [(network or "synthetic", config)] of `kind`: the recorded configurations, then the synthetic ones, each once.  A
+    configuration is identified by every field but the host's choices, in the order of the first one (a recorded one, when
+    any is), so a synthetic dict may list its fields in any order."""
+    configs = [(n, r) for n, recs in production.items() for k, r in recs if k == kind] + [("synthetic", r) for r in synthetic]
+    fields = _key_fields(configs[0][1]) if configs else []
+    seen, out = set(), []
+    for name, r in configs:
+        key = tuple(r[f] for f in fields)
+        if key not in seen:
+            seen.add(key)
+            out.append((name, r))
+    return out
+
+
+def _seed(*parts):
+    return zlib.crc32(repr(parts).encode())
+
+
+# ------------------------------------------------------------------------------------------------------------ networks
+def _gen(seed):
+    return torch.Generator().manual_seed(seed)
+
+
+def waifu2x(name, sd_fn, T=256, n=16, view=None, seed=1):
+    """One batch of n T x T tiles through the waifu2x model `name` (or its to_2x / to_1x view)."""
+    def run():
+        from nunif_b200.nunif.models import create_model
+        m = create_model(name, sd_fn(), DEV)
+        if view:
+            m = getattr(m, view)()
+        m(torch.rand(n, 3, T, T, generator=_gen(seed)).to(DEV))
+    return run
+
+
+def _depth_anything(encoder, v1=False):
+    def run():
+        from nunif_b200.iw3 import DepthAnythingNet
+        from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
+        h, w = preprocess_size(1080, 1920)
+        net = DepthAnythingNet(synth.depth_anything_v2_state_dict(0, encoder=encoder), DEV, encoder=encoder, v1=v1)
+        net(torch.randn(4, 3, h, w, generator=_gen(2)).to(DEV))
+    return run
+
+
+def _zoe_n():
+    from nunif_b200.iw3 import ZoeDepthNet
+    from nunif_b200.iw3.zoedepth_preprocess import preprocess_size
+    _, _, ph, pw, fh, fw = preprocess_size(2160, 3840)
+    ZoeDepthNet(synth.zoedepth_state_dict(0), DEV)(torch.randn(2, 3, fh + 2 * ph, fw + 2 * pw, generator=_gen(3)).clamp_(-1, 1).to(DEV))
+
+
+def zoe_any(kitti, model, seed):
+    """ZoeD_Any_N / ZoeD_Any_K on a 1080p landscape and a portrait frame."""
+    def run():
+        from nunif_b200.iw3 import ZoeDepthAnythingNet
+        from nunif_b200.iw3.zoedepth_preprocess import preprocess_size
+        net = ZoeDepthAnythingNet(synth.zoedepth_any_state_dict(0, None, kitti), DEV, model)
+        for H, W in ((1080, 1920), (1920, 1080)):
+            _, _, ph, pw, fh, fw = preprocess_size(H, W, h_height=392, v_height=518, ensure_multiple_of=14)
+            net(torch.randn(1, 3, fh + 2 * ph, fw + 2 * pw, generator=_gen(seed)).clamp_(-1, 1).to(DEV))
+    return run
+
+
+def _depth_input(B, h, w):
+    from oracle.row_flow import make_input
+    return make_input(synth.synth_depth(7, B, h, w), 2.5, 0.4).to(DEV)
+
+
+def _row_flow_v3():
+    from nunif_b200.iw3 import RowFlowV3
+    RowFlowV3(synth.row_flow_v3_state_dict(0), DEV)(_depth_input(1, 1080, 1920))
+
+
+def _mlbw(layers):
+    def run():
+        from nunif_b200.iw3 import MLBW
+        MLBW(synth.mlbw_state_dict(0, num_layers=layers), DEV)(_depth_input(1, 1080, 1920))
+    return run
+
+
+def _depth_aa():
+    from nunif_b200.iw3.depth_aa import DepthAA
+    from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
+    h, w = preprocess_size(1080, 1920)
+    DepthAA(synth.depth_aa_state_dict(0), DEV)(synth.synth_depth(8, 4, h, w).to(DEV))
+
+
+def _light_inpaint():
+    from nunif_b200.iw3 import LightInpaintV1
+    x = torch.rand(1, 3, 1080, 1920, generator=_gen(5)).to(DEV)
+    mask = (torch.rand(1, 1, 1080, 1920, generator=_gen(6)) < 0.05).float().to(DEV)
+    LightInpaintV1(synth.light_inpaint_v1_state_dict(0), DEV).infer(x, mask)
+
+
+def _transnet():
+    from nunif_b200.nunif.transnetv2 import TransNetV2
+    m = TransNetV2(synth.transnetv2_state_dict(0), DEV)
+    for B in (1, 8):
+        x = torch.stack([torch.from_numpy(synth.shot_sequence(900 + b, 100)).permute(0, 3, 1, 2).float() for b in range(B)])
+        m(x.to(DEV))
+
+
+def swin_sd(scale):
+    return lambda: synth.swin_unet_state_dict(0, scale)
+
+
+MODELS = [
+    ("swin_unet_4x", waifu2x("waifu2x.swin_unet_4x", swin_sd(4))),   # bench swin4x_4k: tile 256, batch 16
+    ("swin_unet_4x.to_2x", waifu2x("waifu2x.swin_unet_4x", swin_sd(4), view="to_2x")),   # bench swin2x_4k
+    ("swin_unet_2x", waifu2x("waifu2x.swin_unet_2x", swin_sd(2))),   # tiled_render default: tile 256, batch 16
+    ("swin_unet_1x", waifu2x("waifu2x.swin_unet_1x", swin_sd(1))),   # tiled_render default: tile 256, batch 16
+    ("upcunet", waifu2x("waifu2x.upcunet", synth.upcunet_state_dict)),      # bench upcunet: tile 256, batch 16
+    ("cunet", waifu2x("waifu2x.cunet", synth.cunet_state_dict)),            # tiled_render default: tile 256, batch 16
+    ("upconv_7", waifu2x("waifu2x.upconv_7", synth.upconv7_state_dict)),    # tiled_render default: tile 256, batch 16
+    ("vgg_7", waifu2x("waifu2x.vgg_7", synth.vgg7_state_dict)),             # tiled_render default: tile 256, batch 16
+    ("depth_anything_v2_s", _depth_anything("vits")),        # bench iw3_1080p: 1080p frames -> 392 x 686, B = 4
+    ("depth_anything_v2_b", _depth_anything("vitb")),        # iw3 Any_V2_B on the same 1080p batch
+    ("depth_anything_v2_l", _depth_anything("vitl")),        # iw3 Any_V2_L on the same 1080p batch
+    ("depth_anything_v1_s", _depth_anything("vits", True)),  # iw3 Any_S (V1) on the same 1080p batch
+    ("zoed_n", _zoe_n),                                      # bench iw3_4k_zoe: 4K frames -> 384 x 704, B = 2
+    ("zoed_any_n", zoe_any(False, "ZoeD_Any_N", 4)),         # iw3 default model: 1080p landscape (392 x 700) and portrait (v_height 518)
+    ("row_flow_v3", _row_flow_v3),                           # iw3 row_flow_v3 on a 1080p depth map
+    ("mlbw_l2", _mlbw(2)),                                   # iw3 mlbw_l2 on a 1080p depth map
+    ("mlbw_l4", _mlbw(4)),                                   # iw3 mlbw_l4 on a 1080p depth map
+    ("depth_aa", _depth_aa),                                 # iw3 depth_aa on the Depth-Anything output of a 1080p batch (392 x 686, B = 4)
+    ("light_inpaint_v1", _light_inpaint),                    # iw3 forward_inpaint on a 1080p frame
+    ("transnetv2", _transnet),                               # --scene-detect: 100-frame windows, one alone and 8 batched
+]
+
+
+# ------------------------------------------------------------------------------------------------------------ guarded buffers
+def guarded(n):
+    """fp16 buffer of GUARD + n + GUARD elements, all SENTINEL."""
+    return torch.full((n + 2 * GUARD,), SENTINEL, dtype=torch.int16, device=DEV).view(torch.float16)
+
+
+def guarded32(n):
+    """fp32 buffer of GUARD + n + GUARD elements, all SENTINEL32."""
+    return torch.full((n + 2 * GUARD,), SENTINEL32, dtype=torch.int32, device=DEV).view(torch.float32)
+
+
+def body(buf, n):
+    """The n elements between the guards (a view whose data_ptr is what the kernel gets)."""
+    return buf[GUARD:GUARD + n]
+
+
+def guards_ok(buf, n):
+    if buf.dtype == torch.float16:
+        b, s = bits(buf), SENTINEL
+    else:
+        b, s = buf.view(torch.int32), SENTINEL32
+    return bool((b[:GUARD] == s).all() and (b[GUARD + n:] == s).all())
+
+
+def bits(t):
+    return t.view(torch.int16)
+
+
+def view(buf, shape, strides, offset=0):
+    return buf.as_strided(shape, strides, GUARD + offset)
+
+
+def extent(shape, strides, offset=0):
+    return offset + sum((s - 1) * st for s, st in zip(shape, strides)) + 1
+
+
+# ------------------------------------------------------------------------------------------------------------ error bounds
+def ulp16(x):
+    """fp16 spacing at |x| (float64), floored at 2^-24 (the subnormal spacing)."""
+    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14)))
+    return torch.exp2(e - 10).clamp_min(2.0 ** -24)
+
+
+def rounded(v, E):
+    """An fp16 rounding point: the kernel rounds a value within E of the float64 v.  Rounding is monotone, so its result lies
+    between the roundings of v - E and v + E: -> (v rounded, bound on |kernel's rounded value - v rounded|).  The bound is 0
+    wherever no rounding boundary lies within E, so only those few elements carry an error forward."""
+    r = v.half().double()
+    return r, torch.maximum((v + E).half().double() - r, r - (v - E).half().double())
+
+
+def round16_bound(ref, E):
+    """Bound on |fp16(v) - ref| for a value v the kernel computes within E of ref: half an fp16 ulp at |ref| + E, plus E."""
+    return 0.5 * ulp16(ref.abs() + E) + E
+
+
+class Tally:
+    """Worst err / bound, elements over their bound, and the other problems of one replayed configuration."""
+
+    def __init__(self):
+        self.worst, self.over, self.bad = 0.0, 0, []
+
+    def add(self, got, ref, bound):
+        ratio = torch.nan_to_num((got.double() - ref).abs() / bound, nan=math.inf)
+        self.worst = max(self.worst, float(ratio.max()))
+        self.over += int((ratio > 1).sum())
+
+    def exact(self, what, got, want):
+        """Bit-identical (int views of the same dtype)."""
+        if not torch.equal(got, want):
+            self.bad.append(f"{what}: {int((got != want).sum())} elements differ")
+
+    def guards(self, what, buf, n):
+        if not guards_ok(buf, n):
+            self.bad.append(f"{what}: guard changed")
+
+    def no_nan(self, what, t):
+        if bool(torch.isnan(t).any()):
+            self.bad.append(f"NaN in {what}")
+
+    def result(self):
+        return self.worst, self.over, self.bad
+
+
+# ------------------------------------------------------------------------------------------------------------ replay
+def replay(kind, cases, check, variant=None):
+    """Replay each configuration of `cases` (configurations()) through check(r, seed) -> Tally.result(), or, with variant =
+    (name, values), through check(r, seed, value) for each value.  Logs each result and the summary, and fails if any
+    configuration has a problem or an element over its bound.  The seed is _seed(network, kind, configuration key)."""
+    values = variant[1] if variant else (None,)
+    fields = _key_fields(cases[0][1])
+    t0, worst, fails = time.time(), 0.0, []
+    for name, r in cases:
+        key = tuple(r[f] for f in fields)
+        cfg = ",".join(f"{f}={v}" for f, v in zip(fields, key))
+        for value in values:
+            extra = {variant[0]: int(value)} if variant else {}
+            ratio, over, bad = check(r, _seed(name, kind, key), *((value,) if variant else ()))
+            log_metric(f"replay_{kind}", model=name, cfg=cfg, **extra, err_over_bound=f"{ratio:.3g}")
+            worst = max(worst, ratio)
+            if bad or over:
+                fails.append(f"{name} {cfg} {extra}: {bad} max err/bound {ratio:.3g}, {over} elements over")
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+    n_prod = sum(1 for n, _ in cases if n != "synthetic")
+    count = {f"{variant[0]}s": len(values)} if variant else {}
+    times = "".join(f" x {n} {k}" for k, n in count.items())
+    print(f"\n{kind}: {len(cases)} configurations ({n_prod} recorded, {len(cases) - n_prod} synthetic){times}, worst err/bound "
+          f"{worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
+    log_metric(f"replay_{kind}_summary", configs=len(cases), **count, worst=worst)
+    assert not fails, "\n".join(fails[:20])

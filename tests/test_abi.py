@@ -122,3 +122,21 @@ def test_launch_recorder_mask_bits_0_to_2(lib):
         assert b"unknown recorder bits" in lib.nb200_last_error()
     buf = ctypes.create_string_buffer(16)
     assert lib.nb200_recorded_launches(buf, 16) == 0 and buf.value == b""
+
+
+def test_launch_recorder_names_each_field(lib):
+    """A recorded line is `kind,name=value,...` with the names the replay tests read, and nb200_recorded_launches returns
+    the same values without the names.  zoe_expand_rel_bias records its launch before it checks ldb, so a call with dummy
+    host pointers and ldb < ph * pw + 1 is refused without touching the device and still leaves its line: no GPU needed."""
+    dummy = ctypes.create_string_buffer(64)
+    assert lib.nb200_record_launches(2) == 0
+    try:
+        assert lib.nb200_zoe_expand_rel_bias_f32(dummy, 3, 5, 4, dummy, 10, None) != 0
+        assert b"bias row stride too small" in lib.nb200_last_error()
+    finally:
+        lib.nb200_record_launches(0)
+    buf = ctypes.create_string_buffer(256)
+    assert lib.nb200_recorded_launches_named(buf, 256) == 0
+    assert buf.value == b"zrelbias,ph=3,pw=5,heads=4,ldb=10\n"
+    assert lib.nb200_recorded_launches(buf, 256) == 0
+    assert buf.value == b"zrelbias,3,5,4,10\n"

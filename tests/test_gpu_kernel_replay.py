@@ -13,211 +13,37 @@ MODELS.  Each unique recorded configuration is then replayed through a low-level
 """
 import ctypes
 import math
-import time
-import zlib
 
 import pytest
 import torch
 import torch.nn.functional as F
 
 from tests.util import log_metric
-from nunif_b200 import _lib, synth
+from tests.replay import (DEV, GUARD, MODELS, Tally, bits, body, configurations, extent, guarded, record_networks, recorded, replay,
+                          rounded, ulp16, view)
+from nunif_b200 import _lib
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 LOG2E = math.log2(math.e)
-SENTINEL = 0x7E5B            # an fp16 NaN payload: guards keep exactly this bit pattern
-GUARD = 4096                 # guard elements before and after every buffer
 CHUNK_BYTES = 2 << 30        # float64 working set of one reference chunk
-
-GEMM_FIELDS = ("kind pad dil B Hi Wi Ci Cin a_row_stride a_img_stride a_planes a_plane_stride N act ldo out_mode cout "
-               "split_stride has_bias has_res ldr res_H res_W res_cy res_cx res_before_act has_a2 Cin2 ld2 out_is_res out_is_a "
-               "block_n bk grid").split()
-FIELDS = {"gemm": GEMM_FIELDS, "attn": "B N heads has_bias ldb".split(), "swin_attn": "B H W C shift".split(),
-          "swin_mlp": "T C proj cs".split()}
+REC_GEMMS = 1                # nb200_record_launches bit of the kinds replayed here
+KINDS = ("gemm", "attn", "swin_attn", "swin_mlp")
 DESC_FIELDS = [f for f, _ in _lib.GemmDesc._fields_]
-# what identifies a GEMM launch (the last three fields are the host code's choices for it)
-GEMM_KEY = [f for f in GEMM_FIELDS if f not in ("block_n", "bk", "grid")]
 # every instantiation gemm.cu launch_bn can select: (BLOCK_N, BK, A2)
 INSTANTIATIONS = {(bn, bk, 0) for bn in (16, 32, 48, 64, 96, 128) for bk in (32, 64)} | {(bn, bk, 1) for bn in (64, 96) for bk in (32, 64)}
-
-
-# ------------------------------------------------------------------------------------------------------------ recorder
-def read_records():
-    lib = _lib.lib()
-    cap = 1 << 20
-    while True:
-        buf = ctypes.create_string_buffer(cap)
-        if lib.nb200_recorded_launches(buf, cap) == 0:
-            break
-        if b"buffer too small" not in lib.nb200_last_error():
-            _lib.check(1)
-        cap *= 4
-    recs = []
-    for line in buf.value.decode().splitlines():
-        kind, *vals = line.split(",")
-        assert len(vals) == len(FIELDS[kind]), line
-        recs.append((kind, dict(zip(FIELDS[kind], (int(v) for v in vals)))))
-    return recs
-
-
-def recorded(fn):
-    """Run fn() with the recorder on; -> its records."""
-    lib = _lib.lib()
-    _lib.check(lib.nb200_record_launches(1))
-    try:
-        fn()
-        torch.cuda.synchronize()
-    finally:
-        lib.nb200_record_launches(0)
-    return read_records()
-
-
-# ------------------------------------------------------------------------------------------------------------ networks
-def _gen(seed):
-    return torch.Generator().manual_seed(seed)
-
-
-def _waifu2x(name, sd_fn, to_2x=False):
-    def run():
-        from nunif_b200.nunif.models import create_model
-        m = create_model(name, sd_fn(), DEV)
-        if to_2x:
-            m = m.to_2x()
-        m(torch.rand(16, 3, 256, 256, generator=_gen(1)).to(DEV))
-    return run
-
-
-def _depth_anything(encoder, v1=False):
-    def run():
-        from nunif_b200.iw3 import DepthAnythingNet
-        from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
-        h, w = preprocess_size(1080, 1920)
-        net = DepthAnythingNet(synth.depth_anything_v2_state_dict(0, encoder=encoder), DEV, encoder=encoder, v1=v1)
-        net(torch.randn(4, 3, h, w, generator=_gen(2)).to(DEV))
-    return run
-
-
-def _zoe_n():
-    from nunif_b200.iw3 import ZoeDepthNet
-    from nunif_b200.iw3.zoedepth_preprocess import preprocess_size
-    _, _, ph, pw, fh, fw = preprocess_size(2160, 3840)
-    ZoeDepthNet(synth.zoedepth_state_dict(0), DEV)(torch.randn(2, 3, fh + 2 * ph, fw + 2 * pw, generator=_gen(3)).clamp_(-1, 1).to(DEV))
-
-
-def _zoe_any_n():
-    from nunif_b200.iw3 import ZoeDepthAnythingNet
-    from nunif_b200.iw3.zoedepth_preprocess import preprocess_size
-    net = ZoeDepthAnythingNet(synth.zoedepth_any_state_dict(0, None, False), DEV, "ZoeD_Any_N")
-    for H, W in ((1080, 1920), (1920, 1080)):
-        _, _, ph, pw, fh, fw = preprocess_size(H, W, h_height=392, v_height=518, ensure_multiple_of=14)
-        net(torch.randn(1, 3, fh + 2 * ph, fw + 2 * pw, generator=_gen(4)).clamp_(-1, 1).to(DEV))
-
-
-def _depth_input(B, h, w):
-    from oracle.row_flow import make_input
-    return make_input(synth.synth_depth(7, B, h, w), 2.5, 0.4).to(DEV)
-
-
-def _row_flow_v3():
-    from nunif_b200.iw3 import RowFlowV3
-    RowFlowV3(synth.row_flow_v3_state_dict(0), DEV)(_depth_input(1, 1080, 1920))
-
-
-def _mlbw(layers):
-    def run():
-        from nunif_b200.iw3 import MLBW
-        MLBW(synth.mlbw_state_dict(0, num_layers=layers), DEV)(_depth_input(1, 1080, 1920))
-    return run
-
-
-def _depth_aa():
-    from nunif_b200.iw3.depth_aa import DepthAA
-    from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
-    h, w = preprocess_size(1080, 1920)
-    DepthAA(synth.depth_aa_state_dict(0), DEV)(synth.synth_depth(8, 4, h, w).to(DEV))
-
-
-def _light_inpaint():
-    from nunif_b200.iw3 import LightInpaintV1
-    x = torch.rand(1, 3, 1080, 1920, generator=_gen(5)).to(DEV)
-    mask = (torch.rand(1, 1, 1080, 1920, generator=_gen(6)) < 0.05).float().to(DEV)
-    LightInpaintV1(synth.light_inpaint_v1_state_dict(0), DEV).infer(x, mask)
-
-
-def _transnet():
-    from nunif_b200.nunif.transnetv2 import TransNetV2
-    m = TransNetV2(synth.transnetv2_state_dict(0), DEV)
-    for B in (1, 8):
-        x = torch.stack([torch.from_numpy(synth.shot_sequence(900 + b, 100)).permute(0, 3, 1, 2).float() for b in range(B)])
-        m(x.to(DEV))
-
-
-MODELS = [
-    ("swin_unet_4x", _waifu2x("waifu2x.swin_unet_4x", lambda: synth.swin_unet_state_dict(0, 4))),   # bench swin4x_4k: tile 256, batch 16
-    ("swin_unet_4x.to_2x", _waifu2x("waifu2x.swin_unet_4x", lambda: synth.swin_unet_state_dict(0, 4), True)),   # bench swin2x_4k
-    ("swin_unet_2x", _waifu2x("waifu2x.swin_unet_2x", lambda: synth.swin_unet_state_dict(0, 2))),   # tiled_render default: tile 256, batch 16
-    ("swin_unet_1x", _waifu2x("waifu2x.swin_unet_1x", lambda: synth.swin_unet_state_dict(0, 1))),   # tiled_render default: tile 256, batch 16
-    ("upcunet", _waifu2x("waifu2x.upcunet", synth.upcunet_state_dict)),      # bench upcunet: tile 256, batch 16
-    ("cunet", _waifu2x("waifu2x.cunet", synth.cunet_state_dict)),            # tiled_render default: tile 256, batch 16
-    ("upconv_7", _waifu2x("waifu2x.upconv_7", synth.upconv7_state_dict)),    # tiled_render default: tile 256, batch 16
-    ("vgg_7", _waifu2x("waifu2x.vgg_7", synth.vgg7_state_dict)),             # tiled_render default: tile 256, batch 16
-    ("depth_anything_v2_s", _depth_anything("vits")),        # bench iw3_1080p: 1080p frames -> 392 x 686, B = 4
-    ("depth_anything_v2_b", _depth_anything("vitb")),        # iw3 Any_V2_B on the same 1080p batch
-    ("depth_anything_v2_l", _depth_anything("vitl")),        # iw3 Any_V2_L on the same 1080p batch
-    ("depth_anything_v1_s", _depth_anything("vits", True)),  # iw3 Any_S (V1) on the same 1080p batch
-    ("zoed_n", _zoe_n),                                      # bench iw3_4k_zoe: 4K frames -> 384 x 704, B = 2
-    ("zoed_any_n", _zoe_any_n),                              # iw3 default model: 1080p landscape (392 x 700) and portrait (v_height 518)
-    ("row_flow_v3", _row_flow_v3),                           # iw3 row_flow_v3 on a 1080p depth map
-    ("mlbw_l2", _mlbw(2)),                                   # iw3 mlbw_l2 on a 1080p depth map
-    ("mlbw_l4", _mlbw(4)),                                   # iw3 mlbw_l4 on a 1080p depth map
-    ("depth_aa", _depth_aa),                                 # iw3 depth_aa on the Depth-Anything output of a 1080p batch (392 x 686, B = 4)
-    ("light_inpaint_v1", _light_inpaint),                    # iw3 forward_inpaint on a 1080p frame
-    ("transnetv2", _transnet),                               # --scene-detect: 100-frame windows, one alone and 8 batched
-]
 
 
 @pytest.fixture(scope="module")
 def production():
     """name -> unique records (kind, config) of one forward of each network of MODELS."""
-    out = {}
-    for name, fn in MODELS:
-        t0 = time.time()
-        recs = recorded(fn)
-        torch.cuda.empty_cache()
-        print(f"{name}: {len(recs)} launches recorded in {time.time() - t0:.1f} s")
-        uniq = []
-        for kind, r in recs:
-            key = (kind, tuple(r.items()))
-            if key not in uniq:
-                uniq.append(key)
-        out[name] = [(k, dict(r)) for k, r in uniq]
-    return out
-
-
-def _unique(production, kind, extra=()):
-    seen, cases = set(), []
-    for name, recs in production.items():
-        for k, r in recs:
-            if k != kind:
-                continue
-            key = tuple(r[f] for f in (GEMM_KEY if kind == "gemm" else FIELDS[kind]))
-            if key not in seen:
-                seen.add(key)
-                cases.append((name, r))
-    for r in extra:
-        key = tuple(r[f] for f in (GEMM_KEY if kind == "gemm" else FIELDS[kind]))
-        if key not in seen:
-            seen.add(key)
-            cases.append(("synthetic", r))
-    return cases
+    return record_networks(REC_GEMMS, MODELS)
 
 
 def test_every_network_records_its_launches(production):
     lines = []
     for name, _ in MODELS:
         recs = production[name]
-        counts = {k: sum(1 for kk, _ in recs if kk == k) for k in FIELDS}
+        counts = {k: sum(1 for kk, _ in recs if kk == k) for k in KINDS}
         inst = sorted({(r["block_n"], r["bk"], r["has_a2"]) for k, r in recs if k == "gemm"})
         lines.append(f"{name:22s} unique: gemm {counts['gemm']:3d} attn {counts['attn']:2d} swin_attn {counts['swin_attn']:2d} "
                      f"swin_mlp {counts['swin_mlp']:2d}   (BLOCK_N, BK, A2): {inst}")
@@ -231,31 +57,8 @@ def test_every_network_records_its_launches(production):
 
 
 # ------------------------------------------------------------------------------------------------------------ helpers
-def ulp16(x):
-    """fp16 spacing at |x| (float64), floored at 2^-24 (the subnormal spacing)."""
-    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14)))
-    return torch.exp2(e - 10).clamp_min(2.0 ** -24)
-
-
-def guarded(n):
-    """fp16 buffer of GUARD + n + GUARD elements, all SENTINEL."""
-    return torch.full((n + 2 * GUARD,), SENTINEL, dtype=torch.int16, device=DEV).view(torch.float16)
-
-
-def view(buf, shape, strides, offset=0):
-    return buf.as_strided(shape, strides, GUARD + offset)
-
-
-def extent(shape, strides, offset=0):
-    return offset + sum((s - 1) * st for s, st in zip(shape, strides)) + 1
-
-
 def fill_normal(v, g, std=1.0):
     v.copy_((torch.randn(v.shape, generator=g, device=DEV) * std).to(v.dtype))
-
-
-def bits(t):
-    return t.view(torch.int16)
 
 
 def gelu64(x):
@@ -267,8 +70,9 @@ ACT = {0: lambda v: v, 1: lambda v: torch.where(v > 0, v, 0.1 * v), 2: gelu64, 3
 
 # ------------------------------------------------------------------------------------------------------------ GEMM replay
 def _gemm_cfg(**kw):
-    r = dict.fromkeys(GEMM_FIELDS, 0)
-    r.update(dil=1, a_planes=1, has_bias=1)
+    """A launch's ConvGemm fields (nb200_gemm_desc) and its recorded flags; what is not given is 0 (dil, a_planes 1, a bias)."""
+    r = dict.fromkeys(DESC_FIELDS, 0)
+    r.update(dil=1, a_planes=1, has_bias=1, has_res=0, has_a2=0, out_is_res=0, out_is_a=0)
     r.update(kw)
     return r
 
@@ -389,9 +193,8 @@ class GemmCase:
                                                      p(self.res), p(self.a2), _lib.stream_ptr()))
         torch.cuda.synchronize()
 
-    def check_guards(self):
-        """-> list of problems: NaN in the output view, guard / unviewed elements changed."""
-        bad = []
+    def check_guards(self, tally):
+        """Problems: NaN in the output view, guard / unviewed elements changed."""
         written = torch.zeros(self.out.numel(), dtype=torch.bool, device=DEV)
         view(written, self.o_shape, self.o_strides).fill_(True)
         for buf in {id(x): x for x in (self.a, self.out, self.res, self.a2) if x is not None}.values():
@@ -399,10 +202,8 @@ class GemmCase:
             changed = (bits(buf) != bits(self.snap[id(buf)])) & keep
             if bool(changed.any()):
                 i = int(changed.nonzero()[0]) - GUARD
-                bad.append(f"element {i} outside the written view changed (buffer of {buf.numel() - 2 * GUARD})")
-        if bool(torch.isnan(view(self.out, self.o_shape, self.o_strides)).any()):
-            bad.append("NaN in the output")
-        return bad
+                tally.bad.append(f"element {i} outside the written view changed (buffer of {buf.numel() - 2 * GUARD})")
+        tally.no_nan("the output", view(self.out, self.o_shape, self.o_strides))
 
     def _tap_slices(self, a16, y0, y1):
         """(float64 [rows, Cin] slice, first K column) per tap for output rows [y0, y1) of the images in a16."""
@@ -473,14 +274,13 @@ class GemmCase:
                 shp = (1, y1 - y0, self.Wo, N)
                 yield (slice(b, b + 1), slice(y0, y1), slice(None)), acc.view(shp), sab.view(shp)
 
-    def check(self):
-        """-> (largest |err| / bound, number of elements over the bound)."""
+    def check(self, tally):
+        """Every output element against the float64 reference."""
         r = self.r
         act = r["act"]
         L = 1.13 if act == 2 else 1.0
         got_all = view(self.out, self.o_shape, self.o_strides)
         res_all = self.res_ref if self.res is not None else None
-        worst, over = 0.0, 0
         for idx, acc, sab in self.reference_chunks():
             v = acc + (self.bias.double() if self.bias is not None else 0.0)
             if res_all is not None:
@@ -488,16 +288,16 @@ class GemmCase:
                 v = ACT[act](v + rv) if r["res_before_act"] else ACT[act](v) + rv
             else:
                 v = ACT[act](v)
-            got = got_all[idx].double().reshape(v.shape)
-            bound = ulp16(v) + 2.0 ** -20 * L * sab + (1e-6 if act == 2 else 0.0)
-            ratio = (got - v).abs() / bound
-            worst = max(worst, float(ratio.max()))
-            over += int((ratio > 1).sum())
-        return worst, over
+            tally.add(got_all[idx].reshape(v.shape), v, ulp16(v) + 2.0 ** -20 * L * sab + (1e-6 if act == 2 else 0.0))
 
 
-def _seed(*parts):
-    return zlib.crc32(repr(parts).encode())
+def gemm_check(r, seed):
+    case = GemmCase(r, seed)
+    case.launch()
+    tally = Tally()
+    case.check_guards(tally)
+    case.check(tally)
+    return tally.result()
 
 
 def test_gemm_instantiation_coverage(production):
@@ -506,7 +306,7 @@ def test_gemm_instantiation_coverage(production):
     rows = []
     for r in _synthetic_gemm():
         case = GemmCase(r, 1)
-        recs = recorded(case.launch)
+        recs = recorded(REC_GEMMS, case.launch)
         rows.append((recs[0][1]["block_n"], recs[0][1]["bk"], recs[0][1]["has_a2"]))
     table = {i: ("recorded" if i in have else ("synthetic" if i in rows else "MISSING")) for i in sorted(INSTANTIATIONS)}
     print("\n" + "\n".join(f"BLOCK_N {bn:3d} BK {bk} A2 {a2}: {src}" for (bn, bk, a2), src in table.items()))
@@ -515,23 +315,7 @@ def test_gemm_instantiation_coverage(production):
 
 
 def test_gemm_replay(production):
-    cases = _unique(production, "gemm", _synthetic_gemm())
-    t0, worst, fails = time.time(), 0.0, []
-    for name, r in cases:
-        case = GemmCase(r, _seed(name, tuple(r[f] for f in GEMM_KEY)))
-        case.launch()
-        bad = case.check_guards()
-        ratio, over = case.check()
-        del case
-        cfg = ",".join(f"{f}={r[f]}" for f in GEMM_KEY if r[f])
-        log_metric("replay_gemm", model=name, cfg=cfg, err_over_bound=f"{ratio:.3g}")
-        worst = max(worst, ratio)
-        if bad or over:
-            fails.append(f"{name} {cfg}: {bad} max err/bound {ratio:.3g}, {over} elements over")
-    torch.cuda.empty_cache()
-    print(f"\ngemm: {len(cases)} configurations, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
-    log_metric("replay_gemm_summary", configs=len(cases), worst=worst)
-    assert not fails, "\n".join(fails[:20])
+    replay("gemm", configurations(production, "gemm", _synthetic_gemm()), gemm_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ flash attention
@@ -581,7 +365,7 @@ def attention_case(r, needle, seed):
     return qkv.half().to(DEV), bias, targets
 
 
-def attention_check(r, needle, seed):
+def attention_check(r, seed, needle):
     """Bound per element: 2^-9 sum_j p_j |v_j| covers the fp16 rounding of P before PV (2^-11 relative), its mismatch with
     the fp32 row sum and ex2.approx.  Where P is below 2^-14 its fp16 value is subnormal and the rounding is absolute, up to
     2^-25 of the running maximum (which is 1 before the row sum l >= 1 divides): 2^-25 sum_j |v_j| / l = 2^-25 max_j p_j
@@ -593,13 +377,10 @@ def attention_check(r, needle, seed):
     _lib.check(_lib.lib().nb200_flash_attention_f16(_lib.ptr(qkv), ctypes.c_void_p(out.data_ptr() + 2 * GUARD), B, N, H,
                                                     _lib.ptr(bias), ldb, _lib.stream_ptr()))
     torch.cuda.synchronize()
-    bad = []
+    tally = Tally()
     got = view(out, (B, N, H, 64), (N * dim, dim, 64, 1))
-    if bool(torch.isnan(got).any()):
-        bad.append("NaN in the output")
-    if not bool((bits(out[:GUARD]) == SENTINEL).all() and (bits(out[GUARD + B * N * dim:]) == SENTINEL).all()):
-        bad.append("guard rows changed")
-    worst, over = 0.0, 0
+    tally.no_nan("the output", got)
+    tally.guards("output", out, B * N * dim)
     for b in range(B):
         q, k, v = (qkv[b, :, i].double().permute(1, 0, 2) for i in range(3))   # [H][N][64]
         s = q @ k.transpose(1, 2) / 8.0
@@ -611,26 +392,12 @@ def attention_check(r, needle, seed):
             assert float(mass.min()) >= 0.9, float(mass.min())
         ref = p @ v
         bound = 2.0 ** -9 * (p @ v.abs()) + 2.0 ** -25 * p.amax(-1, keepdim=True) * v.abs().sum(1, keepdim=True) + ulp16(ref)
-        ratio = (got[b].double().permute(1, 0, 2) - ref).abs() / bound
-        worst = max(worst, float(ratio.max()))
-        over += int((ratio > 1).sum())
-    return worst, over, bad
+        tally.add(got[b].permute(1, 0, 2), ref, bound)
+    return tally.result()
 
 
 def test_flash_attention_replay(production):
-    cases = _unique(production, "attn", SYNTH_ATTN)
-    t0, worst, fails = time.time(), 0.0, []
-    for name, r in cases:
-        for needle in (False, True):
-            ratio, over, bad = attention_check(r, needle, _seed(name, tuple(r.values()), needle))
-            cfg = ",".join(f"{f}={r[f]}" for f in FIELDS["attn"])
-            log_metric("replay_attn", model=name, cfg=cfg, needle=int(needle), err_over_bound=f"{ratio:.3g}")
-            worst = max(worst, ratio)
-            if bad or over:
-                fails.append(f"{name} {cfg} needle={needle}: {bad} max err/bound {ratio:.3g}, {over} elements over")
-    print(f"\nattention: {len(cases)} configurations x 2 inputs, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
-    log_metric("replay_attn_summary", configs=len(cases), worst=worst)
-    assert not fails, "\n".join(fails[:20])
+    replay("attn", configurations(production, "attn", SYNTH_ATTN), attention_check, variant=("needle", (False, True)))
 
 
 # ------------------------------------------------------------------------------------------------------------ Swin head
@@ -698,15 +465,11 @@ def swin_attn_check(r, seed):
     _lib.check(_lib.lib().nb200_swin_attn_fused_f16(_lib.ptr(x), _lib.ptr(wqkv), _lib.ptr(bqkv), _lib.ptr(table),
                                                     ctypes.c_void_p(att.data_ptr() + 2 * GUARD), B, H, W, C, shift, _lib.stream_ptr()))
     torch.cuda.synchronize()
-    bad = []
-    got = att[GUARD:GUARD + n].view(B, H, W, C)
-    if bool(torch.isnan(got).any()):
-        bad.append("NaN in the output")
-    if not bool((bits(att[:GUARD]) == SENTINEL).all() and (bits(att[GUARD + n:]) == SENTINEL).all()):
-        bad.append("guard changed")
-    if not torch.equal(bits(x), bits(x0)):
-        bad.append("x changed")
-    worst, over = 0.0, 0
+    tally = Tally()
+    got = body(att, n).view(B, H, W, C)
+    tally.no_nan("the output", got)
+    tally.guards("output", att, n)
+    tally.exact("x", bits(x), bits(x0))
     for b in range(B):
         # q|k|v are rounded to fp16 after the bias, as the kernel stores them; before that the kernel's fp32 GEMM is within
         # 2^-20 sum|x w| (+ the bias add) of the float64 one
@@ -716,39 +479,18 @@ def swin_attn_check(r, seed):
         ref, spv, sub, eprop = window_attention64(qkv, table.double(), C, shift, eqkv)
         # fp16 P, its fp32 row sum and ex2.approx as in the ViT attention; plus the q|k|v rounding differences
         bound = ulp16(ref) + 2.0 ** -9 * spv + 2.0 ** -25 * sub + eprop
-        ratio = (got[b:b + 1].double() - ref).abs() / bound
-        worst = max(worst, float(ratio.max()))
-        over += int((ratio > 1).sum())
-    return worst, over, bad
+        tally.add(got[b:b + 1], ref, bound)
+    return tally.result()
 
 
 def test_swin_attn_replay(production):
-    cases = _unique(production, "swin_attn", SYNTH_SWIN_ATTN)
-    t0, worst, fails = time.time(), 0.0, []
-    for name, r in cases:
-        ratio, over, bad = swin_attn_check(r, _seed(name, tuple(r.values())))
-        cfg = ",".join(f"{f}={r[f]}" for f in FIELDS["swin_attn"])
-        log_metric("replay_swin_attn", model=name, cfg=cfg, err_over_bound=f"{ratio:.3g}")
-        worst = max(worst, ratio)
-        if bad or over:
-            fails.append(f"{name} {cfg}: {bad} max err/bound {ratio:.3g}, {over} elements over")
-    print(f"\nswin head: {len(cases)} configurations, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
-    log_metric("replay_swin_attn_summary", configs=len(cases), worst=worst)
-    assert not fails, "\n".join(fails[:20])
+    replay("swin_attn", configurations(production, "swin_attn", SYNTH_SWIN_ATTN), swin_attn_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ Swin tail
 SYNTH_SWIN_MLP = [dict(T=16 * 240 * 240, C=192, proj=1, cs=48),      # the 4x model's last block at tile 256, batch 16
                   dict(T=148 * 128 * 3 + 55, C=192, proj=1, cs=48), dict(T=148 * 128 * 2 + 1, C=96, proj=1, cs=16),
                   dict(T=148 * 128 + 127, C=192, proj=1, cs=0), dict(T=777, C=96, proj=0, cs=0)]
-
-
-def rounded(v, E):
-    """An fp16 rounding point: the kernel rounds a value within E of the float64 v.  Rounding is monotone, so its result lies
-    between the roundings of v - E and v + E: -> (v rounded, bound on |kernel's rounded value - v rounded|).  The bound is 0
-    wherever no rounding boundary lies within E, so only those few elements carry an error forward."""
-    r = v.half().double()
-    return r, torch.maximum((v + E).half().double() - r, r - (v - E).half().double())
 
 
 def mlp_reference(x, att, wp, bp, w1, b1, w2, b2, wy, by):
@@ -809,35 +551,19 @@ def swin_mlp_check(r, seed):
                                                 _lib.ptr(w2), _lib.ptr(b2), _lib.stream_ptr()))
         outb, width, x_in = xb, C, x0[GUARD:GUARD + T * C].view(T, C)
     torch.cuda.synchronize()
-    bad = []
-    got = outb[GUARD:GUARD + T * width].view(T, width)
-    if bool(torch.isnan(got).any()):
-        bad.append("NaN in the output")
-    if not bool((bits(outb[:GUARD]) == SENTINEL).all() and (bits(outb[GUARD + T * width:]) == SENTINEL).all()):
-        bad.append("guard changed")
-    if cs and not torch.equal(bits(xb), bits(x0)):
-        bad.append("x changed although y was requested")
-    worst, over = 0.0, 0
+    tally = Tally()
+    got = body(outb, T * width).view(T, width)
+    tally.no_nan("the output", got)
+    tally.guards("output", outb, T * width)
+    if cs:
+        tally.exact("x although y was requested", bits(xb), bits(x0))
     rows = 1 << 16
     for t0 in range(0, T, rows):
         t1 = min(T, t0 + rows)
         ref, bound = mlp_reference(x_in[t0:t1], att[t0:t1] if proj else None, wp, bp, w1, b1, w2, b2, wy, by)
-        ratio = (got[t0:t1].double() - ref).abs() / bound
-        worst = max(worst, float(ratio.max()))
-        over += int((ratio > 1).sum())
-    return worst, over, bad
+        tally.add(got[t0:t1], ref, bound)
+    return tally.result()
 
 
 def test_swin_mlp_replay(production):
-    cases = _unique(production, "swin_mlp", SYNTH_SWIN_MLP)
-    t0, worst, fails = time.time(), 0.0, []
-    for name, r in cases:
-        ratio, over, bad = swin_mlp_check(r, _seed(name, tuple(r.values())))
-        cfg = ",".join(f"{f}={r[f]}" for f in FIELDS["swin_mlp"])
-        log_metric("replay_swin_mlp", model=name, cfg=cfg, err_over_bound=f"{ratio:.3g}")
-        worst = max(worst, ratio)
-        if bad or over:
-            fails.append(f"{name} {cfg}: {bad} max err/bound {ratio:.3g}, {over} elements over")
-    print(f"\nswin tail: {len(cases)} configurations, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
-    log_metric("replay_swin_mlp_summary", configs=len(cases), worst=worst)
-    assert not fails, "\n".join(fails[:20])
+    replay("swin_mlp", configurations(production, "swin_mlp", SYNTH_SWIN_MLP), swin_mlp_check)

@@ -4,7 +4,7 @@ ViT residual add + LayerNorm and the DPT head's bilinear upsample (Depth-Anythin
 (softplus / normed seed, attractors with the bitonic sort, the ConditionalLogBinomial concat and mixture, the BEiT relative
 position bias expansion).
 
-The discipline of tests/test_gpu_kernel_replay.py, whose guard helpers are reused: a module fixture turns on bit 1 of the
+The discipline of tests/test_gpu_kernel_replay.py, with the helpers of tests/replay.py: a module fixture turns on bit 1 of the
 launch recorder (the kinds between the GEMMs; bit 0 keeps the GEMM replay's kinds) and records one forward of each network of
 AUX_MODELS, and each unique configuration (plus a synthetic list that reaches the edges production
 does not) is replayed through the kernel's test entry point on fresh seeded data.  Inputs outside the view a launch reads are
@@ -13,115 +13,51 @@ output element is checked against a float64 reference written from the reference
 oracle/depth_anything.py, oracle/zoedepth*.py, ATen's align_corners=True index arithmetic), within a per-element bound derived
 from the kernel's arithmetic (stated in each check's docstring; U = 2^-24 is the fp32 unit roundoff).
 """
-import ctypes
 import math
-import time
 
 import pytest
 import torch
 
 from tests.util import log_metric
-from tests.test_gpu_kernel_replay import DEV, GUARD, MODELS, SENTINEL, _gen, _seed, bits, guarded, rounded, ulp16
-from nunif_b200 import _lib, synth
+from tests.replay import (DEV, MODELS, SENTINEL32, Tally, bits, body, configurations, guarded, guarded32, record_networks, replay,
+                          round16_bound, rounded, zoe_any)
+from nunif_b200 import _lib
+from nunif_b200._lib import ptr
 
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24                 # fp32 unit roundoff
-SENTINEL32 = 0x7FC05B5B        # an fp32 NaN payload: fp32 guards keep exactly this bit pattern
 CHUNK = 1 << 24                # elements of the largest float64 temporary of one reference chunk
 LOG2E = 1.4426950408889634
 REC_AUX = 2                    # nb200_record_launches bit of the kinds replayed here (bit 0: the GEMM / attention / Swin kinds)
 
-AUX_FIELDS = {k: v.split() for k, v in {
-    "wmha": "B H W C ws heads pad_y pad_x", "reppad": "B H W C", "ln": "rows dim has_delta has_out", "upbl": "B h w C H W",
-    "zadd_up": "B h w C H W", "zsoftplus": "n", "zseed": "npix min max", "zattr": "B h w H W lda na normed min max has_sorted",
-    "zclb_concat": "B h w H W", "zclb_final": "B h w H W ldg", "zrelbias": "ph pw heads ldb"}.items()}
+AUX_KINDS = ("wmha", "reppad", "ln", "upbl", "zadd_up", "zsoftplus", "zseed", "zattr", "zclb_concat", "zclb_final", "zrelbias")
 # window_mha's instantiations: (window, heads, head dim)
 WMHA_INST = {(3, 2, 32), (4, 2, 32), (4, 4, 32), (8, 2, 16)}
 LN_DIMS = {256, 384, 768, 1024}
 
 
-def _num(v):
-    return int(v) if v.lstrip("-").isdigit() else float(v)
-
-
-def recorded_aux(fn):
-    """Run fn() with the recorder on for the kinds of AUX_FIELDS; -> [(kind, {field: value})] of its launches."""
-    lib = _lib.lib()
-    _lib.check(lib.nb200_record_launches(REC_AUX))
-    try:
-        fn()
-        torch.cuda.synchronize()
-    finally:
-        lib.nb200_record_launches(0)
-    cap = 1 << 20
-    while True:
-        buf = ctypes.create_string_buffer(cap)
-        if lib.nb200_recorded_launches(buf, cap) == 0:
-            break
-        if b"buffer too small" not in lib.nb200_last_error():
-            _lib.check(1)
-        cap *= 4
-    recs = []
-    for line in buf.value.decode().splitlines():
-        kind, *vals = line.split(",")
-        assert len(vals) == len(AUX_FIELDS[kind]), line
-        recs.append((kind, dict(zip(AUX_FIELDS[kind], (_num(v) for v in vals)))))
-    return recs
-
-
 # ------------------------------------------------------------------------------------------------------------ networks
-def _zoe_any_k():
-    from nunif_b200.iw3 import ZoeDepthAnythingNet
-    from nunif_b200.iw3.zoedepth_preprocess import preprocess_size
-    net = ZoeDepthAnythingNet(synth.zoedepth_any_state_dict(0, None, True), DEV, "ZoeD_Any_K")
-    for H, W in ((1080, 1920), (1920, 1080)):
-        _, _, ph, pw, fh, fw = preprocess_size(H, W, h_height=392, v_height=518, ensure_multiple_of=14)
-        net(torch.randn(1, 3, fh + 2 * ph, fw + 2 * pw, generator=_gen(9)).clamp_(-1, 1).to(DEV))
-
-
 _NETS = dict(MODELS)
 AUX_MODELS = [(n, _NETS[n]) for n in ("depth_anything_v2_s", "depth_anything_v2_b", "depth_anything_v2_l", "depth_anything_v1_s",
-                                      "zoed_n", "zoed_any_n")] + [("zoed_any_k", _zoe_any_k)] + \
+                                      "zoed_n", "zoed_any_n")] + [("zoed_any_k", zoe_any(True, "ZoeD_Any_K", 9))] + \
              [(n, _NETS[n]) for n in ("row_flow_v3", "mlbw_l2", "mlbw_l4", "depth_aa")]
 
 
 @pytest.fixture(scope="module")
 def production():
-    """name -> unique records (kind, config) of the kinds of AUX_FIELDS in one forward of each network of AUX_MODELS."""
-    out = {}
-    for name, fn in AUX_MODELS:
-        t0 = time.time()
-        recs = recorded_aux(fn)
-        torch.cuda.empty_cache()
-        print(f"{name}: {len(recs)} launches recorded in {time.time() - t0:.1f} s")
-        uniq = []
-        for kind, r in recs:
-            if (kind, r) not in uniq:
-                uniq.append((kind, r))
-        out[name] = uniq
-    return out
-
-
-def _cases(production, kind, synthetic=()):
-    """-> [(network or "synthetic", config)], each configuration once."""
-    seen, cases = set(), []
-    for name, r in [(n, r) for n, recs in production.items() for k, r in recs if k == kind] + [("synthetic", r) for r in synthetic]:
-        key = tuple(r[f] for f in AUX_FIELDS[kind])
-        if key not in seen:
-            seen.add(key)
-            cases.append((name, r))
-    return cases
+    """name -> unique records (kind, config) of the kinds of AUX_KINDS in one forward of each network of AUX_MODELS."""
+    return record_networks(REC_AUX, AUX_MODELS)
 
 
 def test_every_network_records_its_launches(production):
     lines = []
     for name, _ in AUX_MODELS:
-        counts = {k: sum(1 for kk, _ in production[name] if kk == k) for k in AUX_FIELDS}
+        counts = {k: sum(1 for kk, _ in production[name] if kk == k) for k in AUX_KINDS}
         lines.append(f"{name:20s} unique: " + " ".join(f"{k} {n}" for k, n in counts.items() if n))
         log_metric("replay_aux_configs", model=name, **counts)
     print("\n" + "\n".join(lines))
     kinds = {k for recs in production.values() for k, _ in recs}
-    assert kinds == set(AUX_FIELDS), f"never recorded: {set(AUX_FIELDS) - kinds}"
+    assert kinds == set(AUX_KINDS), f"never recorded: {set(AUX_KINDS) - kinds}"
     for name in ("row_flow_v3", "mlbw_l2", "mlbw_l4", "depth_aa"):
         assert {"wmha", "reppad"} <= {k for k, _ in production[name]}, name
     for name in ("depth_anything_v2_s", "depth_anything_v2_l", "zoed_n", "zoed_any_n", "zoed_any_k"):
@@ -133,78 +69,6 @@ def test_every_network_records_its_launches(production):
 
 
 # ------------------------------------------------------------------------------------------------------------ helpers
-def guarded32(n):
-    """fp32 buffer of GUARD + n + GUARD elements, all SENTINEL32."""
-    return torch.full((n + 2 * GUARD,), SENTINEL32, dtype=torch.int32, device=DEV).view(torch.float32)
-
-
-def body(buf, n):
-    """The n elements between the guards (a view whose data_ptr is what the kernel gets)."""
-    return buf[GUARD:GUARD + n]
-
-
-def guards_ok(buf, n):
-    if buf.dtype == torch.float16:
-        b, s = bits(buf), SENTINEL
-    else:
-        b, s = buf.view(torch.int32), SENTINEL32
-    return bool((b[:GUARD] == s).all() and (b[GUARD + n:] == s).all())
-
-
-def ptr(t):
-    return _lib.ptr(t)
-
-
-class Tally:
-    """Worst err / bound, elements over their bound, and the other problems of one replayed configuration."""
-
-    def __init__(self):
-        self.worst, self.over, self.bad = 0.0, 0, []
-
-    def add(self, got, ref, bound):
-        ratio = torch.nan_to_num((got.double() - ref).abs() / bound, nan=math.inf)
-        self.worst = max(self.worst, float(ratio.max()))
-        self.over += int((ratio > 1).sum())
-
-    def exact(self, what, got, want):
-        """Bit-identical (int views of the same dtype)."""
-        if not torch.equal(got, want):
-            self.bad.append(f"{what}: {int((got != want).sum())} elements differ")
-
-    def guards(self, what, buf, n):
-        if not guards_ok(buf, n):
-            self.bad.append(f"{what}: guard changed")
-
-    def no_nan(self, what, t):
-        if bool(torch.isnan(t).any()):
-            self.bad.append(f"NaN in {what}")
-
-    def result(self):
-        return self.worst, self.over, self.bad
-
-
-def round16_bound(ref, E):
-    """Bound on |fp16(v) - ref| for a value v the kernel computes within E of ref: half an fp16 ulp at |ref| + E, plus E."""
-    return 0.5 * ulp16(ref.abs() + E) + E
-
-
-def _replay(kind, cases, check):
-    t0, worst, fails = time.time(), 0.0, []
-    for name, r in cases:
-        ratio, over, bad = check(r, _seed(name, kind, tuple(r[f] for f in AUX_FIELDS[kind])))
-        cfg = ",".join(f"{f}={r[f]}" for f in AUX_FIELDS[kind])
-        log_metric(f"replay_{kind}", model=name, cfg=cfg, err_over_bound=f"{ratio:.3g}")
-        worst = max(worst, ratio)
-        if bad or over:
-            fails.append(f"{name} {cfg}: {bad} max err/bound {ratio:.3g}, {over} elements over")
-    torch.cuda.synchronize()
-    print(f"\n{kind}: {len(cases)} configurations, worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, "
-          f"peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
-    log_metric(f"replay_{kind}_summary", configs=len(cases), worst=worst)
-    assert not fails, "\n".join(fails[:20])
-    return worst
-
-
 # ATen upsample_bilinear2d(align_corners=True): the source coordinate of output index i is the fp32 product
 # ((in - 1) / (out - 1) in fp32) * i, its integer part the first tap and its fraction the weight of the second
 def ac_index(n_in, n_out):
@@ -279,7 +143,7 @@ def wmha_reference(qkv16, qkv_bias, bias, r):
     __expf(s - max) is within 2^-23 (2 + 1.173 |s - max|) relative (CUDA's documented maximum) after the U |s - max| rounding of
     its argument.  A relative error r_j on key j's weight moves the output by sum_j p_j r_j (v_j - o) (first order, 1.1 margin);
     the row sum, the reciprocal, p_j and the PV fma chain add (2N + 4) U sum_j p_j |v_j|."""
-    B, H, W, C, ws, heads, py, px = (r[f] for f in AUX_FIELDS["wmha"])
+    B, H, W, C, ws, heads, py, px = (r[f] for f in ("B", "H", "W", "C", "ws", "heads", "pad_y", "pad_x"))
     d, N, scale = C // heads, ws * ws, (C // heads) ** -0.5
     Hp, Wp = H + 2 * py, W + 2 * px
     pad = torch.cat([torch.zeros(C, dtype=torch.float64, device=DEV), qkv_bias[C:].half().double()])
@@ -308,7 +172,7 @@ def wmha_reference(qkv16, qkv_bias, bias, r):
 
 
 def wmha_check(r, seed):
-    B, H, W, C, ws, heads, py, px = (r[f] for f in AUX_FIELDS["wmha"])
+    B, H, W, C, ws, heads, py, px = (r[f] for f in ("B", "H", "W", "C", "ws", "heads", "pad_y", "pad_x"))
     M, tally = B * H * W, Tally()
     for mode in ("random", "bias") + (("pad",) if py or px else ()):
         qkv16, qkv_bias, bias = wmha_inputs(r, mode, seed)
@@ -334,12 +198,12 @@ def wmha_check(r, seed):
 def test_window_mha_replay(production):
     have = {(r["ws"], r["heads"], r["C"] // r["heads"]) for recs in production.values() for k, r in recs if k == "wmha"}
     print(f"\nwindow_mha instantiations recorded: {sorted(have)}")
-    cases = _cases(production, "wmha", _synthetic_wmha())
+    cases = configurations(production, "wmha", _synthetic_wmha())
     assert {(r["ws"], r["heads"], r["C"] // r["heads"]) for _, r in cases} == WMHA_INST
     for ws, heads, hd in WMHA_INST:
         pads = {(r["pad_y"], r["pad_x"]) for _, r in cases if (r["ws"], r["heads"], r["C"] // r["heads"]) == (ws, heads, hd)}
         assert pads >= ({(0, 0)} | ({(0, ws // 2), (ws // 2, 0), (ws // 2, ws // 2)} if ws % 2 == 0 else set())), (ws, heads, pads)
-    _replay("wmha", cases, wmha_check)
+    replay("wmha", cases, wmha_check)
 
 
 def test_window_mha_refuses_bad_padding():
@@ -366,7 +230,7 @@ SYNTH_REPPAD = [dict(B=2, H=1, W=1, C=8), dict(B=3, H=7, W=5, C=24), dict(B=1, H
 
 def reppad_check(r, seed):
     """Bit-exact against ReplicationPad2d(1) built from clamped indices."""
-    B, H, W, C = (r[f] for f in AUX_FIELDS["reppad"])
+    B, H, W, C = (r[f] for f in ("B", "H", "W", "C"))
     g = torch.Generator(device=DEV).manual_seed(seed)
     n, no = B * H * W * C, B * (H + 2) * (W + 2) * C
     xb, out = guarded(n), guarded(no)
@@ -385,7 +249,7 @@ def reppad_check(r, seed):
 
 
 def test_reppad_replay(production):
-    _replay("reppad", _cases(production, "reppad", SYNTH_REPPAD), reppad_check)
+    replay("reppad", configurations(production, "reppad", SYNTH_REPPAD), reppad_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ add + LayerNorm
@@ -420,7 +284,7 @@ def ln_check(r, seed):
     relative error is (D + 5) U plus e_m^2 / var (Sum(x - mean) = 0 cancels the first-order term), rsqrtf adds 2 ulp and eps one
     rounding, so rstd is within e_r = ((D + 5) U var + e_m^2) / (2 (var + eps)) + U / 2 + 2^-22 relative; the affine tail
     (x - m) rstd w + b rounds three times.  E = 1.1 (|w| rstd (e_m + |x - mean| (e_r + 3 U)) + 2 U (|y| + |b|))."""
-    rows, dim, has_delta, has_out = (r[f] for f in AUX_FIELDS["ln"])
+    rows, dim, has_delta, has_out = (r[f] for f in ("rows", "dim", "has_delta", "has_out"))
     x, delta, w, b = ln_inputs(r, seed)
     n = rows * dim
     xb = guarded32(n)
@@ -459,10 +323,10 @@ def ln_check(r, seed):
 
 
 def test_add_layernorm_replay(production):
-    cases = _cases(production, "ln", SYNTH_LN)
+    cases = configurations(production, "ln", SYNTH_LN)
     assert {r["dim"] for _, r in cases} == LN_DIMS
     assert {(r["has_delta"], r["has_out"]) for _, r in cases} >= {(1, 1), (0, 1), (1, 0)}
-    _replay("ln", cases, ln_check)
+    replay("ln", cases, ln_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ bilinear upsample
@@ -521,11 +385,11 @@ def zadd_up_check(r, seed):
 
 
 def test_upsample_bilinear_replay(production):
-    _replay("upbl", _cases(production, "upbl", SYNTH_UPBL), upbl_check)
+    replay("upbl", configurations(production, "upbl", SYNTH_UPBL), upbl_check)
 
 
 def test_zoe_add_upsampled_replay(production):
-    _replay("zadd_up", _cases(production, "zadd_up", SYNTH_UPBL), zadd_up_check)
+    replay("zadd_up", configurations(production, "zadd_up", SYNTH_UPBL), zadd_up_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ clb concat
@@ -536,7 +400,7 @@ def clb_concat_check(r, seed):
     """A[pix] = [bilinear(emb) 128 | act 32 | fp16(rel) | 31 zeros]: the copy groups (act, rel at this size: the reference's
     interpolate of rel to act's size is the identity, then .to(fp16)) and the zeros bit-exact, the interpolated groups one fp16
     rounding as in upbl_check."""
-    B, h, w, H, W = (r[f] for f in AUX_FIELDS["zclb_concat"])
+    B, h, w, H, W = (r[f] for f in ("B", "h", "w", "H", "W"))
     g = torch.Generator(device=DEV).manual_seed(seed)
     npix, ne = B * H * W, B * h * w * 128
     act, eb, relb, out = guarded(npix * 32), guarded(ne), guarded32(npix), guarded(npix * 192)
@@ -565,7 +429,7 @@ def clb_concat_check(r, seed):
 
 
 def test_zoe_clb_concat_replay(production):
-    _replay("zclb_concat", _cases(production, "zclb_concat", SYNTH_CLB_CONCAT), clb_concat_check)
+    replay("zclb_concat", configurations(production, "zclb_concat", SYNTH_CLB_CONCAT), clb_concat_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ softplus
@@ -597,7 +461,7 @@ def softplus_check(r, seed):
 
 
 def test_zoe_softplus_replay(production):
-    _replay("zsoftplus", _cases(production, "zsoftplus", [dict(n=1), dict(n=12), dict(n=64 * 1001 + 3)]), softplus_check)
+    replay("zsoftplus", configurations(production, "zsoftplus", [dict(n=1), dict(n=12), dict(n=64 * 1001 + 3)]), softplus_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ normed seed
@@ -633,7 +497,8 @@ def seed_check(r, seed):
 
 
 def test_zoe_seed_normed_replay(production):
-    _replay("zseed", _cases(production, "zseed", [dict(npix=1, min=0.001, max=80), dict(npix=8 * 37 + 5, min=0.5, max=10.0)]), seed_check)
+    cases = configurations(production, "zseed", [dict(npix=1, min=0.001, max=80), dict(npix=8 * 37 + 5, min=0.5, max=10.0)])
+    replay("zseed", cases, seed_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ attractors
@@ -724,12 +589,12 @@ def attractor_check(r, seed):
 
 
 def test_zoe_attractor_replay(production):
-    cases = _cases(production, "zattr", SYNTH_ZATTR)
+    cases = configurations(production, "zattr", SYNTH_ZATTR)
     na_max = max(r["na"] for _, r in cases)
     for normed in (0, 1):
         assert {r["na"] for _, r in cases if r["normed"] == normed} >= {1, na_max}, normed
     assert any(r["has_sorted"] and r["h"] == r["H"] and r["w"] == r["W"] for _, r in cases)
-    _replay("zattr", cases, attractor_check)
+    replay("zattr", cases, attractor_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ log-binomial mixture
@@ -758,7 +623,7 @@ def clb_final_check(r, seed):
 
     The first four hidden channels steer t: w2 = [I_4 | 0.05 N(0, 1)], so rows cycle through p near 0 / 1 (clamped at 1e-4 and
     1 - 1e-4), the temperature at its minimum (0.0212) and maximum (50), and random values."""
-    B, h, w, H, W, ldg = (r[f] for f in AUX_FIELDS["zclb_final"])
+    B, h, w, H, W, ldg = (r[f] for f in ("B", "h", "w", "H", "W", "ldg"))
     g = torch.Generator(device=DEV).manual_seed(seed)
     rn = lambda *s: torch.randn(*s, generator=g, device=DEV)
     npix, nb = B * H * W, B * h * w * 64
@@ -831,9 +696,9 @@ def clb_final_check(r, seed):
 
 
 def test_zoe_clb_final_replay(production):
-    cases = _cases(production, "zclb_final", _synthetic_clb_final())
+    cases = configurations(production, "zclb_final", _synthetic_clb_final())
     assert any(r["ldg"] > 80 for _, r in cases) and any(r["ldg"] == 80 for _, r in cases)
-    _replay("zclb_final", cases, clb_final_check)
+    replay("zclb_final", cases, clb_final_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ BEiT bias expansion
@@ -845,7 +710,7 @@ def relbias_check(r, seed):
     gen_relative_position_index (oracle/zoedepth.py relative_position_index, not the kernel's formula); columns N..ldb-1 keep
     their sentinel."""
     from oracle.zoedepth import relative_position_index
-    ph, pw, heads, ldb = (r[f] for f in AUX_FIELDS["zrelbias"])
+    ph, pw, heads, ldb = (r[f] for f in ("ph", "pw", "heads", "ldb"))
     N, rows = ph * pw + 1, (2 * ph - 1) * (2 * pw - 1) + 3
     g = torch.Generator(device=DEV).manual_seed(seed)
     table = torch.randn(rows, heads, generator=g, device=DEV)
@@ -865,4 +730,4 @@ def relbias_check(r, seed):
 
 
 def test_zoe_expand_rel_bias_replay(production):
-    _replay("zrelbias", _cases(production, "zrelbias", SYNTH_ZRELBIAS), relbias_check)
+    replay("zrelbias", configurations(production, "zrelbias", SYNTH_ZRELBIAS), relbias_check)

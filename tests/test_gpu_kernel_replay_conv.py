@@ -3,8 +3,8 @@ production shapes, against float64 references: the first 3x3 conv of every waifu
 UpCUNet tails (tail_conv_mma_kernel), the UpConv7 / VGG7 output heads (head_conv_mma_kernel), the SE block, SwinUNet's
 to_image (pixel shuffle and the bicubic-antialias 2x / 1x views) and every REBNCONV of iw3.sod_v1 (sod_conv_kernel).
 
-The discipline of tests/test_gpu_kernel_replay.py and tests/test_gpu_kernel_replay_aux.py, whose helpers are reused: a module
-fixture turns on bit 2 of the launch recorder and records one forward of each waifu2x network of MODELS (tile 256, batch 16),
+The discipline of tests/test_gpu_kernel_replay.py and tests/test_gpu_kernel_replay_aux.py, with the helpers of tests/replay.py:
+a module fixture turns on bit 2 of the launch recorder and records one forward of each waifu2x network of MODELS (tile 256, batch 16),
 of swin_unet_4x.to_1x() and of SODV1.infer at B = 4 and B = 1; small forwards at other tiles and batches, and a synthetic list,
 add the edges production does not reach.  Each unique configuration is replayed through the kernel's test entry point on fresh
 seeded data, once on the production path and, for the stem / tail / head, once on their SIMT kernels (nb200_tune_set(7, 1));
@@ -21,7 +21,6 @@ cout_pad).  Each output element is checked against a float64 reference written f
 upsample_bicubic2d_aa, the REBNCONV under autocast) within a bound derived from the kernel's arithmetic, stated in each check's
 docstring (U = 2^-24 is the fp32 unit roundoff).
 """
-import ctypes
 import time
 
 import pytest
@@ -29,62 +28,23 @@ import torch
 import torch.nn.functional as F
 
 from tests.util import log_metric
-from tests.test_gpu_kernel_replay import DEV, MODELS, SENTINEL, _gen, _seed, bits, guarded, rounded
-from tests.test_gpu_kernel_replay_aux import Tally, _num, body, guarded32, guards_ok, ptr, round16_bound
+from tests.replay import (DEV, MODELS, SENTINEL, Tally, _gen, bits, body, configurations, guarded, guarded32, guards_ok,
+                          record_networks, recorded, replay, round16_bound, rounded, swin_sd, waifu2x)
 from nunif_b200 import _lib, synth
+from nunif_b200._lib import ptr
 
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24                 # fp32 unit roundoff
 REC_CONV = 4                   # nb200_record_launches bit of the kinds replayed here
 ACC = 2.0 ** -20               # per chained mma.sync k-step: |fp32 accumulator - exact| <= ACC * L * sum |a w|
 
-CONV_FIELDS = {k: v.split() for k, v in {
-    "stem": "n Hi Wi cout_pad ldo path", "tail": "mode epi n Hi Wi z1H z1W clip path", "head": "mode cin n Hi Wi path",
-    "se": "n H W C", "toimg": "n Hs Ws cs r down",
-    "sodconv": "B H W cin cout dil in_ld in_off out_ld out_off has_res res_ld"}.items()}
-# what identifies a configuration: `path` is the host's choice of kernel for it (0 mma.sync, 1 SIMT)
-KEY = {k: [f for f in v if f != "path"] for k, v in CONV_FIELDS.items()}
+CONV_KINDS = ("stem", "tail", "head", "se", "toimg", "sodconv")
 WAIFU2X = ("swin_unet_4x", "swin_unet_4x.to_2x", "swin_unet_2x", "swin_unet_1x", "upcunet", "cunet", "upconv_7", "vgg_7")
 SOD_CONVS = 112                # REBNCONVs per SODV1 forward (csrc/sod_kernels.h sod_layer_list)
 T0 = None                      # start of the module's recording fixture
 
 
-def recorded_conv(fn):
-    """Run fn() with the recorder on for the kinds of CONV_FIELDS; -> [(kind, {field: value})] of its launches."""
-    lib = _lib.lib()
-    _lib.check(lib.nb200_record_launches(REC_CONV))
-    try:
-        fn()
-        torch.cuda.synchronize()
-    finally:
-        lib.nb200_record_launches(0)
-    cap = 1 << 20
-    while True:
-        buf = ctypes.create_string_buffer(cap)
-        if lib.nb200_recorded_launches(buf, cap) == 0:
-            break
-        if b"buffer too small" not in lib.nb200_last_error():
-            _lib.check(1)
-        cap *= 4
-    recs = []
-    for line in buf.value.decode().splitlines():
-        kind, *vals = line.split(",")
-        assert len(vals) == len(CONV_FIELDS[kind]), line
-        recs.append((kind, dict(zip(CONV_FIELDS[kind], (_num(v) for v in vals)))))
-    return recs
-
-
 # ------------------------------------------------------------------------------------------------------------ networks
-def _tiles(name, sd_fn, T, n, view=None):
-    def run():
-        from nunif_b200.nunif.models import create_model
-        m = create_model(name, sd_fn(), DEV)
-        if view:
-            m = getattr(m, view)()
-        m(torch.rand(n, 3, T, T, generator=_gen(11)).to(DEV))
-    return run
-
-
 def _sod(B):
     def run():
         from nunif_b200.iw3 import SODV1
@@ -94,30 +54,26 @@ def _sod(B):
     return run
 
 
-def _sw(scale):
-    return lambda: synth.swin_unet_state_dict(0, scale)
-
-
 _NETS = dict(MODELS)
 CONV_MODELS = [(n, _NETS[n]) for n in WAIFU2X] + [
-    ("swin_unet_4x.to_1x", _tiles("waifu2x.swin_unet_4x", _sw(4), 256, 16, "to_1x")),   # down 4: no network of MODELS
+    ("swin_unet_4x.to_1x", waifu2x("waifu2x.swin_unet_4x", swin_sd(4), view="to_1x", seed=11)),   # down 4: no network of MODELS
     ("sod_v1_b4", _sod(4)),    # iw3 --convergence-mode sod_v1 on the iw3_1080p batch: 4 frames, 392 x 686 depth
     ("sod_v1_b1", _sod(1)),
 ]
 # other tiles and batches: Swin / CUNet / UpCUNet at tile 64, the legacy models at tiles 15 (head output of 1 or 2 rows), 61
 # and 104, batches 1 and 3
 EDGE_MODELS = [
-    ("swin_unet_4x T64 n3", _tiles("waifu2x.swin_unet_4x", _sw(4), 64, 3)),
-    ("swin_unet_4x.to_2x T64 n1", _tiles("waifu2x.swin_unet_4x", _sw(4), 64, 1, "to_2x")),
-    ("swin_unet_4x.to_1x T64 n3", _tiles("waifu2x.swin_unet_4x", _sw(4), 64, 3, "to_1x")),
-    ("swin_unet_2x T64 n1", _tiles("waifu2x.swin_unet_2x", _sw(2), 64, 1)),
-    ("swin_unet_1x T64 n3", _tiles("waifu2x.swin_unet_1x", _sw(1), 64, 3)),
-    ("cunet T64 n3", _tiles("waifu2x.cunet", synth.cunet_state_dict, 64, 3)),
-    ("cunet T64 n1", _tiles("waifu2x.cunet", synth.cunet_state_dict, 64, 1)),
-    ("upcunet T64 n1", _tiles("waifu2x.upcunet", synth.upcunet_state_dict, 64, 1)),
-    ("upcunet T64 n3", _tiles("waifu2x.upcunet", synth.upcunet_state_dict, 64, 3)),
-] + [(f"{m} T{T} n{n}", _tiles(f"waifu2x.{m}", sd, T, n)) for m, sd in (("upconv_7", synth.upconv7_state_dict), ("vgg_7", synth.vgg7_state_dict))
-     for T, n in ((15, 3), (61, 1), (104, 3))]
+    ("swin_unet_4x T64 n3", waifu2x("waifu2x.swin_unet_4x", swin_sd(4), 64, 3, seed=11)),
+    ("swin_unet_4x.to_2x T64 n1", waifu2x("waifu2x.swin_unet_4x", swin_sd(4), 64, 1, "to_2x", 11)),
+    ("swin_unet_4x.to_1x T64 n3", waifu2x("waifu2x.swin_unet_4x", swin_sd(4), 64, 3, "to_1x", 11)),
+    ("swin_unet_2x T64 n1", waifu2x("waifu2x.swin_unet_2x", swin_sd(2), 64, 1, seed=11)),
+    ("swin_unet_1x T64 n3", waifu2x("waifu2x.swin_unet_1x", swin_sd(1), 64, 3, seed=11)),
+    ("cunet T64 n3", waifu2x("waifu2x.cunet", synth.cunet_state_dict, 64, 3, seed=11)),
+    ("cunet T64 n1", waifu2x("waifu2x.cunet", synth.cunet_state_dict, 64, 1, seed=11)),
+    ("upcunet T64 n1", waifu2x("waifu2x.upcunet", synth.upcunet_state_dict, 64, 1, seed=11)),
+    ("upcunet T64 n3", waifu2x("waifu2x.upcunet", synth.upcunet_state_dict, 64, 3, seed=11)),
+] + [(f"{m} T{T} n{n}", waifu2x(f"waifu2x.{m}", sd, T, n, seed=11))
+     for m, sd in (("upconv_7", synth.upconv7_state_dict), ("vgg_7", synth.vgg7_state_dict)) for T, n in ((15, 3), (61, 1), (104, 3))]
 
 
 @pytest.fixture(scope="module")
@@ -125,31 +81,15 @@ def production():
     """name -> [(kind, config)] of every recorded launch (not deduplicated: the coverage test counts them), for the networks
     of CONV_MODELS and EDGE_MODELS."""
     global T0
-    t0 = T0 = time.time()
+    T0 = time.time()
     torch.cuda.reset_peak_memory_stats()
-    out = {}
-    for name, fn in CONV_MODELS + EDGE_MODELS:
-        out[name] = recorded_conv(fn)
-        torch.cuda.empty_cache()
-    print(f"\nrecorded {sum(len(v) for v in out.values())} launches of {len(out)} forwards in {time.time() - t0:.1f} s")
-    return out
-
-
-def _cases(production, kind, synthetic=()):
-    """-> [(network or "synthetic", config)], each configuration once (keyed without the recorded path)."""
-    seen, cases = set(), []
-    for name, r in [(n, r) for n, recs in production.items() for k, r in recs if k == kind] + [("synthetic", r) for r in synthetic]:
-        key = tuple(r[f] for f in KEY[kind])
-        if key not in seen:
-            seen.add(key)
-            cases.append((name, r))
-    return cases
+    return record_networks(REC_CONV, CONV_MODELS + EDGE_MODELS, unique=False)
 
 
 def test_every_network_records_its_launches(production):
     lines = []
     for name in production:
-        counts = {k: sum(1 for kk, _ in production[name] if kk == k) for k in CONV_FIELDS}
+        counts = {k: sum(1 for kk, _ in production[name] if kk == k) for k in CONV_KINDS}
         lines.append(f"{name:28s} launches: " + " ".join(f"{k} {n}" for k, n in counts.items() if n))
         log_metric("replay_conv_launches", model=name, **counts)
     print("\n" + "\n".join(lines))
@@ -194,35 +134,22 @@ def leaky64(v):
 
 def path_check(tally, kind, fn, path):
     """Launch fn() under the recorder: exactly one launch of `kind`, on the kernel path expected."""
-    got = [r["path"] for k, r in recorded_conv(fn) if k == kind]
+    got = [r["path"] for k, r in recorded(REC_CONV, fn) if k == kind]
     if got != [path]:
         tally.bad.append(f"{kind}: recorded paths {got}, expected [{path}]")
 
 
-def _replay(kind, cases, check, paths=(0,)):
-    """check(r, seed, path) -> (worst err / bound, elements over, problems) per configuration and kernel path."""
-    t0, worst, fails, lib = time.time(), 0.0, [], _lib.lib()
-    try:
-        for path in paths:
-            _lib.check(lib.nb200_tune_set(7, path))
-            for name, r in cases:
-                key = tuple(r[f] for f in KEY[kind])
-                ratio, over, bad = check(r, _seed(name, kind, key), path)
-                cfg = ",".join(f"{f}={r[f]}" for f in KEY[kind])
-                log_metric(f"replay_{kind}", model=name, cfg=cfg, path=path, err_over_bound=f"{ratio:.3g}")
-                worst = max(worst, ratio)
-                if bad or over:
-                    fails.append(f"{name} {cfg} path {path}: {bad} max err/bound {ratio:.3g}, {over} elements over")
-    finally:
-        lib.nb200_tune_set(7, 0)
-    torch.cuda.synchronize()
-    n_prod = sum(1 for n, _ in cases if n != "synthetic")
-    print(f"\n{kind}: {len(cases)} configurations ({n_prod} recorded, {len(cases) - n_prod} synthetic) x {len(paths)} paths, "
-          f"worst err/bound {worst:.3g}, {time.time() - t0:.1f} s, peak device memory "
-          f"{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
-    log_metric(f"replay_{kind}_summary", configs=len(cases), paths=len(paths), worst=worst)
-    assert not fails, "\n".join(fails[:20])
-    return worst
+def on_path(check):
+    """check(r, seed, path) with the stem / tail / head kernel knob set for the call (nb200_tune_set(7, path): 0 mma.sync,
+    1 SIMT)."""
+    def run(r, seed, path):
+        lib = _lib.lib()
+        _lib.check(lib.nb200_tune_set(7, path))
+        try:
+            return check(r, seed, path)
+        finally:
+            lib.nb200_tune_set(7, 0)
+    return run
 
 
 # ------------------------------------------------------------------------------------------------------------ stem
@@ -267,9 +194,9 @@ def stem_check(r, seed, path):
 
 
 def test_stem_replay(production):
-    cases = _cases(production, "stem", SYNTH_STEM)
+    cases = configurations(production, "stem", SYNTH_STEM)
     assert {r["cout_pad"] for _, r in cases} == {32, 64}
-    _replay("stem", cases, stem_check, paths=(0, 1))
+    replay("stem", cases, on_path(stem_check), variant=("path", (0, 1)))
 
 
 # ------------------------------------------------------------------------------------------------------------ tail
@@ -322,11 +249,11 @@ def tail_check(r, seed, path):
 
 
 def test_tail_replay(production):
-    cases = _cases(production, "tail", [dict(mode=0, epi=0, n=2, Hi=9, Wi=131, z1H=0, z1W=0, clip=1, path=0),
+    cases = configurations(production, "tail", [dict(mode=0, epi=0, n=2, Hi=9, Wi=131, z1H=0, z1W=0, clip=1, path=0),
                                         dict(mode=1, epi=0, n=1, Hi=5, Wi=67, z1H=0, z1W=0, clip=0, path=0)])
     assert {(r["mode"], r["epi"]) for _, r in cases} == {(0, 0), (0, 1), (1, 0)}
     assert {r["clip"] for _, r in cases if r["epi"] == 0} == {0, 1}
-    _replay("tail", cases, tail_check, paths=(0, 1))
+    replay("tail", cases, on_path(tail_check), variant=("path", (0, 1)))
 
 
 # ------------------------------------------------------------------------------------------------------------ head
@@ -363,17 +290,17 @@ def head_check(r, seed, path):
 
 
 def test_head_replay(production):
-    cases = _cases(production, "head")
+    cases = configurations(production, "head")
     assert {(r["mode"], r["cin"]) for _, r in cases} == {(0, 128), (1, 256)}
     assert {r["Hi"] for _, r in cases} >= {3, 49, 92, 244}
-    _replay("head", cases, head_check, paths=(0, 1))
+    replay("head", cases, on_path(head_check), variant=("path", (0, 1)))
 
 
 # ------------------------------------------------------------------------------------------------------------ SE
 SYNTH_SE = [dict(n=n, H=H, W=W, C=C) for C in (64, 128) for n, H, W in ((3, 7, 9), (1, 32, 64), (3, 3, 683), (1, 122, 122))]
 
 
-def se_check(r, seed, path):
+def se_check(r, seed):
     """x *= sigmoid(conv2(relu(conv1(mean_HW x)))) with the 1x1 convs' weights and biases rounded to fp16, in float64.
 
     First-order bound: a thread sums 2048 / ROWS pixels of its chunk (ROWS = 2048 / C pixel rows per block), the block ROWS
@@ -382,7 +309,7 @@ def se_check(r, seed, path):
     with R = C / 8; sigmoid's slope s (1 - s) carries that, and __expf's 2^-23 (2 + 1.173 |a|) relative error on e^-a moves
     the sigmoid by (1 - s) s times it (plus 2 U for the add and divide).  The scaled output is one fp32 product (U) and one fp16
     rounding; E = 1.1 |x| e_scale + U |x s|."""
-    n, H, W, C = (r[f] for f in KEY["se"])
+    n, H, W, C = (r[f] for f in ("n", "H", "W", "C"))
     HW, R = H * W, C // 8
     rows = 2048 // C
     nchunks = -(-HW // 2048)
@@ -421,11 +348,11 @@ def se_check(r, seed, path):
 
 
 def test_se_replay(production):
-    cases = _cases(production, "se", SYNTH_SE)
+    cases = configurations(production, "se", SYNTH_SE)
     assert {r["C"] for _, r in cases} == {64, 128}
     hw = {r["H"] * r["W"] for _, r in cases}
     assert 14884 in hw and 2048 in hw and 2049 in hw and min(hw) < 2048
-    _replay("se", cases, se_check)
+    replay("se", cases, se_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ to_image
@@ -458,14 +385,14 @@ def aa_weights(n_in, scale):
     return (w / w.sum(1, keepdim=True)).to(DEV)
 
 
-def toimg_check(r, seed, path):
+def toimg_check(r, seed):
     """down 1: bit-exact against clamp(pixel_shuffle(y), 0, 1) in fp16 (an fp16 value clamped in fp32 is fp16 again).
     down 2 / 4: fp32 against the float64 bicubic-antialias resize of that clamp (aa_weights, horizontal then vertical) and a
     clamp after it.  The tap arguments are exact (a power-of-two scale); the cubic's four or five fp32 roundings of terms below 8
     and the division by the sum t >= 1 put every fp32 tap weight within e_w = 2^-20 of the normalised float64 one.  With inputs
     in [0, 1], NT = 4 down taps and Sx, Sy the sums of |weights|: the horizontal pass is within
     NT (e_w + U Sx), the vertical one E = Sy NT (e_w + U Sx) + NT e_w Sx + NT U Sy Sx.  Channels 3 r^2 .. cs-1 of y are NaN."""
-    n, Hs, Ws, cs, rr, down = (r[f] for f in KEY["toimg"])
+    n, Hs, Ws, cs, rr, down = (r[f] for f in ("n", "Hs", "Ws", "cs", "r", "down"))
     S_full = Hs * rr
     S = S_full // down
     g = torch.Generator(device=DEV).manual_seed(seed)
@@ -503,9 +430,9 @@ def toimg_check(r, seed, path):
 
 
 def test_to_image_replay(production):
-    cases = _cases(production, "toimg", SYNTH_TOIMG)
+    cases = configurations(production, "toimg", SYNTH_TOIMG)
     assert {toimg_variant(r) for _, r in cases} == {"r4", "down2", "down4", "generic"}
-    _replay("toimg", cases, toimg_check)
+    replay("toimg", cases, toimg_check)
 
 
 # ------------------------------------------------------------------------------------------------------------ SOD REBNCONV
@@ -521,13 +448,14 @@ SYNTH_SOD = [_sod_cfg(B, H, cin, cout, 8, res) for H, B in ((6, 3), (12, 1)) for
             [_sod_cfg(2, H, cin, cout, d, 1) for H in (6, 12) for cin, cout in ((64, 64), (16, 16)) for d in (2, 4)]
 
 
-def sod_check(r, seed, path):
+def sod_check(r, seed):
     """REBNCONV under autocast, with the kernel's rounding points (csrc/sod.cu): a = fp16(conv3x3_dil(x)) (cuDNN's fp16 output),
     fp16(a + bias), ReLU, then + res (fp32) and one fp16 rounding.  The accumulator is within ACC L sum|x w| with
     L = 9 cin / 16 k16 steps; each fp16 rounding point carries forward only the difference that a rounding boundary within the
     bound allows (rounded()); the bias add and the residual add are fp32 (U |v| each).  The input slice sits in a wider buffer
     whose other channels are NaN; the output slice's neighbours keep their sentinel."""
-    B, H, W, cin, cout, dil, in_ld, in_off, out_ld, out_off, has_res, res_ld = (r[f] for f in KEY["sodconv"])
+    B, H, W, cin, cout, dil, in_ld, in_off, out_ld, out_off, has_res, res_ld = (
+        r[f] for f in ("B", "H", "W", "cin", "cout", "dil", "in_ld", "in_off", "out_ld", "out_off", "has_res", "res_ld"))
     g = torch.Generator(device=DEV).manual_seed(seed)
     npx = B * H * W
     xb, out = guarded(npx * in_ld), guarded(npx * out_ld)
@@ -573,11 +501,11 @@ def sod_check(r, seed, path):
 
 
 def test_sod_conv_replay(production):
-    cases = _cases(production, "sodconv", SYNTH_SOD)
+    cases = configurations(production, "sodconv", SYNTH_SOD)
     have = {(r["cout"], r["dil"]) for _, r in cases}
     assert have >= {(c, d) for c in (16, 64) for d in (1, 2, 4, 8)}, have
     assert {(r["cin"], r["cout"]) for _, r in cases} == set(SOD_PAIRS)
-    _replay("sodconv", cases, sod_check)
+    replay("sodconv", cases, sod_check)
 
 
 def test_wall_time_and_device(production):
