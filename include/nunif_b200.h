@@ -502,7 +502,7 @@ int nb200_sod_conv_f16(const void* in, int in_ld, int in_off, int cin, const voi
 /* shifted-window attention core between the qkv and proj Linears
  * (torchvision swin_transformer.py:166-221), window 6x6, 6 heads.
  * qkv: three dense planes q | k | v, each [B][H][W][C] fp16 (how the engine's qkv GEMM writes them)
- * -> out [B][H][W][C] fp16; bias_table fp32 [121][6]. */
+ * -> out [B][H][W][C] fp16; bias_table fp32 [121][6].  A shift > 0 needs H and W both 6 (no shift) or both larger. */
 int nb200_window_attention_f16(const void* qkv, const float* bias_table, void* out, int B,
                                int H, int W, int C, int heads, int shift, void* stream);
 
@@ -525,7 +525,8 @@ int nb200_swin_mlp_fused_y_f16(void* x, const void* att, long long T, int C, con
 /* Head of one SwinTransformerBlock: qkv Linear + shifted 6x6 window attention (swin_transformer.py:166-221;
  * everything but the proj Linear), the engine's GEMM and window-attention kernels (csrc/swin_block.cu).
  * x, att: [B][H][W][C] fp16; wqkv [3C][C] fp16 and bqkv [3C] fp32 in the reference's row order
- * (q | k | v), bias_table = relative_position_bias_table [121][6] fp32.  C in {96, 192}, H and W multiples of 6. */
+ * (q | k | v), bias_table = relative_position_bias_table [121][6] fp32.  C in {96, 192}, H and W multiples of 6.
+ * A shift > 0 needs H and W both 6 (no shift) or both larger; exactly one side of 6 is refused. */
 int nb200_swin_attn_fused_f16(const void* x, const void* wqkv, const float* bqkv,
                               const float* bias_table, void* att, int B, int H, int W, int C,
                               int shift, void* stream);

@@ -84,7 +84,8 @@ static int num_sms() { return device_sm_count(); }
 std::atomic<int> g_tune_epoch{0};
 int g_tune[16] = {0, 0, 0, /*3 force gather backward warp*/ 0, 0, 0, /*6 attention smem carveout %*/ 0,
                   /*7 SIMT stem / tail convs*/ 0, 0, /*9 CUDA-graph replay of nb200_model_forward*/ 0,
-                  /*10 > 0: grid cap of the persistent Swin tail (swin_block.cu)*/ 0, 0, 0, 0, 0, 0};
+                  /*10 > 0: grid cap of the persistent Swin tail (swin_block.cu)*/ 0,
+                  /*11 > 0: grid cap of the persistent Swin head (swin_attention_mma.cu)*/ 0, 0, 0, 0, 0};
 
 // 4-D NHWC view (c, x, y, b) of an fp16 tensor for the epilogue's TMA stores / residual loads
 static int encode_nhwc4(CUtensorMap* m, const __half* base, int C, int X, int Y, int B, long long sx, long long sy, long long sb,

@@ -27,6 +27,11 @@ extern int g_tune[16];  // gemm.cu (nb200_tune_set)
 
 namespace {
 constexpr int WS = 6, WTOK = 36, WPAD = 48, HEADS = 6;
+// torchvision (:151-155) zeroes the shift of each axis the window covers, but the kernels take one shift for both axes: a
+// shifted map with exactly one side of WS would be rolled along the wrong axes.  SwinUNet's maps are square.
+constexpr const char* SHIFT_ONE_AXIS_MSG =
+    "shifted window attention needs H and W both equal to the 6-token window or both larger (torchvision drops the shift per "
+    "axis; these kernels shift both axes or neither)";
 }  // namespace
 
 constexpr int NKT = 5;   // key tiles of 8 columns covering the 36 keys (columns 36..39 are masked by the bias table)
@@ -287,6 +292,7 @@ int window_attention(cudaStream_t st, const __half* qkv, const float* bias_frag_
     const float4* bias_table = reinterpret_cast<const float4*>(bias_frag_f);
     NB_CHECK(H % WS == 0 && W % WS == 0, "feature map must be a multiple of the 6x6 window");
     NB_CHECK(C == 96 || C == 192, "window attention supports C=96 (d=16) and C=192 (d=32)");
+    NB_CHECK(shift == 0 || (H == WS) == (W == WS), SHIFT_ONE_AXIS_MSG);
     if (WS >= H) shift = 0;  // torchvision :151-155
     dim3 grid((H / WS) * (W / WS), B);
     ProfScope ps(st, PC_ATTN, (double)B * H * W * C * 4 * 2, (double)B * H * W * C * 3 * 2, (double)B * H * W * C * 2);  // q,k,v in; out
@@ -634,6 +640,7 @@ int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const 
     NB_CHECK(x && wqkv && bqkv && bias_frag_f && att, "null pointer");
     NB_CHECK(H % WS == 0 && W % WS == 0, "feature map must be a multiple of the 6x6 window");
     NB_CHECK(C == 96 || C == 192, "fused window attention supports C=96 (d=16) and C=192 (d=32)");
+    NB_CHECK(shift == 0 || (H == WS) == (W == WS), SHIFT_ONE_AXIS_MSG);
     if (WS >= H) shift = 0;  // torchvision :151-155
     const long long nwin = (long long)B * (H / WS) * (W / WS);
     NB_CHECK(nwin > 0 && nwin < (1LL << 31), "window count out of range");
@@ -644,17 +651,19 @@ int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const 
     if (encode(&wmap, wqkv, 2, dims, strides, box, 64)) return 1;
     const double T = (double)B * H * W;
     ProfScope ps(st, PC_FUSED_ATTN, T * 3.0 * C * C * 2 + T * C * 36 * 4, T * C * 2, T * C * 2);   // qkv GEMM + QK^T/PV; x in, att out
-    // persistent: one CTA per SM, each taking every gridDim.x-th tile
+    // persistent: one CTA per SM, each taking every gridDim.x-th tile (g_tune[11] > 0 caps the grid, for tests; a tile's result
+    // does not depend on its CTA)
     const long long ntiles = (nwin + FA_WIN - 1) / FA_WIN;
-    const unsigned grid = (unsigned)std::min<long long>(ntiles, device_sm_count());
+    long long grid = std::min<long long>(ntiles, device_sm_count());
+    if (g_tune[11] > 0) grid = std::min<long long>(grid, g_tune[11]);
     if (rec_on()) rec_launch("swin_attn", {{"B", B}, {"H", H}, {"W", W}, {"C", C}, {"shift", shift}});
     const float4* bf = reinterpret_cast<const float4*>(bias_frag_f);
     if (C == 96) {
         if (ensure_dyn_smem((const void*)swin_attn_fused_kernel<96>, FaCfg<96>::SMEM)) return 1;
-        swin_attn_fused_kernel<96><<<grid, FA_THREADS, FaCfg<96>::SMEM, st>>>(wmap, x, bqkv, bf, att, H, W, shift, (int)nwin);
+        swin_attn_fused_kernel<96><<<(unsigned)grid, FA_THREADS, FaCfg<96>::SMEM, st>>>(wmap, x, bqkv, bf, att, H, W, shift, (int)nwin);
     } else {
         if (ensure_dyn_smem((const void*)swin_attn_fused_kernel<192>, FaCfg<192>::SMEM)) return 1;
-        swin_attn_fused_kernel<192><<<grid, FA_THREADS, FaCfg<192>::SMEM, st>>>(wmap, x, bqkv, bf, att, H, W, shift, (int)nwin);
+        swin_attn_fused_kernel<192><<<(unsigned)grid, FA_THREADS, FaCfg<192>::SMEM, st>>>(wmap, x, bqkv, bf, att, H, W, shift, (int)nwin);
     }
     NB_LAUNCHED();
     return 0;

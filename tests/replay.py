@@ -1,6 +1,7 @@
 """What the float64 kernel-replay modules (tests/test_gpu_kernel_replay*.py) share: the launch recorder's reader, the networks
 whose launches they record, the deduplication of recorded and synthetic configurations, guarded buffers, the error tally and
-the replay loop.
+the replay loop; and the float64 references of the fused Swin block's head and tail, which the persistent-schedule tests
+(tests/test_gpu_swin_head_persistent.py) use too.
 
 A recorded line is `kind,name=value,...`, named where the library's host code writes it (include/nunif_b200.h), so a
 configuration here is the dict {name: value} of one line, in the order the line gives.
@@ -318,3 +319,119 @@ def replay(kind, cases, check, variant=None):
           f"{worst:.3g}, {time.time() - t0:.1f} s, peak device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
     log_metric(f"replay_{kind}_summary", configs=len(cases), **count, worst=worst)
     assert not fails, "\n".join(fails[:20])
+
+
+# ------------------------------------------------------------------------------------------------------------ Swin block references
+def gelu64(x):
+    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
+
+
+def window_attention64(qkv, table, C, shift, eqkv=None, ws=6, heads=6):
+    """float64 torchvision shifted_window_attention body (swin_transformer.py:166-221) without the Linears.  qkv [B][H][W][3C]
+    -> output, sum_j p_j |v_j|, max_j p_j sum_j |v_j|, and with eqkv (a bound on the error of each q|k|v element) the first-order bound on the
+    output error they cause: sum_j p_j (|ds_j| |v_j - o| + ev_j), ds_j the score error.  As torchvision (:151-155), an axis the
+    window covers is not shifted, each axis on its own."""
+    from nunif_b200.synth import relative_position_index
+    B, H, W, _ = qkv.shape
+    d = C // heads
+    sh, sw = (shift if ws < H else 0), (shift if ws < W else 0)
+    nh, nw = H // ws, W // ws
+
+    def windows(t):
+        t = torch.roll(t, shifts=(-sh, -sw), dims=(1, 2)) if sh + sw > 0 else t
+        return t.view(B, nh, ws, nw, ws, 3 * C).permute(0, 1, 3, 2, 4, 5).reshape(B * nh * nw, ws * ws, 3, heads, d).permute(2, 0, 3, 1, 4)
+    xw = windows(qkv)
+    q, k, v = xw[0] * d ** -0.5, xw[1], xw[2]
+    attn = q @ k.transpose(-2, -1)
+    idx = relative_position_index(ws).to(qkv.device)
+    attn = attn + table[idx].view(ws * ws, ws * ws, -1).permute(2, 0, 1).unsqueeze(0)
+    if sh + sw > 0:
+        # torchvision's slices as written: with a zero shift, (-ws, -0) is empty and (-0, None) the whole axis
+        m = torch.zeros((H, W), device=qkv.device, dtype=qkv.dtype)
+        cnt = 0
+        for hs in ((0, -ws), (-ws, -sh), (-sh, None)):
+            for ws_ in ((0, -ws), (-ws, -sw), (-sw, None)):
+                m[hs[0]:hs[1], ws_[0]:ws_[1]] = cnt
+                cnt += 1
+        m = m.view(nh, ws, nw, ws).permute(0, 2, 1, 3).reshape(nh * nw, ws * ws)
+        m = m.unsqueeze(1) - m.unsqueeze(2)
+        m = m.masked_fill(m != 0, -100.0).masked_fill(m == 0, 0.0)
+        attn = (attn.view(B, nh * nw, heads, ws * ws, ws * ws) + m.unsqueeze(1).unsqueeze(0)).view(-1, heads, ws * ws, ws * ws)
+    p = attn.softmax(-1)
+    o = p @ v
+    outs = [o, p @ v.abs(), p.amax(-1, keepdim=True) * v.abs().sum(-2, keepdim=True)]
+    if eqkv is not None:
+        ew = windows(eqkv)
+        eq, ek, ev = ew[0] * d ** -0.5, ew[1], ew[2]
+        ds = eq @ (k.abs() + ek).transpose(-2, -1) + q.abs() @ ek.transpose(-2, -1)
+        pd = p * ds
+        # exp(ds) - 1 <= 1.1 ds for the ds << 0.1 seen here: first order with a margin
+        outs.append(1.1 * (pd @ v.abs() + pd.sum(-1, keepdim=True) * o.abs()) + p @ ev)
+    res = []
+    for o in outs:
+        o = o.transpose(1, 2).reshape(-1, ws * ws, C).view(B, nh, nw, ws, ws, C).permute(0, 1, 3, 2, 4, 5).reshape(B, H, W, C)
+        res.append(torch.roll(o, shifts=(sh, sw), dims=(1, 2)) if sh + sw > 0 else o)
+    return res
+
+
+def swin_attn_check(r, seed):
+    """One call of nb200_swin_attn_fused_f16 (the fused block head) on seeded data against window_attention64, per element
+    within ulp16 + 2^-9 sum_j p_j |v_j| + 2^-25 max_j p_j sum_j |v_j| + the propagated q|k|v rounding differences; the output's
+    guards and x's bits must not change.  -> Tally.result()."""
+    B, H, W, C, shift = r["B"], r["H"], r["W"], r["C"], r["shift"]
+    g = torch.Generator(device=DEV).manual_seed(seed)
+    rn = lambda *shape: torch.randn(*shape, generator=g, device=DEV)
+    x = rn(B, H, W, C).half()
+    wqkv = (rn(3 * C, C) / C ** 0.5).half()
+    bqkv = 0.1 * rn(3 * C)
+    table = 0.5 * rn(121, 6)
+    n = B * H * W * C
+    att = guarded(n)
+    x0 = x.clone()
+    _lib.check(_lib.lib().nb200_swin_attn_fused_f16(_lib.ptr(x), _lib.ptr(wqkv), _lib.ptr(bqkv), _lib.ptr(table),
+                                                    ctypes.c_void_p(att.data_ptr() + 2 * GUARD), B, H, W, C, shift, _lib.stream_ptr()))
+    torch.cuda.synchronize()
+    tally = Tally()
+    got = body(att, n).view(B, H, W, C)
+    tally.no_nan("the output", got)
+    tally.guards("output", att, n)
+    tally.exact("x", bits(x), bits(x0))
+    for b in range(B):
+        # q|k|v are rounded to fp16 after the bias, as the kernel stores them; before that the kernel's fp32 GEMM is within
+        # 2^-20 sum|x w| (+ the bias add) of the float64 one
+        xb = x[b:b + 1].double()
+        v = xb @ wqkv.double().t() + bqkv.double()
+        qkv, eqkv = rounded(v, 2.0 ** -20 * (xb.abs() @ wqkv.double().abs().t()) + 2.0 ** -22 * v.abs())
+        ref, spv, sub, eprop = window_attention64(qkv, table.double(), C, shift, eqkv)
+        # fp16 P, its fp32 row sum and ex2.approx as in the ViT attention; plus the q|k|v rounding differences
+        bound = ulp16(ref) + 2.0 ** -9 * spv + 2.0 ** -25 * sub + eprop
+        tally.add(got[b:b + 1], ref, bound)
+    return tally.result()
+
+
+def mlp_reference(x, att, wp, bp, w1, b1, w2, b2, wy, by):
+    """float64 block tail with the kernel's fp16 rounding points (x1, hidden, and with wy the block output) -> (reference,
+    bound per element).  Before each rounding point, the kernel's fp32 value differs from the float64 one by at most: 2^-20
+    sum|a w| per GEMM (wgmma fp32 accumulation), 2^-21 |v| for the fp32 bias / residual adds and the GELU evaluation, 1e-6 for
+    the GELU polynomial, and the differences carried from the previous rounding point through the GEMM (GELU's slope is at
+    most 1.13).  rounded() turns that into the difference after rounding."""
+    acc = 2.0 ** -20
+    x = x.double()
+    if att is not None:
+        a = att.double()
+        v = x + a @ wp.double().t() + bp.double()
+        x1, e1 = rounded(v, acc * (a.abs() @ wp.double().abs().t()) + 2.0 ** -21 * (x.abs() + v.abs()))
+    else:
+        x1, e1 = x, torch.zeros_like(x)
+    w1a = w1.double().abs()
+    pre = x1 @ w1.double().t() + b1.double()
+    h, eh = rounded(gelu64(pre), 1.13 * (acc * (x1.abs() @ w1a.t()) + e1 @ w1a.t()) + 2.0 ** -21 * pre.abs() + 1e-6)
+    w2a = w2.double().abs()
+    o = x1 + h @ w2.double().t() + b2.double()
+    eo = e1 + acc * (h.abs() @ w2a.t()) + eh @ w2a.t() + 2.0 ** -21 * (x1.abs() + o.abs())
+    if wy is None:
+        return o, ulp16(o) + eo
+    o, eo = rounded(o, eo)
+    wya = wy.double().abs()
+    y = o @ wy.double().t() + by.double()
+    return y, ulp16(y) + acc * (o.abs() @ wya.t()) + eo @ wya.t()
