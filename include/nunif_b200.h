@@ -523,7 +523,7 @@ int nb200_swin_mlp_fused_y_f16(void* x, const void* att, long long T, int C, con
                                void* stream);
 
 /* Head of one SwinTransformerBlock: qkv Linear + shifted 6x6 window attention (swin_transformer.py:166-221;
- * everything but the proj Linear), the engine's GEMM and window-attention kernels (csrc/swin_block.cu).
+ * everything but the proj Linear), the engine's fused block head (csrc/swin_attention_mma.cu).
  * x, att: [B][H][W][C] fp16; wqkv [3C][C] fp16 and bqkv [3C] fp32 in the reference's row order
  * (q | k | v), bias_table = relative_position_bias_table [121][6] fp32.  C in {96, 192}, H and W multiples of 6.
  * A shift > 0 needs H and W both 6 (no shift) or both larger; exactly one side of 6 is refused. */

@@ -63,7 +63,8 @@ void rec_launch(const char* kind, std::initializer_list<RecField> fields) {
 
 static std::mutex g_attr_mu;
 static std::map<std::pair<int, const void*>, size_t> g_dyn_smem;
-int ensure_dyn_smem(const void* func, size_t bytes) {
+static std::map<std::pair<int, const void*>, int> g_carveout;
+int ensure_dyn_smem(const void* func, size_t bytes, int carveout) {
     int dev = 0;
     NB_CUDA(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> lk(g_attr_mu);
@@ -72,8 +73,16 @@ int ensure_dyn_smem(const void* func, size_t bytes) {
         NB_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
         have = bytes;
     }
+    if (carveout > 0) {
+        int& set = g_carveout[{dev, func}];
+        if (set != carveout) {
+            NB_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
+            set = carveout;
+        }
+    }
     return 0;
 }
+int ensure_dyn_smem(const void* func, size_t bytes) { return ensure_dyn_smem(func, bytes, 0); }
 int device_sm_count() {
     static std::atomic<int> cache[64];
     int dev = 0;

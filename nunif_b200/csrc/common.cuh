@@ -89,8 +89,11 @@ int tile_gather_blend_rows(const void* z_all, int z_f32, int C, const ::nb200_ti
 #define NB_PDL_TRIGGER() asm volatile("griddepcontrol.launch_dependents;" ::: "memory")
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a PER-DEVICE attribute: cache the configured size per (device, function)
-// (api.cu).  Thread-safe; a second device in the same process gets its own opt-in.
+// (api.cu).  Thread-safe; a second device in the same process gets its own opt-in.  carveout > 0 also sets the function's
+// preferred shared-memory carveout (percent, also per device), again whenever it changes.  The carveout form is hidden so
+// that the library's dynamic symbol table does not depend on it.
 int ensure_dyn_smem(const void* func, size_t bytes);
+__attribute__((visibility("hidden"))) int ensure_dyn_smem(const void* func, size_t bytes, int carveout);
 // multiprocessor count of the CURRENT device (cached per device)
 int device_sm_count();
 

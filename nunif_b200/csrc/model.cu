@@ -207,7 +207,10 @@ static Lin pack_stem(Packer& pk, const std::string& name, int cout, int cout_pad
 
 struct SwinBlockW {
     Lin qkv, proj, fc1, fc2;
-    size_t table = 0;     // bias in accumulator-fragment order (attention kernel)
+    size_t rpb = 0;       // relative_position_bias_table [121][6] fp32, as in the state_dict
+    // rpb in the attention core's accumulator-fragment order, built on the device at load by build_bias_frag_kernel
+    // (swin_attention_mma.cu), the only definition of that layout
+    size_t table = 0;
     int C = 0, shift = 0;
 };
 
@@ -341,26 +344,8 @@ static void pack_swin_blocks(Packer& pk, std::vector<SwinBlockW>& out, const std
         b.fc2 = pack_linear(pk, p + ".mlp.3", C, 2 * C);
         const float* t = pk.get(p + ".attn.relative_position_bias_table", 121 * 6);
         if (t) {
-            // relative-position bias expanded once into the attention kernel's accumulator-fragment order
-            // (same layout as build_bias_frag_kernel in swin_attention_mma.cu): [head][mt][nt][lane][4]
-            std::vector<float> frag(BIAS_FRAG_FLOATS);
-            for (int head = 0; head < 6; ++head)
-                for (int mt = 0; mt < 3; ++mt)
-                    for (int nt = 0; nt < 6; ++nt)
-                        for (int lane = 0; lane < 32; ++lane)
-                            for (int r = 0; r < 4; ++r) {
-                                const int g = lane >> 2, t4 = lane & 3;
-                                const int row = mt * 16 + g + 8 * (r >> 1), col = nt * 8 + 2 * t4 + (r & 1);
-                                float v;
-                                if (col >= 36) v = -1e30f;
-                                else if (row >= 36) v = 0.f;
-                                else {
-                                    const int qy = row / 6, qx = row % 6, ky = col / 6, kx = col % 6;
-                                    v = 1.4426950408889634f * t[((qy - ky + 5) * 11 + (qx - kx + 5)) * 6 + head];
-                                }
-                                frag[((((size_t)head * 3 + mt) * 6 + nt) * 32 + lane) * 4 + r] = v;
-                            }
-            b.table = pk.add_f32(frag);
+            b.rpb = pk.add_f32(std::vector<float>(t, t + 121 * 6));
+            b.table = pk.add_f32(std::vector<float>(BIAS_FRAG_FLOATS));   // filled by nb200_model_create
         }
         pk.mark(p + ".attn.relative_position_index");  // buffer; the kernel recomputes the index (swin_transformer.py:267-279)
         out.push_back(b);
@@ -572,9 +557,16 @@ extern "C" int nb200_model_create(int kind, int n_tensors, const char* const* na
     m->blob_bytes = pk.blob.size();
     cudaError_t e = cudaMalloc((void**)&m->blob, m->blob_bytes);
     if (e == cudaSuccess) e = cudaMemcpy(m->blob, pk.blob.data(), m->blob_bytes, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-        delete m;
-        return fail(std::string("weight upload failed: ") + cudaGetErrorString(e));
+    // Swin blocks: each bias-fragment slot is built from the block's raw table, then synchronised, since forwards may run on
+    // non-blocking streams
+    int rc = 0;
+    for (const auto* blocks : {&m->sw.s1, &m->sw.s2, &m->sw.s3, &m->sw.s4, &m->sw.s5})
+        for (const SwinBlockW& b : *blocks)
+            if (e == cudaSuccess && !rc) rc = build_bias_frag(0, m->at<float>(b.rpb), m->at<float>(b.table));
+    if (e == cudaSuccess && !rc) e = cudaStreamSynchronize(0);
+    if (e != cudaSuccess || rc) {
+        nb200_model_destroy(m);
+        return rc ? 1 : fail(std::string("weight upload failed: ") + cudaGetErrorString(e));
     }
     *out = m;
     return 0;

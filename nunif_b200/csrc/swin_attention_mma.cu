@@ -18,8 +18,6 @@
 #include "gemm_wgmma.cuh"
 #include "swin_kernels.h"
 #include "tmap.h"
-#include <map>
-#include <mutex>
 
 namespace nb200 {
 
@@ -238,7 +236,8 @@ __global__ void __launch_bounds__(192, D == 16 ? 6 : 4) window_attention_mma_ker
 }
 
 // bias_frag[head][mt][nt][lane] (float4 = accumulator fragment order) = log2(e) * table[rel_index(row, col)][head];
-// padded key columns (>= 36) hold -1e30 so they vanish in the softmax; padded query rows hold 0.
+// padded key columns (>= 36) hold -1e30 so they vanish in the softmax; padded query rows hold 0.  The only definition of this
+// layout: the model's loader (nb200_model_create) and the C entry points below both build the table with it.
 __global__ void build_bias_frag_kernel(const float* __restrict__ table, float4* __restrict__ frag) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;  // ((head*3 + mt)*6 + nt)*32 + lane
     if (i >= HEADS * 3 * 6 * 32) return;
@@ -271,40 +270,32 @@ static size_t attn_smem_bytes() {
     return (size_t)3 * WTOK * LD * 2 + (WTOK + WPAD) * 4 + 16;
 }
 
-// opt-in shared memory + carveout, per (device, kernel): both attributes are per-device state
-static int set_attn_attrs(const void* func, size_t smem, int carveout) {
-    static std::mutex mu;
-    static std::map<std::pair<int, const void*>, int> done;
-    int dev = 0;
-    NB_CUDA(cudaGetDevice(&dev));
-    std::lock_guard<std::mutex> lk(mu);
-    int& have = done[{dev, func}];
-    if (have != carveout) {
-        NB_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        NB_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
-        have = carveout;
-    }
+// The geometry both head paths take (func: the caller, which the messages name): H and W multiples of the window, C = 96 or
+// 192, and a shift on both axes or neither.  *shift is dropped where the window covers the map (torchvision :151-155).
+static int check_window_geometry(const char* func, bool fused, int H, int W, int C, int* shift) {
+    auto refuse = [&](const std::string& msg) { return fail(std::string(func) + ": " + msg); };
+    if (H % WS != 0 || W % WS != 0) return refuse("feature map must be a multiple of the 6x6 window");
+    if (C != 96 && C != 192) return refuse(std::string(fused ? "fused " : "") + "window attention supports C=96 (d=16) and C=192 (d=32)");
+    if (*shift != 0 && (H == WS) != (W == WS)) return refuse(SHIFT_ONE_AXIS_MSG);
+    if (WS >= H) *shift = 0;
     return 0;
 }
 
 int window_attention(cudaStream_t st, const __half* qkv, const float* bias_frag_f, __half* out, int B, int H, int W, int C,
                      int shift, size_t plane) {
     const float4* bias_table = reinterpret_cast<const float4*>(bias_frag_f);
-    NB_CHECK(H % WS == 0 && W % WS == 0, "feature map must be a multiple of the 6x6 window");
-    NB_CHECK(C == 96 || C == 192, "window attention supports C=96 (d=16) and C=192 (d=32)");
-    NB_CHECK(shift == 0 || (H == WS) == (W == WS), SHIFT_ONE_AXIS_MSG);
-    if (WS >= H) shift = 0;  // torchvision :151-155
+    if (check_window_geometry(__func__, false, H, W, C, &shift)) return 1;
     dim3 grid((H / WS) * (W / WS), B);
     ProfScope ps(st, PC_ATTN, (double)B * H * W * C * 4 * 2, (double)B * H * W * C * 3 * 2, (double)B * H * W * C * 2);  // q,k,v in; out
     // shared-memory carveout: just enough for the 4 resident CTAs, the rest stays L1 (the per-head bias fragments,
     // 55 KB per layer, are re-read by every window and should hit there).  g_tune[6] overrides the percentage.
     if (C == 96) {
         const int want = g_tune[6] > 0 ? g_tune[6] : 72;   // 6 CTAs x 23.6 KB
-        if (set_attn_attrs((const void*)window_attention_mma_kernel<16>, attn_smem_bytes<16>(), want)) return 1;
+        if (ensure_dyn_smem((const void*)window_attention_mma_kernel<16>, attn_smem_bytes<16>(), want)) return 1;
         window_attention_mma_kernel<16><<<grid, 192, attn_smem_bytes<16>(), st>>>(qkv, bias_table, out, H, W, shift, plane);
     } else {
         const int want = g_tune[6] > 0 ? g_tune[6] : 86;
-        if (set_attn_attrs((const void*)window_attention_mma_kernel<32>, attn_smem_bytes<32>(), want)) return 1;
+        if (ensure_dyn_smem((const void*)window_attention_mma_kernel<32>, attn_smem_bytes<32>(), want)) return 1;
         window_attention_mma_kernel<32><<<grid, 192, attn_smem_bytes<32>(), st>>>(qkv, bias_table, out, H, W, shift, plane);
     }
     NB_LAUNCHED();
@@ -638,10 +629,7 @@ __global__ void __launch_bounds__(FA_THREADS, 1) swin_attn_fused_kernel(const __
 int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const float* bqkv, const float* bias_frag_f, __half* att,
                     int B, int H, int W, int C, int shift) {
     NB_CHECK(x && wqkv && bqkv && bias_frag_f && att, "null pointer");
-    NB_CHECK(H % WS == 0 && W % WS == 0, "feature map must be a multiple of the 6x6 window");
-    NB_CHECK(C == 96 || C == 192, "fused window attention supports C=96 (d=16) and C=192 (d=32)");
-    NB_CHECK(shift == 0 || (H == WS) == (W == WS), SHIFT_ONE_AXIS_MSG);
-    if (WS >= H) shift = 0;  // torchvision :151-155
+    if (check_window_geometry(__func__, true, H, W, C, &shift)) return 1;
     const long long nwin = (long long)B * (H / WS) * (W / WS);
     NB_CHECK(nwin > 0 && nwin < (1LL << 31), "window count out of range");
     CUtensorMap wmap;
@@ -669,4 +657,35 @@ int swin_attn_fused(cudaStream_t st, const __half* x, const __half* wqkv, const 
     return 0;
 }
 
+// The C entry points take the raw [121][6] table and expand it into a stream-ordered temporary for the call
+template <typename F>
+static int with_bias_frag(void* stream, const float* table, F call) {
+    cudaStream_t st = (cudaStream_t)stream;
+    float* frag = nullptr;
+    NB_CUDA(cudaMallocAsync((void**)&frag, BIAS_FRAG_FLOATS * sizeof(float), st));
+    int rc = build_bias_frag(st, table, frag);
+    if (!rc) rc = call(st, frag);
+    cudaFreeAsync(frag, st);
+    return rc;
+}
+
 }  // namespace nb200
+
+using namespace nb200;
+
+extern "C" int nb200_window_attention_f16(const void* qkv, const float* bias_table, void* out, int B, int H, int W, int C,
+                                          int heads, int shift, void* stream) {
+    NB_CHECK(qkv && bias_table && out, "null pointer");
+    NB_CHECK(heads == 6, "only 6 heads are supported");
+    return with_bias_frag(stream, bias_table, [&](cudaStream_t st, const float* frag) {
+        return window_attention(st, (const __half*)qkv, frag, (__half*)out, B, H, W, C, shift, (size_t)B * H * W * C);
+    });
+}
+
+extern "C" int nb200_swin_attn_fused_f16(const void* x, const void* wqkv, const float* bqkv, const float* bias_table, void* att,
+                                         int B, int H, int W, int C, int shift, void* stream) {
+    NB_CHECK(bias_table, "null pointer");
+    return with_bias_frag(stream, bias_table, [&](cudaStream_t st, const float* frag) {
+        return swin_attn_fused(st, (const __half*)x, (const __half*)wqkv, bqkv, frag, (__half*)att, B, H, W, C, shift);
+    });
+}

@@ -462,15 +462,3 @@ extern "C" int nb200_swin_mlp_fused_y_f16(void* x, const void* att, long long T,
     return swin_mlp_fused((cudaStream_t)stream, (__half*)x, (const __half*)att, T, C, (const __half*)wp, bp, (const __half*)w1, b1,
                           (const __half*)w2, b2, (__half*)y, cs, (const __half*)wy, by);
 }
-
-extern "C" int nb200_swin_attn_fused_f16(const void* x, const void* wqkv, const float* bqkv, const float* bias_table, void* att,
-                                         int B, int H, int W, int C, int shift, void* stream) {
-    NB_CHECK(bias_table, "null pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    float* frag = nullptr;   // relative-position bias in the attention core's fragment order (the model packs it at load)
-    NB_CUDA(cudaMallocAsync((void**)&frag, BIAS_FRAG_FLOATS * sizeof(float), st));
-    int rc = build_bias_frag(st, bias_table, frag);
-    if (!rc) rc = swin_attn_fused(st, (const __half*)x, (const __half*)wqkv, bqkv, frag, (__half*)att, B, H, W, C, shift);
-    cudaFreeAsync(frag, st);
-    return rc;
-}

@@ -345,19 +345,6 @@ int to_image(cudaStream_t st, const __half* y, void* z, int n, int Hs, int Ws, i
 
 using namespace nb200;
 
-extern "C" int nb200_window_attention_f16(const void* qkv, const float* bias_table, void* out, int B, int H, int W, int C,
-                                          int heads, int shift, void* stream) {
-    NB_CHECK(qkv && bias_table && out, "null pointer");
-    NB_CHECK(heads == 6, "only 6 heads are supported");
-    cudaStream_t st = (cudaStream_t)stream;
-    float* frag = nullptr;
-    NB_CUDA(cudaMallocAsync((void**)&frag, BIAS_FRAG_FLOATS * sizeof(float), st));
-    int rc = build_bias_frag(st, bias_table, frag);
-    if (!rc) rc = window_attention(st, (const __half*)qkv, frag, (__half*)out, B, H, W, C, shift, (size_t)B * H * W * C);
-    cudaFreeAsync(frag, st);
-    return rc;
-}
-
 extern "C" int nb200_to_image_f16(const void* y, int n, int Hs, int Ws, int cs, int r, int down, void* z, void* stream) {
     NB_CHECK(y && z, "null pointer");
     NB_CHECK(n > 0 && Hs > 0 && r > 0 && cs >= 3 * r * r, "bad ToImage shape");
