@@ -499,6 +499,32 @@ int nb200_to_image_f16(const void* y, int n, int Hs, int Ws, int cs, int r, int 
 int nb200_sod_conv_f16(const void* in, int in_ld, int in_off, int cin, const void* wt, const float* bias, int cout, int dil,
                        void* out, int out_ld, int out_off, const void* res, int res_ld, int B, int H, int W, void* stream);
 
+/* The input and output stages of the learned stereo networks and of depth_aa (csrc/rowflow_kernels.h, mlbw_kernels.h,
+ * depth_aa_kernels.h, where each is specified), with the geometry their model forwards compute; weight / bias are HOST fp32
+ * tensors in the PyTorch layout.  A geometry whose padded grid does not hold the image is refused before any launch.
+ *   row_flow_prep:      x [B][3][h][w] fp32 -> tokens [B][Hp][Wt][32] fp16 (replicate pad to Hp x 8 Wt, pixel_unshuffle (1, 8)).
+ *   row_flow_last_conv: tokens [B][Hp][Wt][64] fp16 -> delta [B][1][h][w] (pixel_shuffle, crop, ReplicationPad2d(1), conv 3x3
+ *                       8 -> 1, fp16 values); weight [1][8][3][3], bias [1].
+ *   mlbw_prep:          x [B][3][H][W] -> tokens [B][Hp][Wt][8 C1] fp16 (pads ph1 / pw1 leading, lv1_in); weight [C1][3][1][9].
+ *   mlbw_out:           tokens t, t0 [B][Hp][Wt][8 C1] fp16 -> delta, layer_weight [B][L][H][W] and, with hole (L = 2 only),
+ *                       the hole logits [B][1][H][W]; weight [2L (+1)][C1][1][9].  L 2 or 4.
+ *   depth_aa_minmax:    minmax[0], minmax[1] = min, max of x[0..n) (device fp32).
+ *   depth_aa_prep:      x [B][1][H][W] -> tokens [B][Hh][Wh][32] fp16, normalised by minmax unless it is NULL; weight [32][4][1][1].
+ *   depth_aa_out:       tokens [B][Hh][Wh][32] fp16, x -> out [B][1][H][W]: x + filter, clamped to [0, 1] with clamp, or with
+ *                       minmax the de-normalised infer output; weight [4][32][1][1]. */
+int nb200_row_flow_prep_f16(const float* x, int B, int h, int w, int Hp, int Wt, void* out, void* stream);
+int nb200_row_flow_last_conv_f32(const void* x, int B, int Hp, int Wt, int h, int w, const float* weight, const float* bias,
+                                 float* delta, void* stream);
+int nb200_mlbw_prep_f16(const float* x, int B, int H, int W, int ph1, int pw1, int Hp, int Wt, int C1, const float* weight,
+                        const float* bias, void* out, void* stream);
+int nb200_mlbw_out_f32(const void* t, const void* t0, int B, int H, int W, int ph1, int pw1, int Hp, int Wt, int C1, int L,
+                       const float* weight, const float* bias, float* delta, float* layer_weight, float* hole, void* stream);
+int nb200_depth_aa_minmax_f32(const float* x, long long n, float* minmax, void* stream);
+int nb200_depth_aa_prep_f16(const float* x, const float* minmax, int B, int H, int W, int ph1, int pw1, int Hh, int Wh,
+                            const float* weight, const float* bias, void* out, void* stream);
+int nb200_depth_aa_out_f32(const void* tok, const float* x, const float* minmax, int B, int H, int W, int ph1, int pw1, int Hh,
+                           int Wh, const float* weight, const float* bias, int clamp, float* out, void* stream);
+
 /* shifted-window attention core between the qkv and proj Linears
  * (torchvision swin_transformer.py:166-221), window 6x6, 6 heads.
  * qkv: three dense planes q | k | v, each [B][H][W][C] fp16 (how the engine's qkv GEMM writes them)
@@ -627,10 +653,13 @@ int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launc
  *                   pad, the ViT add + LayerNorm, the DPT upsample and the ZoeDepth bins head)
  *   bit 2 (on = 4): stem tail head se toimg sodconv (the waifu2x stem, tail and head convolutions, the SE block, to_image
  *                   and the SOD REBNCONV)
+ *   bit 3 (on = 8): rfprep rflast rf2 mlprep mlout holemask aaminmax aaprep aaout (the input and output stages of row_flow_v3,
+ *                   mlbw and depth_aa, the fused row_flow_v2 delta kernel and the hole mask of mask_mlbw_l2)
  * A line is `kind,name=value,name=value,...`: the launch's fields without its pointers, named where the host code writes
  * them.  Values are integers (flags 0 or 1) or fp32 values printed with 9 significant digits.  recorded_launches_named copies
  * the lines (NUL-terminated) like nb200_profile_dump; recorded_launches copies them without the names (`kind,value,...`, the
- * values in the same order).  Both fail if cap is too small. */
+ * values in the same order).  Both fail if cap is too small.  A few kinds record before their last argument check (zrelbias
+ * before its ldb check, mlout before its L check), so a refused call of those can leave a line for a launch that never ran. */
 int nb200_record_launches(int on);
 int nb200_recorded_launches(char* buf, size_t cap);
 int nb200_recorded_launches_named(char* buf, size_t cap);

@@ -173,6 +173,13 @@ SIGNATURES = {
     "nb200_to_image_f16": (c_int, [c_void_p] + [c_int] * 6 + [c_void_p, c_void_p]),
     "nb200_sod_conv_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p,
                                    c_int, c_int, c_int, c_int, c_void_p]),
+    "nb200_row_flow_prep_f16": (c_int, [c_void_p] + [c_int] * 5 + [c_void_p, c_void_p]),
+    "nb200_row_flow_last_conv_f32": (c_int, [c_void_p] + [c_int] * 5 + [c_void_p] * 4),
+    "nb200_mlbw_prep_f16": (c_int, [c_void_p] + [c_int] * 8 + [c_void_p] * 4),
+    "nb200_mlbw_out_f32": (c_int, [c_void_p, c_void_p] + [c_int] * 9 + [c_void_p] * 6),
+    "nb200_depth_aa_minmax_f32": (c_int, [c_void_p, ctypes.c_longlong, c_void_p, c_void_p]),
+    "nb200_depth_aa_prep_f16": (c_int, [c_void_p, c_void_p] + [c_int] * 7 + [c_void_p] * 4),
+    "nb200_depth_aa_out_f32": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "nb200_swin_mlp_fused_y_f16": (c_int, [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "nb200_record_launches": (c_int, [c_int]),

@@ -123,12 +123,15 @@ __global__ void __launch_bounds__(256) aa_out_kernel(const __half* __restrict__ 
 }  // namespace
 
 int aa_minmax(cudaStream_t st, const float* x, long long n, float* mm) {
+    if (rec_on(REC_STEREO)) rec_launch("aaminmax", {{"n", n}});
     aa_minmax_kernel<<<1, 1024, 0, st>>>(x, n, mm);
     NB_LAUNCHED();
     return 0;
 }
 int aa_prep(cudaStream_t st, const float* x, const float* mm, int B, int H, int W, int ph1, int pw1, int Hh, int Wh, const float* w_in,
             const float* b_in, __half* out) {
+    if (rec_on(REC_STEREO))
+        rec_launch("aaprep", {{"B", B}, {"H", H}, {"W", W}, {"ph1", ph1}, {"pw1", pw1}, {"Hh", Hh}, {"Wh", Wh}, {"norm", mm ? 1 : 0}});
     const long long total = (long long)B * Hh * Wh;
     aa_prep_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(x, mm, B, H, W, ph1, pw1, Hh, Wh, w_in, b_in, out);
     NB_LAUNCHED();
@@ -136,6 +139,9 @@ int aa_prep(cudaStream_t st, const float* x, const float* mm, int B, int H, int 
 }
 int aa_out(cudaStream_t st, const __half* tok, const float* x, const float* mm, int B, int H, int W, int ph1, int pw1, int Hh, int Wh,
            const float* w_out, const float* b_out, int clamp, float* out) {
+    if (rec_on(REC_STEREO))
+        rec_launch("aaout", {{"B", B}, {"H", H}, {"W", W}, {"ph1", ph1}, {"pw1", pw1}, {"Hh", Hh}, {"Wh", Wh}, {"norm", mm ? 1 : 0},
+                             {"clamp", clamp}});
     const long long total = (long long)B * H * W;
     aa_out_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(tok, x, mm, B, H, W, ph1, pw1, Hh, Wh, w_out, b_out, clamp, out);
     NB_LAUNCHED();

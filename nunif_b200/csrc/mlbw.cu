@@ -184,6 +184,8 @@ __global__ void __launch_bounds__(256) hole_mask_kernel(const float* __restrict_
 }  // namespace
 
 int hole_mask(cudaStream_t st, const float* logits, int B, int h, int w, int H, int W, float threshold, int mirror, float* out) {
+    if (rec_on(REC_STEREO))
+        rec_launch("holemask", {{"B", B}, {"h", h}, {"w", w}, {"H", H}, {"W", W}, {"mirror", mirror}, {"threshold", (double)threshold}});
     const long long n = (long long)B * H * W;
     // ATen area_pixel_compute_scale with align_corners: (float)(in - 1) / (out - 1), 0 for a one-pixel output
     const float sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
@@ -195,6 +197,8 @@ int hole_mask(cudaStream_t st, const float* logits, int B, int h, int w, int H, 
 
 int mlbw_prep(cudaStream_t st, const float* x, int B, int H, int W, int ph1, int pw1, int Hp, int Wt, int C1, const float* w_in,
               const float* b_in, __half* out) {
+    if (rec_on(REC_STEREO))
+        rec_launch("mlprep", {{"B", B}, {"H", H}, {"W", W}, {"ph1", ph1}, {"pw1", pw1}, {"Hp", Hp}, {"Wt", Wt}, {"C1", C1}});
     const long long total = (long long)B * Hp * Wt * C1;
     mlbw_prep_kernel<<<(unsigned)cdiv64(total, 256), 256, (size_t)(C1 * 28) * 4, st>>>(x, out, B, H, W, ph1, pw1, Hp, Wt, C1, w_in, b_in);
     NB_LAUNCHED();
@@ -203,6 +207,9 @@ int mlbw_prep(cudaStream_t st, const float* x, int B, int H, int W, int ph1, int
 
 int mlbw_out(cudaStream_t st, const __half* t, const __half* t0, int B, int H, int W, int ph1, int pw1, int Hp, int Wt, int C1, int L,
              const float* w_out, const float* b_out, float* delta, float* lw, float* hole) {
+    if (rec_on(REC_STEREO))
+        rec_launch("mlout", {{"B", B}, {"H", H}, {"W", W}, {"ph1", ph1}, {"pw1", pw1}, {"Hp", Hp}, {"Wt", Wt}, {"C1", C1}, {"L", L},
+                             {"hole", hole ? 1 : 0}});
     const long long total = (long long)B * H * W;
     const int NO = 2 * L + (hole ? 1 : 0);
     const size_t smem = (size_t)(NO * C1 * 9 + NO) * 4;

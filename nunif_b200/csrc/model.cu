@@ -991,3 +991,104 @@ extern "C" int nb200_se_block_f16(void* x, const float* w1, const float* b1, con
     cudaFreeAsync(ws, st);
     return rc;
 }
+
+// ---- test entry points of the learned stereo networks' input and output stages (the kernels a model forward launches between
+// its window-attention blocks): the geometry is what the model's forward computes, the weights host fp32 tensors in the PyTorch
+// layout.  Every check runs before the first CUDA call.
+static int stereo_geometry(int B, int H, int W, int ph1, int pw1, int Hp, int Wp) {
+    NB_CHECK(B > 0 && H > 0 && W > 0, "empty input");
+    NB_CHECK(ph1 >= 0 && pw1 >= 0, "negative leading pad");
+    NB_CHECK(ph1 + H <= Hp, "padded height < ph1 + H");
+    NB_CHECK(pw1 + W <= Wp, "padded width < pw1 + W");
+    return 0;
+}
+
+extern "C" int nb200_row_flow_prep_f16(const float* x, int B, int h, int w, int Hp, int Wt, void* out, void* stream) {
+    NB_CHECK(x && out, "null pointer");
+    if (stereo_geometry(B, h, w, 0, 0, Hp, 8 * Wt)) return 1;
+    return rf_prep((cudaStream_t)stream, x, B, h, w, Hp, Wt, (__half*)out);
+}
+
+extern "C" int nb200_row_flow_last_conv_f32(const void* x, int B, int Hp, int Wt, int h, int w, const float* weight, const float* bias,
+                                            float* delta, void* stream) {
+    NB_CHECK(x && weight && bias && delta, "null pointer");
+    if (stereo_geometry(B, h, w, 0, 0, Hp, 8 * Wt)) return 1;
+    const std::vector<float> wv(weight, weight + 72);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&wv}, &ws, p)) return 1;
+    const int rc = rf_last_conv(st, (const __half*)x, B, Hp, Wt, h, w, p[0], bias[0], delta);
+    cudaFreeAsync(ws, st);
+    return rc;
+}
+
+extern "C" int nb200_mlbw_prep_f16(const float* x, int B, int H, int W, int ph1, int pw1, int Hp, int Wt, int C1, const float* weight,
+                                   const float* bias, void* out, void* stream) {
+    NB_CHECK(x && weight && bias && out, "null pointer");
+    if (stereo_geometry(B, H, W, ph1, pw1, Hp, 8 * Wt)) return 1;
+    NB_CHECK(C1 > 0 && C1 <= 64, "C1 must be 1..64");
+    const std::vector<float> wv(weight, weight + (size_t)C1 * 27), bv(bias, bias + C1);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&wv, &bv}, &ws, p)) return 1;
+    const int rc = mlbw_prep(st, x, B, H, W, ph1, pw1, Hp, Wt, C1, p[0], p[1], (__half*)out);
+    cudaFreeAsync(ws, st);
+    return rc;
+}
+
+extern "C" int nb200_mlbw_out_f32(const void* t, const void* t0, int B, int H, int W, int ph1, int pw1, int Hp, int Wt, int C1, int L,
+                                  const float* weight, const float* bias, float* delta, float* layer_weight, float* hole, void* stream) {
+    NB_CHECK(t && t0 && weight && bias && delta && layer_weight, "null pointer");
+    if (stereo_geometry(B, H, W, ph1, pw1, Hp, 8 * Wt)) return 1;
+    NB_CHECK(C1 > 0 && C1 <= 64, "C1 must be 1..64");
+    NB_CHECK(L == 2 || L == 4, "L must be 2 or 4 (the kernel's instantiations)");
+    NB_CHECK(!hole || L == 2, "the hole head exists for L = 2 only");
+    const int NO = 2 * L + (hole ? 1 : 0);
+    // the kernel reads weights and biases as one [NO][C1][9] + [NO] block
+    std::vector<float> all(weight, weight + (size_t)NO * C1 * 9);
+    all.insert(all.end(), bias, bias + NO);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&all}, &ws, p)) return 1;
+    const int rc = mlbw_out(st, (const __half*)t, (const __half*)t0, B, H, W, ph1, pw1, Hp, Wt, C1, L, p[0], p[0] + NO * C1 * 9, delta,
+                            layer_weight, hole);
+    cudaFreeAsync(ws, st);
+    return rc;
+}
+
+extern "C" int nb200_depth_aa_minmax_f32(const float* x, long long n, float* minmax, void* stream) {
+    NB_CHECK(x && minmax, "null pointer");
+    NB_CHECK(n > 0, "empty input");
+    return aa_minmax((cudaStream_t)stream, x, n, minmax);
+}
+
+extern "C" int nb200_depth_aa_prep_f16(const float* x, const float* minmax, int B, int H, int W, int ph1, int pw1, int Hh, int Wh,
+                                       const float* weight, const float* bias, void* out, void* stream) {
+    NB_CHECK(x && weight && bias && out, "null pointer");
+    if (stereo_geometry(B, H, W, ph1, pw1, 2 * Hh, 2 * Wh)) return 1;
+    const std::vector<float> wv(weight, weight + 128), bv(bias, bias + 32);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&wv, &bv}, &ws, p)) return 1;
+    const int rc = aa_prep(st, x, minmax, B, H, W, ph1, pw1, Hh, Wh, p[0], p[1], (__half*)out);
+    cudaFreeAsync(ws, st);
+    return rc;
+}
+
+extern "C" int nb200_depth_aa_out_f32(const void* tok, const float* x, const float* minmax, int B, int H, int W, int ph1, int pw1, int Hh,
+                                      int Wh, const float* weight, const float* bias, int clamp, float* out, void* stream) {
+    NB_CHECK(tok && x && weight && bias && out, "null pointer");
+    if (stereo_geometry(B, H, W, ph1, pw1, 2 * Hh, 2 * Wh)) return 1;
+    const std::vector<float> wv(weight, weight + 128), bv(bias, bias + 4);
+    cudaStream_t st = (cudaStream_t)stream;
+    float* ws = nullptr;
+    std::vector<const float*> p;
+    if (upload_f32(st, {&wv, &bv}, &ws, p)) return 1;
+    const int rc = aa_out(st, (const __half*)tok, x, minmax, B, H, W, ph1, pw1, Hh, Wh, p[0], p[1], clamp ? 1 : 0, out);
+    cudaFreeAsync(ws, st);
+    return rc;
+}

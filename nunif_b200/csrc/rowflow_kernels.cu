@@ -55,6 +55,7 @@ __global__ void __launch_bounds__(256) rf_last_conv_kernel(const __half* __restr
 }
 
 int rf_prep(cudaStream_t st, const float* x, int B, int h, int w, int Hp, int Wt, __half* out) {
+    if (rec_on(REC_STEREO)) rec_launch("rfprep", {{"B", B}, {"h", h}, {"w", w}, {"Hp", Hp}, {"Wt", Wt}});
     const long long total = (long long)B * Hp * Wt * 4;
     rf_prep_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(x, out, B, h, w, Hp, Wt);
     NB_LAUNCHED();
@@ -62,6 +63,7 @@ int rf_prep(cudaStream_t st, const float* x, int B, int h, int w, int Hp, int Wt
 }
 
 int rf_last_conv(cudaStream_t st, const __half* x, int B, int Hp, int Wt, int h, int w, const float* wt72, float bias, float* delta) {
+    if (rec_on(REC_STEREO)) rec_launch("rflast", {{"B", B}, {"Hp", Hp}, {"Wt", Wt}, {"h", h}, {"w", w}});
     const long long total = (long long)B * h * w;
     rf_last_conv_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(x, delta, B, Hp, Wt, h, w, wt72, bias);
     NB_LAUNCHED();

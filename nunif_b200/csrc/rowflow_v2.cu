@@ -216,6 +216,7 @@ __global__ void __launch_bounds__(THREADS, 2) rf2_kernel(const float* __restrict
 int rf2_forward(cudaStream_t st, const void* params, const float* x, int B, int h, int w, float* delta) {
     NB_CHECK(B <= 65535 && cdiv(h, RF2_ROWS) <= 65535, "batch or height too large for the row_flow_v2 grid");
     if (ensure_dyn_smem((const void*)rf2_kernel, SMEM_BYTES)) return 1;
+    if (rec_on(REC_STEREO)) rec_launch("rf2", {{"B", B}, {"h", h}, {"w", w}});
     // algorithmic HBM traffic: x (3 planes) in, delta out
     ProfScope ps(st, PC_OTHER, (double)B * h * w * 16);
     dim3 grid(cdiv(w, RF2_T), cdiv(h, RF2_ROWS), B);

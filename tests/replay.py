@@ -208,6 +208,53 @@ MODELS = [
 ]
 
 
+# the learned stereo networks' own kernels (tests/test_gpu_kernel_replay_stereo.py): each on a 1080p landscape and a portrait
+# depth map, one frame at a time as iw3 runs them
+STEREO_FRAMES = ((1080, 1920), (1920, 1080))
+
+
+def _stereo(build):
+    def run():
+        net = build()
+        for h, w in STEREO_FRAMES:
+            net(_depth_input(1, h, w))
+    return run
+
+
+def _mlbw_inpaint():
+    """iw3 mlbw_l2_inpaint on a 1080p frame: the hole-mask MLBW warps each eye, the left one mirrored, then
+    postprocess_hole_mask and light_inpaint_v1 fill the holes."""
+    from nunif_b200.iw3 import MLBW, LightInpaintV1, MLBWInpaint
+    net = MLBWInpaint(LightInpaintV1(synth.light_inpaint_v1_state_dict(0), DEV), MLBW(synth.mask_mlbw_state_dict(0), DEV), DEV)
+    x = torch.rand(1, 3, 1080, 1920, generator=_gen(10)).to(DEV)
+    net.infer(x, synth.synth_depth(11, 1, 1080, 1920).to(DEV), 2.5, 0.4)
+
+
+def _depth_aa_infer():
+    from nunif_b200.iw3.depth_aa import DepthAA
+    from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
+    h, w = preprocess_size(1080, 1920)
+    DepthAA(synth.depth_aa_state_dict(0), DEV).infer(synth.synth_depth(8, 4, h, w).to(DEV))
+
+
+def _iw3(cls, sd):
+    def build():
+        from nunif_b200 import iw3
+        return getattr(iw3, cls)(sd(), DEV)
+    return build
+
+
+STEREO_MODELS = [
+    ("row_flow_v3", _stereo(_iw3("RowFlowV3", synth.row_flow_v3_state_dict))),          # iw3's default method
+    ("row_flow_v2", _stereo(_iw3("RowFlowV2", synth.row_flow_v2_state_dict))),
+    ("mlbw_l2", _stereo(_iw3("MLBW", lambda: synth.mlbw_state_dict(0, 2)))),
+    ("mlbw_l4", _stereo(_iw3("MLBW", lambda: synth.mlbw_state_dict(0, 4)))),
+    ("mask_mlbw_l2", _stereo(_iw3("MLBW", synth.mask_mlbw_state_dict))),                # the hole head
+    ("mlbw_l2_inpaint", _mlbw_inpaint),                     # postprocess_hole_mask with mirror 0 (right eye) and 1 (left eye)
+    ("depth_aa", _depth_aa_infer),                          # DepthAA.infer, as Depth-Anything's batch_infer calls it (392 x 686, B = 4)
+]
+
+
 # ------------------------------------------------------------------------------------------------------------ guarded buffers
 def guarded(n):
     """fp16 buffer of GUARD + n + GUARD elements, all SENTINEL."""

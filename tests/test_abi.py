@@ -111,15 +111,45 @@ def test_zoe_preprocess_size_host_rule_bit_exact(lib):
         assert (fh + 2 * p_h, fw + 2 * p_w, p_h, p_w) == (int(oh), int(ow), int(ph), int(pw)), (H, W)
 
 
-def test_launch_recorder_mask_bits_0_to_2(lib):
+def test_launch_recorder_mask_bits_0_to_3(lib):
     """nb200_record_launches takes a mask of the recorded kinds (bit 0: GEMM / attention / Swin, bit 1: the kernels between
-    them, bit 2: the waifu2x stem / tail / head convolutions, SE, to_image and the SOD REBNCONV) and refuses other bits; host
-    only, no device needed."""
-    for on in (1, 2, 3, 4, 7, 0):
+    them, bit 2: the waifu2x stem / tail / head convolutions, SE, to_image and the SOD REBNCONV, bit 3: the stereo networks'
+    input / output stages, row_flow_v2 and the hole mask) and refuses other bits; host only, no device needed."""
+    for on in (1, 2, 3, 4, 7, 8, 15, 0):
         assert lib.nb200_record_launches(on) == 0, on
-    for on in (8, 15):
+    for on in (16, 31):
         assert lib.nb200_record_launches(on) != 0, on
         assert b"unknown recorder bits" in lib.nb200_last_error()
+    buf = ctypes.create_string_buffer(16)
+    assert lib.nb200_recorded_launches(buf, 16) == 0 and buf.value == b""
+
+
+def test_stereo_entry_points_refuse_bad_geometry(lib):
+    """The stereo test entry points refuse a padded grid that does not hold the image, an L without an instantiation and a hole
+    head with L != 2 before their first CUDA call: dummy host pointers, no device needed, and nothing is recorded."""
+    d = ctypes.create_string_buffer(4096)
+    cases = [
+        (lambda: lib.nb200_row_flow_prep_f16(d, 1, 13, 16, 12, 2, d, None), b"padded height"),            # Hp < h
+        (lambda: lib.nb200_row_flow_prep_f16(d, 1, 12, 17, 12, 2, d, None), b"padded width"),             # 8 Wt < w
+        (lambda: lib.nb200_row_flow_last_conv_f32(d, 1, 12, 2, 12, 17, d, d, d, None), b"padded width"),
+        (lambda: lib.nb200_row_flow_last_conv_f32(d, 0, 12, 2, 12, 16, d, d, d, None), b"empty input"),
+        (lambda: lib.nb200_mlbw_prep_f16(d, 1, 4, 16, 1, 1, 4, 3, 8, d, d, d, None), b"padded height"),   # ph1 + H > Hp
+        (lambda: lib.nb200_mlbw_prep_f16(d, 1, 4, 16, 1, 1, 6, 2, 8, d, d, d, None), b"padded width"),    # pw1 + W > 8 Wt
+        (lambda: lib.nb200_mlbw_prep_f16(d, 1, 4, 16, -1, 0, 6, 4, 8, d, d, d, None), b"negative leading pad"),
+        (lambda: lib.nb200_mlbw_out_f32(d, d, 1, 4, 16, 1, 8, 6, 2, 8, 2, d, d, d, d, None, None), b"padded width"),
+        (lambda: lib.nb200_mlbw_out_f32(d, d, 1, 4, 16, 1, 8, 6, 4, 8, 3, d, d, d, d, None, None), b"L must be 2 or 4"),
+        (lambda: lib.nb200_mlbw_out_f32(d, d, 1, 4, 16, 1, 8, 6, 4, 16, 4, d, d, d, d, d, None), b"hole head"),
+        (lambda: lib.nb200_depth_aa_minmax_f32(d, 0, d, None), b"empty input"),
+        (lambda: lib.nb200_depth_aa_prep_f16(d, None, 1, 16, 16, 8, 0, 8, 8, d, d, d, None), b"padded height"),   # ph1 + H > 2 Hh
+        (lambda: lib.nb200_depth_aa_out_f32(d, d, None, 1, 16, 17, 0, 0, 8, 8, d, d, 1, d, None), b"padded width"),
+    ]
+    assert lib.nb200_record_launches(8) == 0
+    try:
+        for i, (call, msg) in enumerate(cases):
+            assert call() != 0, i
+            assert msg in lib.nb200_last_error(), (i, lib.nb200_last_error())
+    finally:
+        lib.nb200_record_launches(0)
     buf = ctypes.create_string_buffer(16)
     assert lib.nb200_recorded_launches(buf, 16) == 0 and buf.value == b""
 
