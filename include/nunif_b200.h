@@ -574,6 +574,25 @@ enum { NB200_TRC_PQ = 16, NB200_TRC_HLG = 18, NB200_SDR_BT709 = 0, NB200_SDR_BT6
 int nb200_hdr2sdr(const uint16_t* x, int B, int H, int W, int trc, int colorspace, const double* params_host,
                   int out_float, void* out, void* stream);
 
+/* Film grain (waifu2x --grain: waifu2x/ui_utils.py:58-61 images, :167-175 video) through nunif/utils/rgb_noise.py.
+ * Noise: each normal is Philox4x32-10 keyed by seed at the counter (element, 2 * channel + field, frame, offset), turned
+ * into N(0, 1) by Box-Muller; field 0 = the full-resolution field, field 1 = level 2's (H / 2) x (W / 2) field.  A different
+ * sample from the distribution of the reference's torch.randn draws, not their bits.
+ * nb200_rgb_noise: rgb_noise_like (rgb_noise.py:5-17) -> out [B][C][H][W] fp32; frame b of the batch uses frame word b.
+ *   level 1: the full field; level 2: 0.5 * full + 0.5 * half upsampled by F.interpolate's nearest rule (H, W >= 2). */
+int nb200_rgb_noise(uint64_t seed, uint32_t offset, int level, int B, int C, int H, int W, float* out, void* stream);
+/* nb200_apply_rgb_noise: apply_rgb_noise (rgb_noise.py:20-36) of rgb [B][C][H][W] fp32, in the reference's fp32 op order.
+ *   noise [B][C][H][W], or null: frame b's noise is nb200_rgb_noise(seed, offset + b, level) of that frame alone.
+ *   buffer [C][H][W], or null: the video path's temporal noise buffer (ui_utils.py:167-175), advanced over the B frames in
+ *   order, b = b * (1 - speed) + n * speed, and the blended buffer applied; buffer_reset = 1: frame 0 copies its noise into
+ *   the buffer (the reference's first frame and every frame-shape change).
+ *   params_host = {strength, gamma, light_decay_strength, speed} as the Python floats.
+ *   out_bits = 0: out [B][C][H][W] fp32; 8 / 16: out [B][H][W][3] uint8 / uint16, (y * 255 | 65535).round_() as
+ *   from_tensor (nunif/utils/video.py:236-245) makes the encoder's frame (C must be 3). */
+int nb200_apply_rgb_noise(const float* rgb, int B, int C, int H, int W, const float* noise, uint64_t seed, uint32_t offset,
+                          int level, float* buffer, int buffer_reset, const double* params_host, int light_decay, int out_bits,
+                          void* out, void* stream);
+
 /* DepthAnything batch_preprocess (iw3/depth_anything_model.py:69-110): size rule (host,
  * integers) and the fused antialiased-bilinear resize + clamp + ImageNet normalise:
  * x [B][3][H][W] fp32 in [0,1] -> out [B][3][new_h][new_w] fp32. */

@@ -132,6 +132,19 @@ __device__ __forceinline__ uint32_t order_key(float f) {
 }
 __device__ __forceinline__ float order_key_inv(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
 
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11): four 32-bit words that are a pure
+// function of a 128-bit counter and a 64-bit key, so any element of a random field can be recomputed by any thread
+__host__ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+        const uint64_t p0 = (uint64_t)0xD2511F53u * c.x, p1 = (uint64_t)0xCD9E8D57u * c.z;
+        c = make_uint4((uint32_t)(p1 >> 32) ^ c.y ^ k.x, (uint32_t)p1, (uint32_t)(p0 >> 32) ^ c.w ^ k.y, (uint32_t)p0);
+        k.x += 0x9E3779B9u;
+        k.y += 0xBB67AE85u;
+    }
+    return c;
+}
+
 // bicubic weight with A = -0.5 (ATen's antialiased bicubic filter)
 __device__ __forceinline__ float cubic_aa(float x) {
     const float a = -0.5f;

@@ -18,6 +18,10 @@ submission order (possibly empty) - the calling convention of ``FrameCallbackPoo
 ``hdr2sdr`` is the reference's HDR input stage (video.py:309-416, applied by input_reformatter :1025-1041 when
 ``use_hdr2sdr`` holds): PQ / HLG BT.2020 rgb48 frames tone-mapped to BT.709 / BT.601 SDR by csrc/hdr2sdr.cu.
 ``FrameBatchPipeline(..., hdr2sdr=(color_trc, output_colorspace))`` runs it as the uint16 -> float conversion of each batch.
+
+``FrameBatchPipeline(..., grain=(strength, speed[, seed]))`` is waifu2x's video film grain (waifu2x/ui_utils.py:167-175):
+the float -> uint8 / uint16 conversion of each callback output becomes the fused temporal grain + quantise kernel
+(csrc/rgb_noise.cu), whose noise buffer stays on the device and advances over the emitted frames in ticket order.
 """
 import ctypes
 
@@ -25,6 +29,7 @@ import torch
 
 from .. import _lib
 from ..iw3.frames import hwc_to_chw_float, chw_float_to_hwc
+from .rgb_noise import TemporalGrain
 
 COLORSPACE_BT2020 = 9
 COLOR_TRC_SMPTE2084 = 16            # PQ (HDR10)
@@ -92,8 +97,15 @@ class _Slot:
 
 
 class FrameBatchPipeline:
-    def __init__(self, frame_callback, batch_size, device="cuda:0", depth=3, use_16bit=False, copy_output=True, hdr2sdr=None):
+    def __init__(self, frame_callback, batch_size, device="cuda:0", depth=3, use_16bit=False, copy_output=True, hdr2sdr=None,
+                 grain=None):
         assert batch_size > 0 and depth >= 2
+        # (strength, speed[, seed]): add temporal film grain to every emitted frame as it is converted for the encoder
+        if grain is not None:
+            if len(grain) not in (2, 3):
+                raise ValueError("grain must be (strength, speed) or (strength, speed, seed)")
+            grain = TemporalGrain(*grain)
+        self.grain = grain
         # (color_trc, output_colorspace): tone-map each uint16 batch to SDR (hdr2sdr(..., output="float")) in place of the
         # plain uint16 -> float conversion, so the callback receives SDR frames
         if hdr2sdr is not None:
@@ -134,6 +146,10 @@ class FrameBatchPipeline:
         frame = torch.as_tensor(frame)
         assert frame.ndim == 3 and frame.shape[2] == 3 and frame.dtype == self.dtype, "HWC uint8/uint16 frame expected"
         slot = self.slots[self.head]
+        if self.fill > 0 and tuple(frame.shape) != tuple(slot.h_in.shape[1:]):
+            # the frame size changed inside a batch: submit the frames of the old size as a partial batch
+            self._launch(slot, self.fill)
+            slot = self.slots[self.head]
         if self.fill == 0:
             if self.head in self.inflight:           # ring is full: the oldest ticket must be returned first
                 out = self._collect(block=True)
@@ -174,7 +190,10 @@ class FrameBatchPipeline:
                 x = hdr2sdr(slot.d_in[:n], *self.hdr2sdr, output="float")
             y = self.frame_callback(x)
             if y is not None and y.numel() > 0:
-                u = chw_float_to_hwc(y, use_16bit=self.bits == 16)
+                if self.grain is None:
+                    u = chw_float_to_hwc(y, use_16bit=self.bits == 16)
+                else:
+                    u = self.grain(y, dtype=self.dtype)
                 slot.n_out = u.shape[0]
                 if slot.h_out is None or tuple(slot.h_out.shape[1:]) != tuple(u.shape[1:]) or slot.h_out.shape[0] < u.shape[0]:
                     slot.h_out = torch.empty((max(u.shape[0], self.batch_size),) + tuple(u.shape[1:]), dtype=self.dtype).pin_memory()
