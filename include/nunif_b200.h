@@ -374,6 +374,27 @@ int nb200_mapper_apply(const float* depth, long long n, const nb200_mapper* mapp
 int nb200_minmax_mapper(const float* depth, int B, int n_per_frame, const nb200_mapper* mapper_host,
                         float* out, float* minmax_out /* [B][2] or NULL */, void* stream);
 
+/* Depth export (iw3/utils.py:1323-1328 images, :1378-1382 video, then iw3/base_depth_model.py:203-204
+ * save_normalized_depth): depth [B][1][h][w] normalised -> out uint16 [B][H][W] = (0xffff * clamp(d', 0, 1)) truncated,
+ * where d' is the mapper applied to each source pixel (mapper_host NULL or 0 stages: none), then, with fit != 0, the
+ * antialiased bilinear resize to H x W (align_corners 1: F.interpolate(..., align_corners=True) of the image path,
+ * 0: TF.resize of the video path).  fit = 0 ignores H, W and align_corners and writes h x w. */
+int nb200_depth_export_u16(const float* depth, int B, int h, int w, const nb200_mapper* mapper_host, int fit, int H, int W,
+                           int align_corners, uint16_t* out, void* stream);
+/* Depth import (iw3/base_depth_model.py:225-232 load_depth) of B decoded depth maps, channels interleaved as the
+ * decoder leaves them, of element type dtype:
+ *   NB200_DEPTH_U8   uint8, C = 1..4      NB200_DEPTH_U16  uint16, C = 1   (PNG "L" / "RGB" / "RGBA", "I;16")
+ *   NB200_DEPTH_I32  int32, C = 1         NB200_DEPTH_F32  float32, C = 1  (Pillow modes "I" and "F")
+ * Integer channels are divided by 0xffff (8-bit maps too) and clamped to [0, 1]; float maps are taken as they are.  The
+ * channels are averaged (alpha included), and with has_range != 0 (the iw3_min_depth_value / iw3_max_depth_value text
+ * keys) d * (float)(hi - lo) + (float)lo.  out fp32 [B][1][H][W]. */
+#define NB200_DEPTH_U8 1
+#define NB200_DEPTH_U16 2
+#define NB200_DEPTH_I32 3
+#define NB200_DEPTH_F32 4
+int nb200_depth_import(const void* src, int dtype, int C, int B, int H, int W, double lo, double hi, int has_range,
+                       float* out, void* stream);
+
 /* iw3/anaglyph.py:51-92 on already-warped eyes: l,r,out [B][3][H][W] */
 int nb200_anaglyph_dubois(const float* l, const float* r, int B, int H, int W, int clip_before,
                           float* out, void* stream);

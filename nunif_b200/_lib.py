@@ -148,6 +148,9 @@ SIGNATURES = {
     "nb200_depth_mapper": (c_int, [c_void_p, ctypes.c_longlong, c_float, c_void_p, c_void_p]),
     "nb200_mapper_apply": (c_int, [c_void_p, ctypes.c_longlong, ctypes.POINTER(Mapper), c_void_p, c_void_p]),
     "nb200_minmax_mapper": (c_int, [c_void_p, c_int, c_int, ctypes.POINTER(Mapper), c_void_p, c_void_p, c_void_p]),
+    "nb200_depth_export_u16": (c_int, [c_void_p, c_int, c_int, c_int, ctypes.POINTER(Mapper), c_int, c_int, c_int, c_int, c_void_p,
+                                       c_void_p]),
+    "nb200_depth_import": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_double, c_int, c_void_p, c_void_p]),
     "nb200_anaglyph_dubois": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_conv_gemm_f16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int,
                                     c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,

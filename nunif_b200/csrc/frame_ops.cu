@@ -5,6 +5,7 @@
 //     one fused kernel over the output (the reference makes 1 resize + 3 elementwise passes).
 // All HBM-bound: the conversions move 3+12 B/px, the preprocess reads the 24.9 MB fp32 frame once.
 #include "common.cuh"
+#include "aa_resize.cuh"
 #include <cmath>
 #include "../../include/nunif_b200.h"
 
@@ -48,14 +49,11 @@ struct DaPrepParams {
     int B, H, W, oh, ow;  // oh x ow = resized frame; the output is (oh + 2*pad_h) x (ow + 2*pad_w), reflection padded
     int pad_h, pad_w;
     float sy, sx;         // in/out scale (align_corners=False)
-    float supy, supx;     // filter support: scale if scale >= 1 else 1
-    float invy, invx;     // 1/scale if scale >= 1 else 1
     float mean[3], stdv[3];
     int plain;            // 1: the resize alone (no clamp, no normalisation)
 };
 
-// ATen UpSampleKernel (_upsample_bilinear2d_aa): centre = scale*(i+0.5); taps [xmin, xmin+xsize);
-// w_j = tri((j + xmin - centre + 0.5) * invscale) / sum.  Horizontal pass first (fp32), then vertical.
+// ATen UpSampleKernel (_upsample_bilinear2d_aa, csrc/aa_resize.cuh), align_corners=False.
 __global__ void __launch_bounds__(128) da_preprocess_kernel(DaPrepParams p) {
     const int px = blockIdx.x * blockDim.x + threadIdx.x, py = blockIdx.y, b = blockIdx.z;
     const int OW = p.ow + 2 * p.pad_w, OH = p.oh + 2 * p.pad_h;
@@ -65,28 +63,12 @@ __global__ void __launch_bounds__(128) da_preprocess_kernel(DaPrepParams p) {
     int ox = px - p.pad_w, oy = py - p.pad_h;
     if (p.pad_w > 0) { const int m = 2 * (p.ow - 1); ox = ((ox % m) + m) % m; ox = ox < p.ow ? ox : m - ox; }
     if (p.pad_h > 0) { const int m = 2 * (p.oh - 1); oy = ((oy % m) + m) % m; oy = oy < p.oh ? oy : m - oy; }
-    // the centre is a rounded fp32 product in ATen; without _rn the compiler fuses it into the tap-offset subtraction
-    // below (fma), which shifts every weight by up to 1e-5
-    const float cy = __fmul_rn(p.sy, (float)oy + 0.5f), cx = __fmul_rn(p.sx, (float)ox + 0.5f);
-    const int ymin = max(0, (int)(cy - p.supy + 0.5f)), ysize = min(p.H, (int)(cy + p.supy + 0.5f)) - ymin;
-    const int xmin = max(0, (int)(cx - p.supx + 0.5f)), xsize = min(p.W, (int)(cx + p.supx + 0.5f)) - xmin;
-    float wxs = 0.f, wys = 0.f;
-    for (int j = 0; j < xsize; ++j) wxs += fmaxf(0.f, 1.f - fabsf(((float)(j + xmin) - cx + 0.5f) * p.invx));
-    for (int j = 0; j < ysize; ++j) wys += fmaxf(0.f, 1.f - fabsf(((float)(j + ymin) - cy + 0.5f) * p.invy));
+    const AaTaps ty = aa_taps(p.sy, oy, p.H), tx = aa_taps(p.sx, ox, p.W);
+    const float sum_y = aa_weight_sum(ty), sum_x = aa_weight_sum(tx);
     const size_t plane = (size_t)p.H * p.W;
     for (int c = 0; c < 3; ++c) {
         const float* src = p.x + ((size_t)b * 3 + c) * plane;
-        float acc = 0.f;
-        for (int jy = 0; jy < ysize; ++jy) {
-            const float wy = fmaxf(0.f, 1.f - fabsf(((float)(jy + ymin) - cy + 0.5f) * p.invy)) / wys;
-            const float* row = src + (size_t)(ymin + jy) * p.W + xmin;
-            float h = 0.f;
-            for (int jx = 0; jx < xsize; ++jx) {
-                const float wx = fmaxf(0.f, 1.f - fabsf(((float)(jx + xmin) - cx + 0.5f) * p.invx)) / wxs;
-                h += wx * __ldg(row + jx);
-            }
-            acc += wy * h;
-        }
+        float acc = aa_sample(ty, tx, sum_y, sum_x, [&](int y, int x) { return __ldg(src + (size_t)y * p.W + x); });
         if (!p.plain) {
             acc = clamp01(acc);                                                // depth_anything_model.py:104 / zoedepth_model.py:75
             acc = __fdiv_rn(__fsub_rn(acc, p.mean[c]), p.stdv[c]);             // :107-109 / :78-80
@@ -191,10 +173,6 @@ static int launch_prep(const float* x, int B, int H, int W, int frame_h, int fra
     p.x = x; p.out = out; p.B = B; p.H = H; p.W = W; p.oh = frame_h; p.ow = frame_w; p.pad_h = pad_h; p.pad_w = pad_w;
     p.sy = (float)H / (float)frame_h;   // area_pixel_compute_scale, align_corners=False, no scale_factor given
     p.sx = (float)W / (float)frame_w;
-    p.supy = p.sy >= 1.f ? p.sy : 1.f;
-    p.supx = p.sx >= 1.f ? p.sx : 1.f;
-    p.invy = p.sy >= 1.f ? 1.f / p.sy : 1.f;
-    p.invx = p.sx >= 1.f ? 1.f / p.sx : 1.f;
     for (int c = 0; c < 3; ++c) { p.mean[c] = mean[c]; p.stdv[c] = stdv[c]; }
     cudaStream_t st = (cudaStream_t)stream;
     const int OH = frame_h + 2 * pad_h, OW = frame_w + 2 * pad_w;

@@ -22,6 +22,7 @@
 //  All fp32 arithmetic that feeds floor()/compare uses non-contracted _rn intrinsics so
 //  results are bit-identical to the reference's op-by-op evaluation.
 #include "common.cuh"
+#include "aa_resize.cuh"
 #include "../../include/nunif_b200.h"
 #include <math.h>
 
@@ -46,67 +47,38 @@ struct FwParams {
     const float4* coltab;    // per output column: {xmin (as int bits), w0, w1, w2} of the AA resize (upsampling only), or null
 };
 
-__device__ __forceinline__ float tri(float x) {
-    x = fabsf(x);
-    return x < 1.f ? 1.f - x : 0.f;
-}
-
 // ATen upsample_bilinear2d_aa (align_corners=True only changes the scale): one output
 // sample at (y, X); horizontal pass first, then vertical (separable, fp32).
 __device__ float aa_bilinear_sample(const float* __restrict__ src, int h, int w, float scale_y, float scale_x,
                                     int y, int X) {
-    const float sup_y = scale_y >= 1.f ? scale_y : 1.f, inv_y = scale_y >= 1.f ? 1.f / scale_y : 1.f;
-    const float sup_x = scale_x >= 1.f ? scale_x : 1.f, inv_x = scale_x >= 1.f ? 1.f / scale_x : 1.f;
-    const float cy = __fmul_rn(scale_y, (float)y + 0.5f), cx = __fmul_rn(scale_x, (float)X + 0.5f);
-    const int ymin = max((int)(cy - sup_y + 0.5f), 0);
-    const int ysize = min((int)(cy + sup_y + 0.5f), h) - ymin;
-    const int xmin = max((int)(cx - sup_x + 0.5f), 0);
-    const int xsize = min((int)(cx + sup_x + 0.5f), w) - xmin;
-    float tx = 0.f, ty = 0.f;
-    for (int j = 0; j < xsize; ++j) tx += tri(((float)(j + xmin) - cx + 0.5f) * inv_x);
-    for (int i = 0; i < ysize; ++i) ty += tri(((float)(i + ymin) - cy + 0.5f) * inv_y);
-    float acc = 0.f;
-    for (int i = 0; i < ysize; ++i) {
-        const float* row = src + (size_t)(ymin + i) * w + xmin;
-        float hs = 0.f;
-        for (int j = 0; j < xsize; ++j) {
-            float wx = tri(((float)(j + xmin) - cx + 0.5f) * inv_x) / tx;
-            hs += __ldg(row + j) * wx;
-        }
-        float wy = tri(((float)(i + ymin) - cy + 0.5f) * inv_y) / ty;
-        acc += hs * wy;
-    }
-    return acc;
+    const AaTaps ty = aa_taps(scale_y, y, h), tx = aa_taps(scale_x, X, w);
+    return aa_sample(ty, tx, aa_weight_sum(ty), aa_weight_sum(tx),
+                     [&](int yy, int xx) { return __ldg(src + (size_t)yy * w + xx); });
 }
 
 // Horizontal taps of the AA resize depend only on the output column: computed once per call (upsampling: <= 3 taps).
 __global__ void depth_coltab_kernel(float4* __restrict__ tab, int W, int w, float scale_x) {
     const int X = blockIdx.x * blockDim.x + threadIdx.x;
     if (X >= W) return;
-    const float cx = __fmul_rn(scale_x, (float)X + 0.5f);
-    const int xmin = max((int)(cx - 1.0f + 0.5f), 0);
-    const int xsize = min((int)(cx + 1.0f + 0.5f), w) - xmin;
-    float wv[3] = {0.f, 0.f, 0.f}, tx = 0.f;
-    for (int j = 0; j < xsize && j < 3; ++j) { wv[j] = tri((float)(j + xmin) - cx + 0.5f); tx += wv[j]; }
-    tab[X] = make_float4(__int_as_float(xmin), wv[0] / tx, wv[1] / tx, wv[2] / tx);
+    const AaTaps tx = aa_taps(scale_x, X, w);
+    float wv[3] = {0.f, 0.f, 0.f}, sum = 0.f;
+    for (int j = 0; j < tx.size && j < 3; ++j) { wv[j] = aa_weight(tx, j); sum += wv[j]; }
+    tab[X] = make_float4(__int_as_float(tx.min), wv[0] / sum, wv[1] / sum, wv[2] / sum);
 }
 
 // same arithmetic as aa_bilinear_sample for the upsampling case, with the horizontal taps taken from the table
 __device__ __forceinline__ float aa_bilinear_sample_tab(const float* __restrict__ src, int h, int w, float scale_y, int y,
                                                         const float4 ct) {
-    const float cy = __fmul_rn(scale_y, (float)y + 0.5f);
-    const int ymin = max((int)(cy - 1.0f + 0.5f), 0);
-    const int ysize = min((int)(cy + 1.0f + 0.5f), h) - ymin;
+    const AaTaps ty = aa_taps(scale_y, y, h);
     const int xmin = __float_as_int(ct.x);
-    float ty = 0.f;
-    for (int i = 0; i < ysize; ++i) ty += tri((float)(i + ymin) - cy + 0.5f);
+    const float sum_y = aa_weight_sum(ty);
     float acc = 0.f;
-    for (int i = 0; i < ysize; ++i) {
-        const float* row = src + (size_t)(ymin + i) * w + xmin;
+    for (int i = 0; i < ty.size; ++i) {
+        const float* row = src + (size_t)(ty.min + i) * w + xmin;
         float hs = __ldg(row) * ct.y;
         if (xmin + 1 < w) hs += __ldg(row + 1) * ct.z;
         if (xmin + 2 < w) hs += __ldg(row + 2) * ct.w;
-        acc += hs * (tri((float)(i + ymin) - cy + 0.5f) / ty);
+        acc += hs * (aa_weight(ty, i) / sum_y);
     }
     return acc;
 }

@@ -162,9 +162,12 @@ class BaseDepthModel:
                 self.reset_ema()
         return out
 
-    # ---- depth image files (:196-249): host-side PNG I/O, 16-bit like the reference
+    # ---- depth image files (:196-249): host-side PNG I/O, 16-bit like the reference.  The device path: save a uint16
+    # map from depth_io.export_depth_u16; load_depth(..., device=) decodes on the GPU (depth_io.import_depth).
     @staticmethod
     def save_normalized_depth(depth, file_path, png_info={}, min_depth_value=None, max_depth_value=None):
+        """``depth``: normalised fp32 (1,h,w), quantised here as the reference does, or the uint16 (h,w) map of
+        ``export_depth_u16``, written as is."""
         from PIL import Image
         from PIL.PngImagePlugin import PngInfo
         info = dict(png_info)
@@ -175,11 +178,16 @@ class BaseDepthModel:
         meta = PngInfo()
         for k, v in info.items():
             meta.add_text(k, str(v))
-        px = (0xffff * torch.clamp(depth, 0, 1)).to(torch.uint16).squeeze(0).cpu().numpy()
+        if depth.dtype == torch.uint16:
+            px = depth.cpu().numpy()
+        else:
+            px = (0xffff * torch.clamp(depth, 0, 1)).to(torch.uint16).squeeze(0).cpu().numpy()
         Image.fromarray(px).save(file_path, pnginfo=meta)
 
     @staticmethod
-    def load_depth(file_path):
+    def load_depth(file_path, device=None):
+        """-> (depth (1,H,W) fp32, PNG text + filename).  With ``device`` the decoded map is uploaded as is and
+        converted there (nb200_depth_import); without, on the host."""
         import numpy as np
         from PIL import Image
         with Image.open(file_path) as im:
@@ -190,6 +198,10 @@ class BaseDepthModel:
             lo, hi = float(text["iw3_min_depth_value"]), float(text["iw3_max_depth_value"])
         except (KeyError, ValueError, TypeError):
             lo = hi = None
+        text["filename"] = file_path
+        if device is not None:
+            from .depth_io import import_depth
+            return import_depth(arr, device, (lo, hi) if lo is not None else None), text
         depth = torch.from_numpy(arr.astype(np.float32))
         depth = depth.unsqueeze(0) if depth.ndim == 2 else depth.permute(2, 0, 1)
         if arr.dtype != np.float32:
@@ -198,5 +210,4 @@ class BaseDepthModel:
             depth = depth.mean(dim=0, keepdim=True)
         if lo is not None and hi is not None:
             depth = depth * (hi - lo) + lo
-        text["filename"] = file_path
         return depth, text

@@ -23,6 +23,7 @@ from .row_flow import apply_divergence_nn_LR
 from .postprocess import postprocess_image, resize_bicubic_aa, rot90
 from .convergence_estimator import ConvergenceEstimator
 from ..nunif import autocrop as _autocrop
+from .export import export_images, process_config_images  # noqa: F401
 
 _WARP = {"grid_sample": "backward", "backward": "backward", "forward": "forward", "forward_fill": "forward"}
 
