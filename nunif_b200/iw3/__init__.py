@@ -31,3 +31,4 @@ from .forward_inpaint import ForwardInpaint, LightInpaintV1  # noqa: F401
 from .mlbw_inpaint import MLBWInpaint  # noqa: F401
 from .convergence_estimator import ConvergenceEstimator, SODV1  # noqa: F401
 from .utils import apply_divergence, process_image, preprocess_image, apply_rgbd, debug_depth_image  # noqa: F401
+from .video import bind_single_frame_callback, bind_batch_frame_callback  # noqa: F401
