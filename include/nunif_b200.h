@@ -622,6 +622,11 @@ int nb200_da_preprocess_size(int H, int W, int lower_bound, int max_aspect_ratio
 int nb200_da_preprocess(const float* x, int B, int H, int W, int new_h, int new_w, float* out,
                         void* stream);
 
+/* iw3's NULL depth model (iw3/null_depth_model.py:17-21 NullDepth.forward): F.interpolate(x, (R, R), mode="bilinear",
+ * align_corners=False) then x.mean(dim=1, keepdim=True) in one pass, with the arithmetic of ATen's CUDA kernels:
+ * x [B][3][H][W] fp32 -> out [B][1][R][R] fp32.  out must not alias x. */
+int nb200_null_depth(const float* x, int B, int H, int W, int R, float* out, void* stream);
+
 /* ZoeDepth batch_preprocess (iw3/zoedepth_model.py:30-85): size rule (host integers) and the fused
  * antialiased resize + reflection pad (nunif/modules/reflection_pad2d.py:57-68) + clamp + normalise:
  * x [B][3][H][W] -> out [B][3][frame_h + 2*pad_h][frame_w + 2*pad_w] (== new_h x new_w in landscape). */

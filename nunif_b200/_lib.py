@@ -113,6 +113,7 @@ SIGNATURES = {
                                       c_void_p, c_int, ctypes.POINTER(c_double), c_int, c_int, c_void_p, c_void_p]),
     "nb200_da_preprocess_size": (c_int, [c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),
     "nb200_da_preprocess": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "nb200_null_depth": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_zoe_preprocess_size": (c_int, [c_int] * 5 + [ctypes.POINTER(c_int)] * 6),
     "nb200_zoe_preprocess": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_anaglyph": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),

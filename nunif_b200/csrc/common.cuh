@@ -145,6 +145,29 @@ __host__ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
     return c;
 }
 
+// ATen's CUDA bilinear resize (align_corners=False, no antialias, output size given), UpSampleBilinear2d.cu: the scale is
+// (float)in / out, the source index scale * (dst + 0.5) - 0.5 is one FMA there, clamped at 0, and so is the first product
+// of each lerp pair.  Used by the sod_v1 resizes (sod.cu) and the NULL depth model (null_depth.cu).
+struct BilTap {
+    int i0, i1;
+    float l0, l1;
+};
+
+__device__ __forceinline__ BilTap bil_tap(float scale, int dst, int in_size) {
+    float r = fmaf(scale, (float)dst + 0.5f, -0.5f);
+    r = r < 0.f ? 0.f : r;
+    BilTap t;
+    t.i0 = (int)r;
+    t.i1 = t.i0 + ((t.i0 < in_size - 1) ? 1 : 0);
+    t.l1 = r - (float)t.i0;
+    t.l0 = 1.f - t.l1;
+    return t;
+}
+
+__device__ __forceinline__ float bil_mix(const BilTap& ty, const BilTap& tx, float v00, float v01, float v10, float v11) {
+    return fmaf(ty.l0, fmaf(tx.l0, v00, tx.l1 * v01), ty.l1 * fmaf(tx.l0, v10, tx.l1 * v11));
+}
+
 // bicubic weight with A = -0.5 (ATen's antialiased bicubic filter)
 __device__ __forceinline__ float cubic_aa(float x) {
     const float a = -0.5f;

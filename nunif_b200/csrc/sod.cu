@@ -19,30 +19,6 @@
 
 namespace nb200 {
 
-// ---------------------------------------------------------------------------------------------
-// ATen's bilinear resize (align_corners=False, no antialias), UpSampleBilinear2d.cu: the source index
-// scale * (dst + 0.5) - 0.5 is one FMA there, and so is the first product of each lerp pair.
-// ---------------------------------------------------------------------------------------------
-struct BilTap {
-    int i0, i1;
-    float l0, l1;
-};
-
-__device__ __forceinline__ BilTap bil_tap(float scale, int dst, int in_size) {
-    float r = fmaf(scale, (float)dst + 0.5f, -0.5f);
-    r = r < 0.f ? 0.f : r;
-    BilTap t;
-    t.i0 = (int)r;
-    t.i1 = t.i0 + ((t.i0 < in_size - 1) ? 1 : 0);
-    t.l1 = r - (float)t.i0;
-    t.l0 = 1.f - t.l1;
-    return t;
-}
-
-__device__ __forceinline__ float bil_mix(const BilTap& ty, const BilTap& tx, float v00, float v01, float v10, float v11) {
-    return fmaf(ty.l0, fmaf(tx.l0, v00, tx.l1 * v01), ty.l1 * fmaf(tx.l0, v10, tx.l1 * v11));
-}
-
 // rgb [B][3][H][W], depth [B][1][h][w] -> x [B][192][192][16] fp16 (r, g, b, d, sqrt(d), d*d, 0 ...), depth192 fp32
 __global__ void __launch_bounds__(256) sod_prep_kernel(const float* __restrict__ rgb, int H, int W, const float* __restrict__ depth,
                                                        int h, int w, __half* __restrict__ x, float* __restrict__ depth192) {

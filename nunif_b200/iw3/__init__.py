@@ -21,6 +21,7 @@ from .depth_anything_model import DepthAnythingModel, DepthAnythingNet, batch_in
 from . import zoedepth_preprocess  # noqa: F401
 from .zoedepth_model import ZoeDepthModel, ZoeDepthNet  # noqa: F401
 from .zoedepth_any_model import ZoeDepthAnythingModel, ZoeDepthAnythingNet  # noqa: F401
+from .null_depth_model import NullDepthModel, NullDepthNet  # noqa: F401
 from .depth_model_factory import create_depth_model  # noqa: F401
 from .row_flow import RowFlowV3, MLBW, apply_divergence_nn_LR, apply_divergence_nn_delta, apply_divergence_nn_delta_weight  # noqa: F401
 from .row_flow import RowFlowV2, apply_divergence_nn_symmetric, load_row_flow_model  # noqa: F401
