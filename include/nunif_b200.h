@@ -282,7 +282,7 @@ enum { NB200_COMPOSE_NONE = 0,      /* separate left/right planar tensors       
 /* iw3/backward_warp.py:96-121 apply_divergence_grid_sample.
  * c: [B][3][H][W], depth: [B][1][h][w] (any resolution).
  * compose NONE: left,right = [B][3][H][W]; SBS: left = [B][3][H][2W], right unused;
- * ANAGLYPH: left = [B][3][H][W], right unused. */
+ * ANAGLYPH: left = [B][3][H][W], right unused.  B and H above 65535 are refused. */
 int nb200_backward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w,
                         double divergence, double convergence, int synthetic_view, int compose,
                         float* left, float* right, void* stream);
@@ -700,6 +700,8 @@ int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launc
  *                   and the SOD REBNCONV)
  *   bit 3 (on = 8): rfprep rflast rf2 mlprep mlout holemask aaminmax aaprep aaout (the input and output stages of row_flow_v3,
  *                   mlbw and depth_aa, the fused row_flow_v2 delta kernel and the hole mask of mask_mlbw_l2)
+ *   bit 4 (on = 16): bwarp bwdelta aaresize (nb200_backward_warp / _conv with the kernel path taken, the learned-delta warps
+ *                   nb200_backward_warp_delta / _f16 / _sym, and nb200_depth_resize_aa)
  * A line is `kind,name=value,name=value,...`: the launch's fields without its pointers, named where the host code writes
  * them.  Values are integers (flags 0 or 1) or fp32 values printed with 9 significant digits.  recorded_launches_named copies
  * the lines (NUL-terminated) like nb200_profile_dump; recorded_launches copies them without the names (`kind,value,...`, the

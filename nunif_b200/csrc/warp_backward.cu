@@ -17,8 +17,8 @@
 namespace nb200 {
 
 __device__ __forceinline__ float linspace_m1_1(int j, int n, float step) {
-    // torch.linspace(-1, 1, n) fp32 (ATen RangeFactories: symmetric evaluation)
-    return (j < n / 2) ? (-1.0f + step * (float)j) : (1.0f - step * (float)(n - j - 1));
+    // torch.linspace(-1, 1, n) fp32 (ATen RangeFactories: symmetric evaluation; one point is the start, -1)
+    return (j < n / 2 || n == 1) ? (-1.0f + step * (float)j) : (1.0f - step * (float)(n - j - 1));
 }
 
 __device__ __forceinline__ float srgb_to_linear(float x) {
@@ -69,9 +69,10 @@ struct BwParams {
     int warp_left, warp_right;
 };
 
-// One thread = VEC consecutive output pixels of one row, both eyes, 3 channels.
+// One thread = VEC consecutive output pixels of one row, both eyes, 3 channels.  vec_ok: W % 4 == 0 and 16-byte aligned
+// outputs, so the float4 stores are aligned.
 template <int COMPOSE, int VEC>
-__global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
+__global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p, int vec_ok) {
     const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * VEC;
     const int y = blockIdx.y;
     const int b = blockIdx.z;
@@ -160,7 +161,7 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
         for (int v = 0; v < VEC; ++v) dubois_px(outl[v], outr[v], true, res[v]);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
-            if (VEC == 4 && x0 + 3 < p.W && (p.W & 3) == 0) {
+            if (VEC == 4 && x0 + 3 < p.W && vec_ok) {
                 *reinterpret_cast<float4*>(orow + k * plane + x0) = make_float4(res[0][k], res[1][k], res[2][k], res[3][k]);
             } else {
                 for (int v = 0; v < VEC; ++v)
@@ -175,7 +176,7 @@ __global__ void __launch_bounds__(256) backward_warp_kernel(BwParams p) {
     float* rrow = (COMPOSE == NB200_COMPOSE_SBS) ? lrow + p.W : p.right + ((size_t)b * 3 * p.H + y) * ow;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-        if (VEC == 4 && x0 + 3 < p.W && (p.W & 3) == 0) {
+        if (VEC == 4 && x0 + 3 < p.W && vec_ok) {
             *reinterpret_cast<float4*>(lrow + k * oplane + x0) = make_float4(outl[0][k], outl[1][k], outl[2][k], outl[3][k]);
             *reinterpret_cast<float4*>(rrow + k * oplane + x0) = make_float4(outr[0][k], outr[1][k], outr[2][k], outr[3][k]);
         } else {
@@ -369,6 +370,9 @@ static int backward_warp(const float* c, const float* depth, int B, int H, int W
     NB_CHECK(compose != NB200_COMPOSE_NONE || right, "right output required for compose=NONE");
     NB_CHECK(B > 0 && H > 0 && W > 0 && h > 0 && w > 0, "bad shape");
     NB_CHECK(synthetic_view >= 0 && synthetic_view <= 2, "synthetic_view must be both/left/right");
+    // both kernels put the batch (and the gather kernel the row) on a grid axis limited to 65535
+    NB_CHECK(B <= 65535, "batch too large for one launch (B > 65535)");
+    NB_CHECK(H <= 65535, "image too tall for one launch (H > 65535)");
     BwParams p;
     p.c = c; p.depth = depth; p.left = left; p.right = right;
     p.B = B; p.H = H; p.W = W; p.h = h; p.w = w;
@@ -391,9 +395,14 @@ static int backward_warp(const float* c, const float* depth, int B, int H, int W
     ProfScope ps(st, PC_WARP_BW, (double)B * H * W * 4 * (3 + (compose == NB200_COMPOSE_ANAGLYPH_DUBOIS ? 3 : 6)) + (double)B * h * w * 4);
     const int S = (W + 1 + 3) & ~3;
     const size_t smem = sizeof(GridTab) * (size_t)(w + 1) + sizeof(float) * 3 * (size_t)S;
-    if (smem <= 200 * 1024 && g_tune[3] == 0 && B <= 65535) {
-        const bool aligned = (((uintptr_t)c | (uintptr_t)left | (uintptr_t)(right ? right : left)) & 15) == 0;
-        const int vec_ok = (W % 4 == 0) && aligned;
+    const bool row_staged = smem <= 200 * 1024 && g_tune[3] == 0;
+    const bool aligned = (((uintptr_t)c | (uintptr_t)left | (uintptr_t)(right ? right : left)) & 15) == 0;
+    const int vec_ok = (W % 4 == 0) && aligned;
+    if (rec_on(REC_WARP))
+        rec_launch("bwarp", {{"B", B}, {"H", H}, {"W", W}, {"h", h}, {"w", w}, {"view", synthetic_view}, {"compose", compose},
+                             {"conv", conv ? 1 : 0}, {"shift", (double)p.shift}, {"shift_conv", (double)p.shift_conv},
+                             {"delta_scale", (double)p.delta_scale}, {"path", row_staged ? 0 : 1}});
+    if (row_staged) {
         int rc;
         switch (compose) {
             case NB200_COMPOSE_NONE: rc = launch_bw_row<NB200_COMPOSE_NONE>(p, smem, S, vec_ok, st); break;
@@ -406,10 +415,10 @@ static int backward_warp(const float* c, const float* depth, int B, int H, int W
         return 0;
     }
     switch (compose) {
-        case NB200_COMPOSE_NONE: backward_warp_kernel<NB200_COMPOSE_NONE, VEC><<<grid, block, 0, st>>>(p); break;
-        case NB200_COMPOSE_SBS: backward_warp_kernel<NB200_COMPOSE_SBS, VEC><<<grid, block, 0, st>>>(p); break;
+        case NB200_COMPOSE_NONE: backward_warp_kernel<NB200_COMPOSE_NONE, VEC><<<grid, block, 0, st>>>(p, vec_ok); break;
+        case NB200_COMPOSE_SBS: backward_warp_kernel<NB200_COMPOSE_SBS, VEC><<<grid, block, 0, st>>>(p, vec_ok); break;
         case NB200_COMPOSE_ANAGLYPH_DUBOIS:
-            backward_warp_kernel<NB200_COMPOSE_ANAGLYPH_DUBOIS, VEC><<<grid, block, 0, st>>>(p); break;
+            backward_warp_kernel<NB200_COMPOSE_ANAGLYPH_DUBOIS, VEC><<<grid, block, 0, st>>>(p, vec_ok); break;
         default: return fail("nb200_backward_warp: unknown compose mode");
     }
     NB_LAUNCHED();
@@ -460,6 +469,9 @@ static int backward_warp_delta(const float* c, const float* delta, int B, int H,
     const int S = (W + 1 + 3) & ~3;
     const size_t smem = sizeof(GridTab) * (size_t)(w + 1) + sizeof(float) * 3 * (size_t)S;
     NB_CHECK(smem <= 200 * 1024 && B <= 65535, "image row too wide for the row-staged warp");
+    if (rec_on(REC_WARP))
+        rec_launch("bwdelta", {{"B", B}, {"H", H}, {"W", W}, {"h", h}, {"w", w}, {"mode", f16 ? 1 : 0}, {"warp_left", 0},
+                               {"warp_right", 1}, {"delta_scale", (double)p.delta_scale}});
     const bool aligned = (((uintptr_t)c | (uintptr_t)out) & 15) == 0;
     ProfScope ps(st, PC_WARP_BW, (double)B * H * W * 4 * 6 + (double)B * h * w * 4);
     const int vec_ok = (W % 4 == 0) && aligned;
@@ -499,6 +511,9 @@ extern "C" int nb200_backward_warp_delta_sym(const float* c, const float* delta,
     const int S = (W + 1 + 3) & ~3;
     const size_t smem = sizeof(GridTab) * (size_t)(w + 1) + sizeof(float) * 3 * (size_t)S;
     NB_CHECK(smem <= 200 * 1024 && B <= 65535, "image row too wide for the row-staged warp");
+    if (rec_on(REC_WARP))
+        rec_launch("bwdelta", {{"B", B}, {"H", H}, {"W", W}, {"h", h}, {"w", w}, {"mode", 2}, {"warp_left", p.warp_left},
+                               {"warp_right", p.warp_right}, {"delta_scale", (double)p.delta_scale}});
     const bool aligned = (((uintptr_t)c | (uintptr_t)left | (uintptr_t)right) & 15) == 0;
     ProfScope ps(st, PC_WARP_BW, (double)B * H * W * 4 * 9 + (double)B * h * w * 4);
     if (launch_bw_row<NB200_COMPOSE_NONE>(p, smem, S, (W % 4 == 0) && aligned, st)) return 1;

@@ -382,6 +382,7 @@ extern "C" int nb200_forward_warp_conv(const float* c, const float* depth, int B
 extern "C" int nb200_depth_resize_aa(const float* depth, int B, int h, int w, int H, int W, float* out, void* stream) {
     NB_CHECK(depth && out, "null pointer");
     float sy = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f, sx = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
+    if (rec_on(REC_WARP)) rec_launch("aaresize", {{"B", B}, {"h", h}, {"w", w}, {"H", H}, {"W", W}});
     depth_resize_aa_kernel<<<dim3(cdiv(W, 128), H, B), 128, 0, (cudaStream_t)stream>>>(depth, out, B, H, W, h, w, sy, sx);
     NB_LAUNCHED();
     return 0;

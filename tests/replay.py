@@ -255,6 +255,77 @@ STEREO_MODELS = [
 ]
 
 
+# the backward stereo warps and the AA depth resize (tests/test_gpu_kernel_replay_warp.py): production flows through the
+# Python API, as bench.py and iw3.utils.apply_divergence call them, on seeded frames and depth maps at the sizes the depth
+# models return (Depth-Anything's preprocess_size)
+def _frames(seed, B, H, W):
+    return torch.stack([synth.synth_image(seed + i, 3, H, W, smooth=False) for i in range(B)]).to(DEV)
+
+
+def _bench_sbs(B, H, W, h, w, **kw):
+    def run():
+        from nunif_b200.iw3 import stereo_sbs
+        stereo_sbs(_frames(50, B, H, W), synth.synth_depth(60, B, h, w).to(DEV), 2.0, 0.5, method="backward",
+                   edge_dilation=[2, 1], **kw)
+    return run
+
+
+def _args(method, view="both", convergence=0.5, **kw):
+    from types import SimpleNamespace
+    return SimpleNamespace(method=method, mapper="none", divergence=2.0, convergence=convergence, synthetic_view=view,
+                           **{**dict(warp_steps=None, preserve_screen_border=False, stereo_width=None, disable_amp=False,
+                                     state=None), **kw})
+
+
+def _grid_sample_views():
+    """A 1080p landscape frame, a portrait frame and a 240 x 320 frame (whose 392 x 518 depth is larger than the frame),
+    each with synthetic_view both, left and right."""
+    from nunif_b200.iw3.utils import apply_divergence
+    from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
+    for k, (H, W) in enumerate(((1080, 1920), (1920, 1080), (240, 320))):
+        h, w = preprocess_size(H, W)
+        for view in ("both", "left", "right"):
+            apply_divergence(synth.synth_depth(70 + k, 1, h, w).to(DEV), _frames(80 + k, 1, H, W), _args("grid_sample", view), None)
+
+
+def _grid_sample_conv_tensor():
+    """Auto-convergence's B,1,1,1 convergence tensor on a batch of four 1080p frames."""
+    from nunif_b200.iw3.utils import apply_divergence
+    conv = torch.tensor([0.5, 0.0, 0.9, 0.25], device=DEV).view(4, 1, 1, 1)
+    apply_divergence(synth.synth_depth(73, 4, 392, 686).to(DEV), _frames(83, 4, 1080, 1920), _args("grid_sample", convergence=conv), None)
+
+
+def _learned(method, build, H=1080, W=1920, views=("both",), **kw):
+    """A learned warp (apply_divergence's side-model branch) on a frame with the Depth-Anything-sized depth of a 1080p frame."""
+    def run():
+        from nunif_b200.iw3.utils import apply_divergence
+        model = build()
+        for view in views:
+            apply_divergence(synth.synth_depth(74, 1, 392, 686).to(DEV), _frames(84, 1, H, W), _args(method, view, **kw), model)
+    return run
+
+
+def _rf_sym():
+    from nunif_b200.iw3 import RowFlowV3
+    return RowFlowV3(synth.row_flow_v3_state_dict(0), DEV, symmetric=True)
+
+
+WARP_FLOWS = [
+    ("stereo_sbs_1080p", _bench_sbs(4, 1080, 1920, 392, 686)),                                 # bench configs[2]
+    ("stereo_sbs_4k_dubois", _bench_sbs(2, 2160, 3840, 384, 704, mapper="div_6", anaglyph="dubois")),   # bench configs[4]
+    ("grid_sample_views", _grid_sample_views),
+    ("grid_sample_conv_tensor", _grid_sample_conv_tensor),
+    ("row_flow_v3", _learned("row_flow_v3", _iw3("RowFlowV3", synth.row_flow_v3_state_dict), warp_steps=1)),
+    ("row_flow_v3_steps2", _learned("row_flow_v3", _iw3("RowFlowV3", synth.row_flow_v3_state_dict), warp_steps=2)),
+    ("row_flow_v2", _learned("row_flow_v2", _iw3("RowFlowV2", synth.row_flow_v2_state_dict))),
+    ("row_flow_v3_sym", _learned("row_flow_v3_sym", _rf_sym, views=("both", "left"))),
+    ("mlbw_l2", _learned("mlbw_l2", _iw3("MLBW", lambda: synth.mlbw_state_dict(0, 2)))),
+    ("mlbw_l4", _learned("mlbw_l4", _iw3("MLBW", lambda: synth.mlbw_state_dict(0, 4)))),
+    ("mask_mlbw_l2", _learned("mask_mlbw_l2", _iw3("MLBW", synth.mask_mlbw_state_dict))),
+    ("row_flow_v3_stereo_width", _learned("row_flow_v3", _iw3("RowFlowV3", synth.row_flow_v3_state_dict), 2160, 3840, stereo_width=1920)),
+]
+
+
 # ------------------------------------------------------------------------------------------------------------ guarded buffers
 def guarded(n):
     """fp16 buffer of GUARD + n + GUARD elements, all SENTINEL."""

@@ -111,13 +111,14 @@ def test_zoe_preprocess_size_host_rule_bit_exact(lib):
         assert (fh + 2 * p_h, fw + 2 * p_w, p_h, p_w) == (int(oh), int(ow), int(ph), int(pw)), (H, W)
 
 
-def test_launch_recorder_mask_bits_0_to_3(lib):
+def test_launch_recorder_mask_bits_0_to_4(lib):
     """nb200_record_launches takes a mask of the recorded kinds (bit 0: GEMM / attention / Swin, bit 1: the kernels between
     them, bit 2: the waifu2x stem / tail / head convolutions, SE, to_image and the SOD REBNCONV, bit 3: the stereo networks'
-    input / output stages, row_flow_v2 and the hole mask) and refuses other bits; host only, no device needed."""
-    for on in (1, 2, 3, 4, 7, 8, 15, 0):
+    input / output stages, row_flow_v2 and the hole mask, bit 4: the backward stereo warps and the AA depth resize) and
+    refuses other bits; host only, no device needed."""
+    for on in (1, 2, 3, 4, 7, 8, 15, 16, 31, 0):
         assert lib.nb200_record_launches(on) == 0, on
-    for on in (16, 31):
+    for on in (32, 63):
         assert lib.nb200_record_launches(on) != 0, on
         assert b"unknown recorder bits" in lib.nb200_last_error()
     buf = ctypes.create_string_buffer(16)
@@ -144,6 +145,34 @@ def test_stereo_entry_points_refuse_bad_geometry(lib):
         (lambda: lib.nb200_depth_aa_out_f32(d, d, None, 1, 16, 17, 0, 0, 8, 8, d, d, 1, d, None), b"padded width"),
     ]
     assert lib.nb200_record_launches(8) == 0
+    try:
+        for i, (call, msg) in enumerate(cases):
+            assert call() != 0, i
+            assert msg in lib.nb200_last_error(), (i, lib.nb200_last_error())
+    finally:
+        lib.nb200_record_launches(0)
+    buf = ctypes.create_string_buffer(16)
+    assert lib.nb200_recorded_launches(buf, 16) == 0 and buf.value == b""
+
+
+def test_backward_warp_entry_points_refuse_bad_geometry(lib):
+    """nb200_backward_warp / _conv refuse a batch or a height beyond a grid axis (65535) for either kernel, and the
+    learned-delta warps a row too wide for the row-staged kernel's 200 KB of shared memory (W = 7313 with a full-resolution
+    delta), all before their first CUDA call: dummy host pointers, no device needed, and nothing is recorded."""
+    d = ctypes.create_string_buffer(4096)
+    bw = lambda B, H: lib.nb200_backward_warp(d, d, B, H, 8, 4, 4, 2.0, 0.5, 0, 0, d, d, None)
+    bwc = lambda B, H: lib.nb200_backward_warp_conv(d, d, B, H, 8, 4, 4, 2.0, d, 0, 1, d, None, None)
+    cases = [
+        (lambda: bw(65536, 8), b"batch too large"),
+        (lambda: bw(1, 65536), b"image too tall"),
+        (lambda: bwc(65536, 8), b"batch too large"),
+        (lambda: bwc(1, 65536), b"image too tall"),
+        (lambda: lib.nb200_backward_warp_delta(d, d, 1, 2, 7313, 2, 7313, 0.001, d, None), b"image row too wide"),
+        (lambda: lib.nb200_backward_warp_delta_f16(d, d, 1, 2, 7313, 2, 7313, 0.001, d, None), b"image row too wide"),
+        (lambda: lib.nb200_backward_warp_delta_sym(d, d, 1, 2, 7313, 2, 7313, 0.001, 1, 1, d, d, None), b"image row too wide"),
+        (lambda: lib.nb200_backward_warp_delta(d, d, 65536, 2, 8, 2, 8, 0.001, d, None), b"image row too wide"),
+    ]
+    assert lib.nb200_record_launches(16) == 0
     try:
         for i, (call, msg) in enumerate(cases):
             assert call() != 0, i
