@@ -296,7 +296,9 @@ int nb200_backward_warp_conv(const float* c, const float* depth, int B, int H, i
 /* iw3/forward_warp.py:246-256 apply_divergence_forward_warp (inconsistent_shift=False).
  * depth: [B][1][h][w]; if (h,w)!=(H,W) it is resized like forward_warp.py:146-148.
  * fill!=0 <=> method=="forward_fill".  masks may be NULL (return_mask=False).
- * workspace: nb200_forward_warp_workspace() bytes (may be NULL if depth is full-res). */
+ * workspace: nb200_forward_warp_workspace() bytes (may be NULL if depth is full-res), 16-byte aligned when both axes of the
+ * depth upsample.  Refused before any CUDA call: empty sizes, B > 65535, a divergence whose padding
+ * P = (int)(base * divergence * 0.01 + 2) is negative, and a padded row W + 2P over 8301 cells (227 KB of shared memory). */
 size_t nb200_forward_warp_workspace(int B, int H, int W, int h, int w);
 int nb200_forward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w,
                        double divergence, double convergence, int fill, int synthetic_view,
@@ -686,7 +688,9 @@ int nb200_tune_set(int key, int value);   /* kernel-selection knobs (csrc/gemm.c
 int nb200_debug_tap(int id, void* dev_buf, size_t capacity);  /* copy intermediate `id` of nb200_zoedepth_forward (ids 0..14,
                                                                15 = the sorted centres of a normed head, DESIGN.md §5)
                                                                or nb200_light_inpaint (ids 100..173, DESIGN.md §5)
-                                                               or nb200_transnetv2_forward (ids 200..205) to dev_buf */
+                                                               or nb200_transnetv2_forward (ids 200..205) to dev_buf;
+                                                               id 300: the padded depth rows of nb200_forward_warp / _conv,
+                                                               fp32 [B][H][Wp], written by the warp kernel itself */
 int nb200_profile_enable(int on);
 int nb200_profile_report(char* buf, size_t cap);
 int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launch: class,ms,work,read_bytes,write_bytes */
@@ -700,8 +704,9 @@ int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launc
  *                   and the SOD REBNCONV)
  *   bit 3 (on = 8): rfprep rflast rf2 mlprep mlout holemask aaminmax aaprep aaout (the input and output stages of row_flow_v3,
  *                   mlbw and depth_aa, the fused row_flow_v2 delta kernel and the hole mask of mask_mlbw_l2)
- *   bit 4 (on = 16): bwarp bwdelta aaresize (nb200_backward_warp / _conv with the kernel path taken, the learned-delta warps
- *                   nb200_backward_warp_delta / _f16 / _sym, and nb200_depth_resize_aa)
+ *   bit 4 (on = 16): bwarp bwdelta aaresize fwarp (nb200_backward_warp / _conv with the kernel path taken, the learned-delta
+ *                   warps nb200_backward_warp_delta / _f16 / _sym, nb200_depth_resize_aa, and nb200_forward_warp / _conv with
+ *                   its depth-resize path: 0 none, 1 column table, 2 generic taps)
  * A line is `kind,name=value,name=value,...`: the launch's fields without its pointers, named where the host code writes
  * them.  Values are integers (flags 0 or 1) or fp32 values printed with 9 significant digits.  recorded_launches_named copies
  * the lines (NUL-terminated) like nb200_profile_dump; recorded_launches copies them without the names (`kind,value,...`, the

@@ -66,7 +66,7 @@ struct ProfScope {
 // the kinds: REC_GEMMS the GEMM, ViT attention and fused Swin block; REC_AUX the WABlock core, add + LayerNorm, DPT upsample
 // and ZoeDepth bins head; REC_CONV the waifu2x stem / tail / head convolutions, the SE block, to_image and the SOD REBNCONV;
 // REC_STEREO the input / output stages of row_flow_v3, mlbw and depth_aa, the fused row_flow_v2 kernel and the hole mask;
-// REC_WARP the backward stereo warps and the antialiased depth resize.
+// REC_WARP the backward and forward stereo warps and the antialiased depth resize.
 enum { REC_GEMMS = 1, REC_AUX = 2, REC_CONV = 4, REC_STEREO = 8, REC_WARP = 16 };
 extern std::atomic<int> g_rec_enabled;
 inline bool rec_on(int kinds = REC_GEMMS) { return (g_rec_enabled.load(std::memory_order_relaxed) & kinds) != 0; }
@@ -80,6 +80,10 @@ struct RecField {
 };
 // appends the line `kind,name=value,...`; the call sites are the record format's only definition
 void rec_launch(const char* kind, std::initializer_list<RecField> fields);
+
+// debug taps (nb200_debug_tap, model.cu) that a kernel writes itself: *buf = the armed buffer when tap `id` is armed, else
+// null; an armed buffer smaller than `bytes` is refused
+int debug_tap_target(int id, size_t bytes, void** buf);
 
 // seam_blend.cu: rows [y0, y1) of the blended output (used by the band-pipelined host render in model.cu)
 int tile_gather_blend_rows(const void* z_all, int z_f32, int C, const ::nb200_tile_config* cfg, int scale, int offset, int tile_size,

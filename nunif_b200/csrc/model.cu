@@ -475,7 +475,7 @@ static int swin_forward(nb200_model* m, cudaStream_t st, const __half* x, int n,
 #include "legacy_model.inl"
 // debug tap (nb200_debug_tap): stage `g_tap_id` of the next ZoeDepth, light_inpaint_v1 or TransNetV2 forward is copied to
 // `g_tap_buf` (ZoeDepth ids 0..15 in zoe_model.inl; light_inpaint_v1 ids 100..173, table in DESIGN.md §5; TransNetV2 ids
-// 200..205 in transnet_model.inl)
+// 200..205 in transnet_model.inl); the forward warp's kernel writes id 300 itself (warp_forward.cu)
 static int g_tap_id = -1;
 static void* g_tap_buf = nullptr;
 static size_t g_tap_cap = 0;
@@ -483,6 +483,14 @@ static int tap_copy(cudaStream_t st, int id, const void* src, size_t bytes) {
     if (id != g_tap_id || !g_tap_buf) return 0;
     NB_CHECK(bytes <= g_tap_cap, "debug tap buffer too small: need " + std::to_string(bytes) + " bytes");
     NB_CUDA(cudaMemcpyAsync(g_tap_buf, src, bytes, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+int nb200::debug_tap_target(int id, size_t bytes, void** buf) {
+    *buf = nullptr;
+    if (id != g_tap_id || !g_tap_buf) return 0;
+    NB_CHECK(bytes <= g_tap_cap, "debug tap buffer too small: need " + std::to_string(bytes) + " bytes");
+    *buf = g_tap_buf;
     return 0;
 }
 
@@ -760,8 +768,8 @@ extern "C" int nb200_tiled_render_host(nb200_model* m, const float* x_host, int 
     return rc;   // scratch_guard frees xd / od behind the last copy (stream-ordered)
 }
 
-// debug: copy intermediate `id` of the following nb200_zoedepth_forward / nb200_light_inpaint calls into dev_buf (capacity bytes);
-// id < 0 disables
+// debug: copy intermediate `id` of the following nb200_zoedepth_forward / nb200_light_inpaint / nb200_transnetv2_forward calls,
+// or the padded depth rows of the following nb200_forward_warp calls (id 300), into dev_buf (capacity bytes); id < 0 disables
 extern "C" int nb200_debug_tap(int id, void* dev_buf, size_t capacity) {
     g_tap_id = id; g_tap_buf = dev_buf; g_tap_cap = capacity;
     return 0;

@@ -11,7 +11,10 @@
 //    writer with the largest depth wins".  Two writers with equal depth can never hit the
 //    same destination cell of the same (floor|ceil) buffer (equal depth => equal shift =>
 //    destinations differ by the source distance >= 1), so a shared-memory atomicMax
-//    z-buffer on the order-preserving depth key reproduces the sort exactly.
+//    z-buffer on the order-preserving depth key reproduces the sort exactly -- except in
+//    the clamped end cells 0 and Wp-1, which are visible when P = 0: there the stable sort
+//    gives the cell to the largest source index among the deepest, so the winner is taken
+//    with atomicMax too, and -0.0 keys as +0.0 (the sort ties them).
 //  * shift_fill (<=100 iterations of 1-px propagation) == "nearest valid cell within 100
 //    to the left, else the value 100 cells to the left"; F.pad's zero at the edge is a
 //    virtual valid cell holding 0.
@@ -93,7 +96,9 @@ __global__ void depth_resize_aa_kernel(const float* __restrict__ depth, float* _
     out[((size_t)b * H + y) * W + X] = aa_bilinear_sample(depth + (size_t)b * h * w, h, w, scale_y, scale_x, y, X);
 }
 
-__global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p) {
+// dep_tap (debug tap 300, null in production): the padded depth rows [B][H][Wp] this launch warps.  It is an argument of
+// its own: one more FwParams member (136 instead of 128 bytes) made ptxas spill and cost 8 to 15 % at 1080p (H100).
+__global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p, float* __restrict__ dep_tap) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int Wp = p.Wp, W = p.W, P = p.P;
     // 7 row arrays of Wp 32-bit cells
@@ -123,6 +128,8 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
             DEP[P + W + t] = DEP[P + W - 1];
         }
         __syncthreads();
+        if (dep_tap)
+            for (int t = tid; t < Wp; t += FW_THREADS) dep_tap[((size_t)b * p.H + y) * Wp + t] = DEP[t];
     }
 
     // a convergence tensor makes shift_size * convergence an fp32 tensor op (forward_warp.py:167)
@@ -144,20 +151,25 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
             float is = __fsub_rn(__fmul_rn(d, p.shift_size), conv_term);
             float fi = fminf(fmaxf(__fadd_rn((float)xp, sg * is), 0.f), (float)(Wp - 1));
             int fl = (int)floorf(fi), ce = (int)ceilf(fi);
-            unsigned key = order_key(d);
+            unsigned key = order_key(__fadd_rn(d, 0.f));  // -0.0 + 0.0 = +0.0
             atomicMax(&ZF[fl], key);
             atomicMax(&ZC[ce], key);
         }
         __syncthreads();
-        // ---- pass 2: winners (unique per visible cell, see header)
+        // ---- pass 2: winners: the largest source index of the deepest key (unique except in the clamped cells, see header)
         for (int xp = tid; xp < Wp; xp += FW_THREADS) {
             float d = DEP[xp];
             float is = __fsub_rn(__fmul_rn(d, p.shift_size), conv_term);
             float fi = fminf(fmaxf(__fadd_rn((float)xp, sg * is), 0.f), (float)(Wp - 1));
             int fl = (int)floorf(fi), ce = (int)ceilf(fi);
-            unsigned key = order_key(d);
-            if (ZF[fl] == key) SF[fl] = xp;
-            if (ZC[ce] == key) SC[ce] = xp;
+            unsigned key = order_key(__fadd_rn(d, 0.f));
+            if (P == 0) {
+                if (ZF[fl] == key) atomicMax(&SF[fl], xp);
+                if (ZC[ce] == key) atomicMax(&SC[ce], xp);
+            } else {
+                if (ZF[fl] == key) SF[fl] = xp;
+                if (ZC[ce] == key) SC[ce] = xp;
+            }
         }
         __syncthreads();
         // ---- resolve each visible destination (:129-130, unpad :180-183).
@@ -289,14 +301,15 @@ __global__ void __launch_bounds__(FW_THREADS) forward_warp_row_kernel(FwParams p
     }
 }
 
-// copy of the source image into an eye (synthetic_view left/right returns src_image, :222-243)
+// copy of the source image into an eye (synthetic_view left/right returns src_image, :222-243); an SBS frame clamps
+// both halves (iw3/utils.py:469)
 __global__ void copy_eye_kernel(const float* __restrict__ c, float* __restrict__ out, int H, int W, int ow, int xoff,
-                                size_t total) {
+                                size_t total, int sbs) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     int x = (int)(i % W);
     size_t r = i / W;  // (b*3 + k)*H + y
-    out[r * ow + xoff + x] = c[i];
+    out[r * ow + xoff + x] = sbs ? clamp01(c[i]) : c[i];
 }
 
 }  // namespace nb200
@@ -312,10 +325,13 @@ extern "C" size_t nb200_forward_warp_workspace(int B, int H, int W, int h, int w
 static int forward_warp(const float* c, const float* depth, int B, int H, int W, int h, int w, double divergence,
                         double convergence, const float* conv, int fill, int synthetic_view, int width_base, int compose,
                         float* left, float* right, float* left_mask, float* right_mask, void* workspace, void* stream) {
+    // every refusal comes before the first CUDA call
     NB_CHECK(c && depth && left, "null pointer");
     NB_CHECK(compose == NB200_COMPOSE_NONE || compose == NB200_COMPOSE_SBS, "compose must be NONE or SBS");
     NB_CHECK(compose == NB200_COMPOSE_SBS || right, "right output required");
     NB_CHECK(synthetic_view >= 0 && synthetic_view <= 2, "synthetic_view must be both/left/right");
+    NB_CHECK(B > 0 && H > 0 && W > 0 && h > 0 && w > 0, "bad shape");
+    NB_CHECK(B <= 65535, "batch too large for one launch (B > 65535)");  // the row kernel's grid is (H, B)
     FwParams p;
     p.c = c; p.depth = depth; p.left = left; p.right = right; p.left_mask = left_mask; p.right_mask = right_mask;
     p.B = B; p.H = H; p.W = W; p.h = h; p.w = w;
@@ -323,7 +339,11 @@ static int forward_warp(const float* c, const float* depth, int B, int H, int W,
     if (synthetic_view != NB200_VIEW_BOTH) div *= 2;                 // forward_warp.py:149-150
     const double base = width_base ? (double)W : (double)(H > W ? H : W);  // :153-156
     p.P = (int)(base * div * 0.01 + 2);                              // :158
+    // P < 0 (divergence <= -300 / base) would write the depth row below shared memory, where the reference pads nothing
+    NB_CHECK(p.P >= 0, "divergence too negative: the row padding (int)(base * divergence * 0.01 + 2) is below 0");
     p.Wp = W + 2 * p.P;
+    const size_t smem = (size_t)p.Wp * 7 * sizeof(float);
+    NB_CHECK(smem <= 227 * 1024, "row (with divergence padding) does not fit shared memory");
     const double shift_size = div * 0.01 * base * 0.5;               // :166
     p.shift_size = (float)shift_size;
     p.conv_term = (float)(shift_size * convergence);         // :167
@@ -334,20 +354,27 @@ static int forward_warp(const float* c, const float* depth, int B, int H, int W,
     p.compose = compose;
     p.scale_y = H > 1 ? (float)(h - 1) / (float)(H - 1) : 0.f;
     p.scale_x = W > 1 ? (float)(w - 1) / (float)(W - 1) : 0.f;
-    p.coltab = nullptr;
-    cudaStream_t st0 = (cudaStream_t)stream;
-    if ((h != H || w != W) && workspace && p.scale_x < 1.f && p.scale_y < 1.f) {
-        p.coltab = reinterpret_cast<const float4*>(workspace);
-        depth_coltab_kernel<<<cdiv(W, 256), 256, 0, st0>>>(reinterpret_cast<float4*>(workspace), W, w, p.scale_x);
+    const bool resize = h != H || w != W;
+    const bool table = resize && workspace && p.scale_x < 1.f && p.scale_y < 1.f;
+    // the column table is stored and loaded as float4
+    NB_CHECK(!table || ((uintptr_t)workspace & 15) == 0, "workspace must be 16-byte aligned");
+    void* tap = nullptr;
+    if (debug_tap_target(300, (size_t)B * H * p.Wp * sizeof(float), &tap)) return 1;
+    p.coltab = table ? reinterpret_cast<const float4*>(workspace) : nullptr;
+    if (rec_on(REC_WARP))
+        rec_launch("fwarp", {{"B", B}, {"H", H}, {"W", W}, {"h", h}, {"w", w}, {"P", p.P}, {"Wp", p.Wp},
+                             {"shift", (double)p.shift_size}, {"conv_term", (double)p.conv_term}, {"conv", conv ? 1 : 0},
+                             {"fill", fill}, {"view", synthetic_view}, {"compose", compose}, {"lmask", left_mask ? 1 : 0},
+                             {"rmask", right_mask ? 1 : 0}, {"path", !resize ? 0 : table ? 1 : 2}});
+    cudaStream_t st = (cudaStream_t)stream;
+    if (table) {
+        depth_coltab_kernel<<<cdiv(W, 256), 256, 0, st>>>(reinterpret_cast<float4*>(workspace), W, w, p.scale_x);
         NB_LAUNCHED();
     }
-    const size_t smem = (size_t)p.Wp * 7 * sizeof(float);
-    NB_CHECK(smem <= 227 * 1024, "row (with divergence padding) does not fit shared memory");
-    cudaStream_t st = (cudaStream_t)stream;
     NB_CUDA(cudaFuncSetAttribute(forward_warp_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     {
         ProfScope ps(st, PC_WARP_FW, (double)B * H * W * 4 * 9 + (double)B * h * w * 4);
-        forward_warp_row_kernel<<<dim3(H, B), FW_THREADS, smem, st>>>(p);
+        forward_warp_row_kernel<<<dim3(H, B), FW_THREADS, smem, st>>>(p, static_cast<float*>(tap));
     }
     NB_LAUNCHED();
     if (synthetic_view != NB200_VIEW_BOTH) {
@@ -356,7 +383,7 @@ static int forward_warp(const float* c, const float* depth, int B, int H, int W,
         const bool sbs = compose == NB200_COMPOSE_SBS;
         float* dst = synthetic_view == NB200_VIEW_RIGHT ? left : (sbs ? left : right);
         int ow = sbs ? 2 * W : W, xoff = (sbs && synthetic_view == NB200_VIEW_LEFT) ? W : 0;
-        copy_eye_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(c, dst, H, W, ow, xoff, total);
+        copy_eye_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(c, dst, H, W, ow, xoff, total, sbs);
         NB_LAUNCHED();
     }
     return 0;

@@ -12,11 +12,13 @@ import time
 import zlib
 
 import torch
+import torch.nn.functional as F
 
 from tests.util import log_metric
 from nunif_b200 import _lib, synth
 
 DEV = "cuda:0"
+U = 2.0 ** -24                 # fp32 unit roundoff
 SENTINEL = 0x7E5B              # an fp16 NaN payload: fp16 guards keep exactly this bit pattern
 SENTINEL32 = 0x7FC05B5B        # an fp32 NaN payload: fp32 guards keep exactly this bit pattern
 GUARD = 4096                   # guard elements before and after every buffer
@@ -324,6 +326,111 @@ WARP_FLOWS = [
     ("mask_mlbw_l2", _learned("mask_mlbw_l2", _iw3("MLBW", synth.mask_mlbw_state_dict))),
     ("row_flow_v3_stereo_width", _learned("row_flow_v3", _iw3("RowFlowV3", synth.row_flow_v3_state_dict), 2160, 3840, stereo_width=1920)),
 ]
+
+
+# the forward stereo warp (tests/test_gpu_kernel_replay_forward_warp.py): production flows through the Python API, on seeded
+# frames and depth maps at the sizes the depth models return
+def _fwd_sbs(B, H, W, h, w, method="forward_fill", **kw):
+    def run():
+        from nunif_b200.iw3 import stereo_sbs
+        stereo_sbs(_frames(50, B, H, W), synth.synth_depth(60, B, h, w).to(DEV), 2.0, 0.5, method=method, edge_dilation=[2, 1], **kw)
+    return run
+
+
+def _forward_views():
+    """forward_fill and forward in every synthetic_view on a 1080p landscape frame, a portrait frame and a 240 x 320 frame
+    (whose 392 x 518 Depth-Anything depth is larger than the frame)."""
+    from nunif_b200.iw3.utils import apply_divergence
+    from nunif_b200.iw3.depth_anything_preprocess import preprocess_size
+    for k, (H, W) in enumerate(((1080, 1920), (1920, 1080), (240, 320))):
+        h, w = preprocess_size(H, W)
+        for method in ("forward_fill", "forward"):
+            for view in ("both", "left", "right"):
+                apply_divergence(synth.synth_depth(90 + k, 1, h, w).to(DEV), _frames(95 + k, 1, H, W), _args(method, view), None)
+
+
+def _forward_conv_tensor():
+    """Auto-convergence's B,1,1,1 convergence tensor on a batch of four 1080p frames."""
+    from nunif_b200.iw3.utils import apply_divergence
+    conv = torch.tensor([0.5, 0.0, 0.9, 0.25], device=DEV).view(4, 1, 1, 1)
+    apply_divergence(synth.synth_depth(93, 4, 392, 686).to(DEV), _frames(98, 4, 1080, 1920), _args("forward_fill", convergence=conv), None)
+
+
+def _forward_inpaint(max_width):
+    """forward_inpaint (synthetic light_inpaint_v1 weights) on a 1080p frame, at full width or resized to max_width."""
+    def run():
+        from nunif_b200.iw3.utils import apply_divergence
+        from nunif_b200.iw3 import ForwardInpaint
+        model = ForwardInpaint(synth.light_inpaint_v1_state_dict(0), DEV)
+        apply_divergence(synth.synth_depth(94, 1, 392, 686).to(DEV), _frames(99, 1, 1080, 1920),
+                         _args("forward_inpaint", inpaint_max_width=max_width), model)
+    return run
+
+
+def _forward_null_depth():
+    """The NULL depth model at the frame's own size (a square frame): the warp's resize-free path."""
+    from nunif_b200.iw3.null_depth_model import NullDepthNet
+    from nunif_b200.iw3 import stereo_sbs
+    x = _frames(100, 1, 512, 512)
+    stereo_sbs(x, NullDepthNet(512)(x), 2.0, 0.5, method="forward_fill")
+
+
+FWARP_FLOWS = [
+    ("stereo_sbs_1080p", _fwd_sbs(4, 1080, 1920, 392, 686)),                                    # bench configs[2]
+    ("stereo_anaglyph", _fwd_sbs(1, 1080, 1920, 392, 686, method="forward", anaglyph="dubois")),   # both eyes, compose NONE
+    ("forward_views", _forward_views),
+    ("forward_conv_tensor", _forward_conv_tensor),
+    ("forward_inpaint", _forward_inpaint(None)),
+    ("forward_inpaint_max_width", _forward_inpaint(640)),
+    ("null_depth", _forward_null_depth),
+]
+
+
+# ------------------------------------------------------------------------------------------------------------ AA resize bound
+DW = 10.5 * U   # one tap weight tri(((j + min) - centre + 0.5) * inv) at a given centre: the subtraction, + 0.5 and * inv
+                # rounded, inv = 1 / scale within 2U / scale of the exact (|t| <= support + 1.5): (5 + 4.5 / scale) U <= 9.5U
+                # downsampling, 5.5U upsampling; then 1 - |arg| rounded (U)
+
+
+def aa_axis(n_in, n_out):
+    """One axis of ATen's antialiased bilinear resize with align_corners=True (csrc/aa_resize.cuh): per output index the
+    exact centre c = s (i + 0.5), s = (n_in - 1) / (n_out - 1), its taps [lo, hi) and their weight sum S.  -> (window start,
+    window length, centre term, weight term, taps) where
+      the centre term = slope * E_c: E_c = 2U c (the fp32 scale and the product rounded); the taps that enter or leave as
+        the centre moves weigh zero there, so the sample is continuous in c, and |dv/dc| = |sum_j (w'_j / S)(x_j - v)|
+        <= (taps + 2) inv / S * (max - min of x over the window), |w'_j| <= inv
+      the weight term = 2 taps DW / S + (taps + 1) U: each weight's DW, the sum S (taps DW + taps U S) and the division
+    The window [lo - 1, hi] holds every tap a centre within E_c of c can use."""
+    s = (n_in - 1) / (n_out - 1) if n_out > 1 else 0.0
+    support, inv = (s, 1 / s) if s >= 1 else (1.0, 1.0)
+    c = s * (torch.arange(n_out, dtype=torch.float64) + 0.5)
+    lo = (c - support + 0.5).trunc().clamp(min=0)
+    hi = (c + support + 0.5).trunc().clamp(max=n_in)
+    size = hi - lo
+    K = int(size.max()) + 2
+    j = lo.view(-1, 1) + torch.arange(K, dtype=torch.float64).view(1, -1)
+    wts = ((1 - ((j - c.view(-1, 1) + 0.5) * inv).abs()).clamp(min=0) * (j < hi.view(-1, 1))).sum(1)
+    slope = (size + 2) * inv / wts
+    start = (lo - 1).clamp(min=0).long()
+    to = lambda t: t.to(DEV)
+    return to(start), K, to(slope * 2 * U * c), to(2 * size * DW / wts + (size + 1) * U), to(size)
+
+
+def aa_resize_reference(x64, H, W):
+    """F.interpolate(x64, (H, W), bilinear, align_corners=True, antialias=True) in float64 and the bound on the kernels' fp32
+    sample (csrc/aa_resize.cuh) of x64 [B][C][h][w]:
+      R (cterm_y + cterm_x) + M (wterm_y + wterm_x + (taps_y + taps_x) U)
+    with aa_axis's terms, M the largest |x| and R the range of x over the window, and the two fp32 accumulations
+    (taps - 1 sums each, first order).  -> (reference, bound), the bound without SECOND_ORDER's margin."""
+    h, w = x64.shape[-2:]
+    ref = F.interpolate(x64, size=(H, W), mode="bilinear", align_corners=True, antialias=True)
+    ys, Ky, cy, wy, ny = aa_axis(h, H)
+    xs, Kx, cx, wx, nx = aa_axis(w, W)
+    xp = F.pad(x64, (0, Kx, 0, Ky), mode="replicate")
+    win = lambda m: F.max_pool2d(m, (Ky, Kx), 1)[:, :, ys][:, :, :, xs]
+    hi, lo = win(xp), -win(-xp)
+    M, R = torch.maximum(hi.abs(), lo.abs()), hi - lo
+    return ref, R * (cy.view(H, 1) + cx.view(1, W)) + M * (wy.view(H, 1) + wx.view(1, W) + (ny.view(H, 1) + nx.view(1, W)) * U)
 
 
 # ------------------------------------------------------------------------------------------------------------ guarded buffers

@@ -183,6 +183,40 @@ def test_backward_warp_entry_points_refuse_bad_geometry(lib):
     assert lib.nb200_recorded_launches(buf, 16) == 0 and buf.value == b""
 
 
+def test_forward_warp_entry_points_refuse_bad_geometry(lib):
+    """nb200_forward_warp / _conv refuse, before their first CUDA call: a divergence whose row padding
+    P = (int)(base * divergence * 0.01 + 2) is negative (W = 64, divergence -5: P = -1), a padded row over 227 KB at 28 B per
+    cell with a depth that upsamples on both axes and a workspace (H = 3 from h = 2, W = 8002 from w = 3000, P = 150:
+    Wp = 8302), so that checking after the column-table launch would fail on that launch instead,
+    B over the grid's 65535, a misaligned workspace that the column table would use, and empty sizes.  Dummy host pointers,
+    no device needed, and nothing is recorded."""
+    d = ctypes.create_string_buffer(4096)
+    ws = ctypes.addressof(d) + (16 - ctypes.addressof(d) % 16) % 16      # 16-byte aligned inside d
+    fw = lambda B, H, W, h, w, div, work=ws: lib.nb200_forward_warp(d, d, B, H, W, h, w, div, 0.5, 1, 0, 1, 0, d, d, d, d, work, None)
+    fwc = lambda B, H, W, h, w, div, work=ws: lib.nb200_forward_warp_conv(d, d, B, H, W, h, w, div, d, 1, 0, 1, 1, d, None, None,
+                                                                          None, work, None)
+    cases = []
+    for f in (fw, fwc):
+        cases += [
+            (lambda f=f: f(1, 4, 64, 4, 64, -5.0), b"divergence too negative"),
+            (lambda f=f: f(1, 3, 8002, 2, 3000, 1.85), b"does not fit shared memory"),
+            (lambda f=f: f(65536, 4, 64, 2, 32, 2.0), b"batch too large"),
+            (lambda f=f: f(1, 4, 64, 2, 32, 2.0, ws + 4), b"16-byte aligned"),
+            (lambda f=f: f(0, 4, 64, 2, 32, 2.0), b"bad shape"),
+            (lambda f=f: f(1, 4, 64, 0, 32, 2.0), b"bad shape"),
+            (lambda f=f: f(1, 4, 0, 2, 32, 2.0), b"bad shape"),
+        ]
+    assert lib.nb200_record_launches(16) == 0
+    try:
+        for i, (call, msg) in enumerate(cases):
+            assert call() != 0, i
+            assert msg in lib.nb200_last_error(), (i, lib.nb200_last_error())
+    finally:
+        lib.nb200_record_launches(0)
+    buf = ctypes.create_string_buffer(16)
+    assert lib.nb200_recorded_launches(buf, 16) == 0 and buf.value == b""
+
+
 def test_launch_recorder_names_each_field(lib):
     """A recorded line is `kind,name=value,...` with the names the replay tests read, and nb200_recorded_launches returns
     the same values without the names.  zoe_expand_rel_bias records its launch before it checks ldb, so a call with dummy

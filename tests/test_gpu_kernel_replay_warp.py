@@ -25,13 +25,12 @@ import torch
 import torch.nn.functional as F
 
 from tests.util import log_metric
-from tests.replay import (DEV, GUARD, SENTINEL32, WARP_FLOWS, Tally, configurations, guarded32, record_networks, recorded,
-                          replay, rounded)
+from tests.replay import (DEV, GUARD, SENTINEL32, U, WARP_FLOWS, Tally, aa_resize_reference, configurations, guarded32,
+                          record_networks, recorded, replay, rounded)
 from nunif_b200 import _lib
 from nunif_b200._lib import ptr
 
 pytestmark = pytest.mark.gpu
-U = 2.0 ** -24                 # fp32 unit roundoff
 REC_WARP = 16                  # nb200_record_launches bit of the kinds replayed here
 TINY = 1e-300                  # bound floor: an exact element has err / bound 0
 SECOND_ORDER = 1 + 2.0 ** -20  # the first-order bounds below leave out products of two roundings
@@ -464,41 +463,9 @@ def test_backward_warp_delta_replay(production):
 
 
 # ------------------------------------------------------------------------------------------------------------ aaresize
-DW = 10.5 * U   # one tap weight tri(((j + min) - centre + 0.5) * inv) at a given centre: the subtraction, + 0.5 and * inv
-                # rounded, inv = 1 / scale within 2U / scale of the exact (|t| <= support + 1.5): (5 + 4.5 / scale) U <= 9.5U
-                # downsampling, 5.5U upsampling; then 1 - |arg| rounded (U)
-
-
-def aa_axis(n_in, n_out):
-    """One axis of ATen's antialiased bilinear resize with align_corners=True (csrc/aa_resize.cuh): per output index the
-    exact centre c = s (i + 0.5), s = (n_in - 1) / (n_out - 1), its taps [lo, hi) and their weight sum S.  -> (window start,
-    window length, centre term, weight term, taps) where
-      the centre term = slope * E_c: E_c = 2U c (the fp32 scale and the product rounded); the taps that enter or leave as
-        the centre moves weigh zero there, so the sample is continuous in c, and |dv/dc| = |sum_j (w'_j / S)(x_j - v)|
-        <= (taps + 2) inv / S * (max - min of x over the window), |w'_j| <= inv
-      the weight term = 2 taps DW / S + (taps + 1) U: each weight's DW, the sum S (taps DW + taps U S) and the division
-    The window [lo - 1, hi] holds every tap a centre within E_c of c can use."""
-    s = (n_in - 1) / (n_out - 1) if n_out > 1 else 0.0
-    support, inv = (s, 1 / s) if s >= 1 else (1.0, 1.0)
-    c = s * (torch.arange(n_out, dtype=torch.float64) + 0.5)
-    lo = (c - support + 0.5).trunc().clamp(min=0)
-    hi = (c + support + 0.5).trunc().clamp(max=n_in)
-    size = hi - lo
-    K = int(size.max()) + 2
-    j = lo.view(-1, 1) + torch.arange(K, dtype=torch.float64).view(1, -1)
-    wts = ((1 - ((j - c.view(-1, 1) + 0.5) * inv).abs()).clamp(min=0) * (j < hi.view(-1, 1))).sum(1)
-    slope = (size + 2) * inv / wts
-    start = (lo - 1).clamp(min=0).long()
-    to = lambda t: t.to(DEV)
-    return to(start), K, to(slope * 2 * U * c), to(2 * size * DW / wts + (size + 1) * U), to(size)
-
-
 def aaresize_check(r, seed, off):
-    """F.interpolate(depth, (H, W), bilinear, align_corners=True, antialias=True) in float64, on depth in [-0.25, 1.25].
-    The kernel's fp32 sample differs from it by at most
-      R (cterm_y + cterm_x) + M (wterm_y + wterm_x + (taps_y + taps_x) U)
-    with aa_axis's terms, M the largest |x| and R the range of x over the window, and the two fp32 accumulations
-    (taps - 1 sums each, first order)."""
+    """F.interpolate(depth, (H, W), bilinear, align_corners=True, antialias=True) in float64, on depth in [-0.25, 1.25],
+    within aa_resize_reference's bound."""
     B, h, w, H, W = (r[f] for f in ("B", "h", "w", "H", "W"))
     g = _gen(seed)
     tally = Tally()
@@ -512,16 +479,8 @@ def aaresize_check(r, seed, off):
     tally.exact("depth", xb.view(torch.int32), x0.view(torch.int32))
     guards(tally, "out", ob, no, off)
     tally.no_nan("out", out)
-    x64 = x.view(B, 1, h, w).double()
-    ref = F.interpolate(x64, size=(H, W), mode="bilinear", align_corners=True, antialias=True)
-    ys, Ky, cy, wy, ny = aa_axis(h, H)
-    xs, Kx, cx, wx, nx = aa_axis(w, W)
-    xp = F.pad(x64, (0, Kx, 0, Ky), mode="replicate")
-    win = lambda m: F.max_pool2d(m, (Ky, Kx), 1)[:, :, ys][:, :, :, xs]
-    hi, lo = win(xp), -win(-xp)
-    M, R = torch.maximum(hi.abs(), lo.abs()), hi - lo
-    bound = SECOND_ORDER * (R * (cy.view(H, 1) + cx.view(1, W)) + M * (wy.view(H, 1) + wx.view(1, W) + (ny.view(H, 1) + nx.view(1, W)) * U))
-    tally.add(out.view(B, 1, H, W), ref, bound + TINY)
+    ref, bound = aa_resize_reference(x.view(B, 1, h, w).double(), H, W)
+    tally.add(out.view(B, 1, H, W), ref, SECOND_ORDER * bound + TINY)
     return tally.result()
 
 
