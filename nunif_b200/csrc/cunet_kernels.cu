@@ -239,7 +239,7 @@ __global__ void __launch_bounds__(256) tail_conv_mma_kernel(const __half* __rest
         iy0 = (oy0 + 3 - ky_hi) >> 1;                            // may be -1 at the top edge (zero-filled)
         ix0 = j0;                                                // columns j0 .. j0 + 65 (see tap table below)
     }
-    {   // fp16 B fragments are stored right behind the fp32 [tap][ci][co] array (cunet_model.inl pack_tail)
+    {   // fp16 B fragments are stored right behind the fp32 [tap][ci][co] array (cunet_model.cu pack_tail)
         const uint4* frag = reinterpret_cast<const uint4*>(wt + TAPS * 192);
         for (int i = tid; i < TAPS * 64; i += 256) reinterpret_cast<uint4*>(sB)[i] = __ldg(frag + i);
     }

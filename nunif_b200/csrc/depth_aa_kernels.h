@@ -1,4 +1,4 @@
-// Non-GEMM kernels of the learned depth anti-aliasing filter iw3.depth_aa (depth_aa.cu); wiring in depth_aa_model.inl.
+// Non-GEMM kernels of the learned depth anti-aliasing filter iw3.depth_aa (depth_aa.cu); wiring in depth_aa_model.cu.
 #pragma once
 #include "common.cuh"
 

@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(256) add_layernorm_kernel(float* __restrict__ 
 // ring; S and O live in mma.sync accumulator fragments, softmax is online in base 2 (scale*log2e folded into S).
 constexpr int FA_D = 64, FA_BM = 64, FA_BN = 64, FA_LD = FA_D + 8;   // +8 halves: conflict-free fragment loads
 
-// BIAS: an additive score bias [heads][N][ldb] fp32, pre-multiplied by log2(e) (BEiT relative position bias, zoe_model.inl);
+// BIAS: an additive score bias [heads][N][ldb] fp32, pre-multiplied by log2(e) (BEiT relative position bias, zoe_model.cu);
 // ldb >= cdiv(N, 64) * 64 so that the tail block's loads stay in bounds (those columns are masked below)
 template <bool BIAS>
 __global__ void __launch_bounds__(128) flash_attention_kernel(const __half* __restrict__ qkv, __half* __restrict__ out, int N, int heads,

@@ -1,4 +1,4 @@
-// Kernels of the Depth-Anything-V2 path that are not GEMMs (depth_kernels.cu); model wiring in depth_model.inl.
+// Kernels of the Depth-Anything-V2 path that are not GEMMs (depth_kernels.cu); model wiring in depth_model.cu.
 #pragma once
 #include "common.cuh"
 

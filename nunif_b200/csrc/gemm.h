@@ -7,6 +7,9 @@ namespace nb200 {
 // CG_TCONV3: a (3,1,1) convolution over time with dilation `dil` and zero padding `dil`; A is viewed as [B][T = Hi][Wi][Ci]
 // (Wi = the pixels of one frame), taps t - dil, t, t + dil
 enum : int { CG_LINEAR_FLAT = 0, CG_LINEAR_2D = 1, CG_CONV3 = 2, CG_DOWN2 = 3, CG_TCONV3 = 5 };
+// ConvGemm::act (the epilogue's activation) and ConvGemm::out_mode
+enum : int { ACT_NONE = 0, ACT_LRELU01 = 1, ACT_GELU = 2, ACT_RELU = 3 };
+enum : int { OUT_NHWC = 0, OUT_PIXSHUF2 = 1, OUT_SPLIT = 2 };
 
 struct ConvGemm {
     const __half* A = nullptr;  // NHWC fp16 activations [B][Hi][Wi][Ci]

@@ -20,13 +20,11 @@
 // co-resident per SM, which overlaps one tile's epilogue with the next tile's loads.
 #pragma once
 #include "common.cuh"
+#include "gemm.h"
 #include "ptx.cuh"
 #include <cuda.h>
 
 namespace nb200 {
-
-enum : int { ACT_NONE = 0, ACT_LRELU01 = 1, ACT_GELU = 2, ACT_RELU = 3 };
-enum : int { OUT_NHWC = 0, OUT_PIXSHUF2 = 1, OUT_SPLIT = 2 };
 
 struct GemmParams {
     // output tiling: the M dimension is (b, y, x) over Ho x Wo pixels, tiled TH x TW (TH*TW == 128)

@@ -1,6 +1,6 @@
 // iw3 forward_inpaint: the kernels of inpaint.light_inpaint_v1 (iw3/models/light_inpaint_v1.py) and its mask preparation
 // (iw3/dilation.py, iw3/forward_inpaint.py:18-40) that are not convolutions.  The convolutions and Linears run on the wgmma
-// implicit GEMM (gemm.cu); the sequence is in inpaint_model.inl.
+// implicit GEMM (gemm.cu); the sequence is in inpaint_model.cu.
 #include "inpaint_kernels.h"
 #include "ptx.cuh"
 #include <cmath>

@@ -210,7 +210,7 @@ static int launch_head(cudaStream_t st, bool mma, const __half* x, const float* 
         if (ensure_dyn_smem((const void*)head_conv_mma_kernel<MODE, CIN>, Cfg::SMEM)) return 1;
         const int npx = MODE == 1 ? Wo / 2 : Wo;
         const dim3 grid(cdiv(npx, 64), MODE == 0 ? cdiv(Ho, 2) : cdiv(Ho + 1, 2), n);
-        // fp16 B fragments follow the fp32 [tap][ci][co] array (legacy_model.inl pack_head)
+        // fp16 B fragments follow the fp32 [tap][ci][co] array (legacy_model.cu pack_head)
         const __half* frag = reinterpret_cast<const __half*>(wt + (size_t)Cfg::TAPS * CIN * 3);
         head_conv_mma_kernel<MODE, CIN><<<grid, 256, Cfg::SMEM, st>>>(x, frag, bias, out, Hi, Wi, Ho, Wo);
     } else {

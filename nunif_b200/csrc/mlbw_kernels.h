@@ -1,4 +1,4 @@
-// Non-GEMM kernels of the multi-layer learned stereo warp sbs.mlbw (mlbw.cu); wiring in mlbw_model.inl.
+// Non-GEMM kernels of the multi-layer learned stereo warp sbs.mlbw (mlbw.cu); wiring in mlbw_model.cu.
 #pragma once
 #include "common.cuh"
 

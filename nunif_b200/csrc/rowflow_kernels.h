@@ -1,4 +1,4 @@
-// Non-GEMM kernels of the learned stereo warp sbs.row_flow_v3 (rowflow_kernels.cu); wiring in rowflow_model.inl.
+// Non-GEMM kernels of the learned stereo warp sbs.row_flow_v3 (rowflow_kernels.cu); wiring in rowflow_model.cu.
 #pragma once
 #include "common.cuh"
 
@@ -11,7 +11,7 @@ int rf_prep(cudaStream_t st, const float* x, int B, int h, int w, int Hp, int Wt
 int rf_last_conv(cudaStream_t st, const __half* x, int B, int Hp, int Wt, int h, int w, const float* wt72, float bias, float* delta);
 
 // sbs.row_flow_v2 (rowflow_v2.cu): one fused kernel, RF2_ROWS x RF2_T output pixels per CTA.  Its weights are one parameter
-// block of RF2_PARAM_BYTES (packed by rowflow_v2_model.inl) that each CTA copies to shared memory:
+// block of RF2_PARAM_BYTES (packed by rowflow_v2_model.cu) that each CTA copies to shared memory:
 //   mma.sync B fragments in lane order [k-step][n8 tile][lane] (uint2), k = (row * taps + tap) * cin + ci:
 //     RF2_FRAG1 conv #1 (9 k-steps x 2 tiles), RF2_FRAG2 conv #2 (9 x 4), RF2_FRAG3 conv #3 (18 x 4), RF2_FRAG4 3x3 (18 x 1)
 //   then fp32 (fp16-representable) scalars at RF2_F32, indexed in floats: feature weight [16][3][3] and bias, head weight [16]

@@ -45,7 +45,7 @@ static_assert(RF2_PARAM_BYTES % 16 == 0 && OFF_C3 % 16 == 0 && OFF_NOV % 16 == 0
 
 // One warp, two m16 tiles (columns m0 .. m0 + 15 and m0 + 64 .. m0 + 79): acc[mt][nt] += sum over the k-steps of
 // A[col][k] * B[k][n], k-step ks = (row * TAPS + tap) * CIN/16 + chunk reading channels chunk*16 .. +15 of column col + tap of
-// src[row].  The weights are B fragments in lane order, [ks][nt][lane] (rf2 packing in rowflow_v2_model.inl).
+// src[row].  The weights are B fragments in lane order, [ks][nt][lane] (rf2 packing in rowflow_v2_model.cu).
 template <int CIN, int NT, int TAPS, int ROWS>
 __device__ __forceinline__ void conv_mma(float (&acc)[2][NT][4], const __half* const (&src)[ROWS], int stride, int m0,
                                          const uint2* __restrict__ frag, int lane) {

@@ -1,5 +1,5 @@
 // iw3.sod_v1 (iw3/models/sod_v1.py): U^2-Net-p (nunif/utils/u2netp.py) on 192 x 192 NHWC fp16, and the convergence
-// estimate of iw3/convergence_estimator.py.  Packed by sod_model.inl, run by sod.cu.
+// estimate of iw3/convergence_estimator.py.  Packed by sod_model.cu, run by sod.cu.
 #pragma once
 #include "common.cuh"
 #include <string>

@@ -1,5 +1,5 @@
 // The small kernels of TransNetV2 (nunif/utils/transnetv2.py); the convolutions and fc1 run on the wgmma GEMM
-// (transnet_model.inl).  Every kernel works on one frame or one (frame, branch) pair per CTA with a fixed reduction order, so
+// (transnet_model.cu).  Every kernel works on one frame or one (frame, branch) pair per CTA with a fixed reduction order, so
 // a window's result does not depend on the other windows of the batch.
 //
 //   * tn_prep_kernel: [n][3][27][48] fp32 -> NHWC fp16 with the channels padded to 32.

@@ -1,4 +1,4 @@
-// TransNetV2 (nunif/utils/transnetv2.py), the shot-boundary network of iw3's --scene-detect.  Packed by transnet_model.inl,
+// TransNetV2 (nunif/utils/transnetv2.py), the shot-boundary network of iw3's --scene-detect.  Packed by transnet_model.cu,
 // small kernels in transnet.cu; every convolution runs on the wgmma implicit GEMM (gemm.h: CG_CONV3 and CG_TCONV3).
 #pragma once
 #include "common.cuh"

@@ -1,6 +1,6 @@
 // Kernels of the window-attention block WABlock that sbs.row_flow_v3, sbs.mlbw and iw3.depth_aa are built from
 // (iw3/models/row_flow_v3.py:13-29, mlbw.py:18-34, depth_aa.py:11-26): the WindowMHA2d core between its qkv and head_proj
-// Linears, and the replication pad of conv_mlp.  Everything else of the block runs on the wgmma GEMM (wa_block.inl).
+// Linears, and the replication pad of conv_mlp.  Everything else of the block runs on the wgmma GEMM (wa_block.cu).
 #include "window_mha.h"
 
 namespace nb200 {

@@ -1,5 +1,5 @@
 // Non-GEMM kernels of the window-attention block WABlock (window_mha.cu) that sbs.row_flow_v3, sbs.mlbw and iw3.depth_aa share;
-// wiring in wa_block.inl.
+// wiring in wa_block.cu.
 #pragma once
 #include "common.cuh"
 

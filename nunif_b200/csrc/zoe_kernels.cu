@@ -273,7 +273,7 @@ __global__ void __launch_bounds__(256) zoe_attractor_normed_kernel(const __half*
 }
 
 // one thread per (pixel, group of 8 channels): groups 0..15 = the resampled embedding, 16..19 = the activation, 20 = relative
-// depth + zeros, 21..23 = zeros (channel order chosen at pack time, zoe_model.inl)
+// depth + zeros, 21..23 = zeros (channel order chosen at pack time, zoe_model.cu)
 __global__ void __launch_bounds__(256) zoe_clb_concat_kernel(const __half* __restrict__ act, const float* __restrict__ rel,
                                                               const __half* __restrict__ emb, int B, int h, int w, int H, int W, float sy,
                                                               float sx, __half* __restrict__ A) {

@@ -1,5 +1,5 @@
 // Kernels of the ZoeD_N path that are neither GEMMs nor shared with Depth-Anything (zoe_kernels.cu); model wiring in
-// zoe_model.inl.  Restated architecture + parity anchor: oracle/zoedepth.py.
+// zoe_model.cu.  Restated architecture + parity anchor: oracle/zoedepth.py.
 #pragma once
 #include "common.cuh"
 

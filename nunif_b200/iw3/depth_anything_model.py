@@ -3,7 +3,7 @@ Depth-Anything-V2 (Any_V2_S/B/L) and V1 (Any_S/B/L) relative-depth networks on t
 
 The reference obtains the network from torch.hub ("nagadomi/Depth-Anything_iw3:main", DepthAnything(encoder="v2_vits"),
 depth_anything_model.py:223-230); here the same checkpoint (upstream key names ``pretrained.*`` / ``depth_head.*``) is
-packed into the native container (csrc/depth_model.inl) and run as wgmma GEMMs + the kernels in
+packed into the native container (csrc/depth_model.cu) and run as wgmma GEMMs + the kernels in
 csrc/depth_kernels.cu.  ``infer`` keeps the reference's signature and output convention: depth B,1,h,w (or 1,h,w)
 float32 on ``x.device``, larger = nearer.
 """

@@ -2,7 +2,7 @@
 holes behind foreground edges, and the `inpaint.light_inpaint_v1` network (iw3/models/light_inpaint_v1.py) paints them.
 
 The warp is csrc/warp_forward.cu, the mask chain and the network are csrc/inpaint_kernels.cu + the wgmma GEMM
-(csrc/inpaint_model.inl).  Video mode (`light_video_inpaint_v1`, a 12-frame queue) is not implemented and raises.
+(csrc/inpaint_model.cu).  Video mode (`light_video_inpaint_v1`, a 12-frame queue) is not implemented and raises.
 """
 import contextlib
 import os

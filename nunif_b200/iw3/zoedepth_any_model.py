@@ -4,7 +4,7 @@ The reference builds these through torch.hub ("nagadomi/Depth-Anything_iw3:main"
 "indoor" / "outdoor", zoedepth_model.py:154-170): ZoeDepth's metric bins head over a Depth-Anything V1 ViT-L/14 encoder and
 DPT head, with ``prep_mod = 14`` and network heights 392 (landscape) / 518 (portrait) (:190-199).  Here the same checkpoints
 (upstream key names ``core.core.pretrained.*``, ``core.core.depth_head.*``, ``conv2``, ``seed_bin_regressor``, ...) are packed into
-the native container (csrc/zoe_model.inl) and run by ``nb200_zoedepth_forward``.  ZoeD_Any_N has the "softplus" bins head of
+the native container (csrc/zoe_model.cu) and run by ``nb200_zoedepth_forward``.  ZoeD_Any_N has the "softplus" bins head of
 ZoeD_N; ZoeD_Any_K the "normed" one (bins bounded to [1e-3, 80], sorted at the last level).  Loading, ``batch_infer`` and
 ``infer`` are ZoeDepthModel's (the reference uses one class for all ZoeDepth checkpoints).
 """

@@ -4,7 +4,7 @@ H100 engine.
 The reference obtains the network from torch.hub ("nagadomi/ZoeDepth_iw3:main", ZoeD_N, config_mode="infer",
 zoedepth_model.py:151-157) and removes its internal resize/normalise (`model.core.prep = lambda x: x`, :169); here the
 same checkpoint (ZoeD_M12_N.pt, upstream key names `core.core.pretrained.*`, `core.core.scratch.*`, `conv2`,
-`seed_bin_regressor`, ...) is packed into the native container (csrc/zoe_model.inl) and run as wgmma GEMMs + the
+`seed_bin_regressor`, ...) is packed into the native container (csrc/zoe_model.cu) and run as wgmma GEMMs + the
 kernels in csrc/depth_kernels.cu / zoe_kernels.cu.  ``infer`` keeps the reference's signature and output convention:
 B,1,h,w (or 1,h,w) float32 on ``x.device`` = the NEGATED metric depth of the unpadded frame (larger = nearer).
 

@@ -81,7 +81,7 @@ def test_pos_table_interpolation_matches_oracle():
 
 @pytest.mark.parametrize("encoder,H,W", [("vitb", 14 * 6, 14 * 9), ("vitl", 14 * 5, 14 * 7)])
 def test_depth_anything_base_and_large_encoders(encoder, H, W):
-    """Any_V2_B / Any_V2_L share the code path; only the table in depth_model.inl changes (dim, heads, depth, head widths)."""
+    """Any_V2_B / Any_V2_L share the code path; only the table in depth_model.cu changes (dim, heads, depth, head widths)."""
     from nunif_b200.iw3 import DepthAnythingNet
     sd = synth.depth_anything_v2_state_dict(5, encoder=encoder, pos_grid=8)
     x = torch.randn(1, 3, H, W, generator=torch.Generator().manual_seed(H * W))

@@ -77,7 +77,7 @@ def test_row_flow_feature_values():
 @pytest.mark.parametrize("g,ph,pw", [(24, 24, 32), (24, 24, 44), (6, 4, 6), (6, 6, 6), (5, 9, 3)])
 def test_zoe_relative_position_table_resample_matches_oracle(g, ph, pw):
     """Host logic of the ZoeD_N path (no GPU): the BEiT relative-position table resampled for a non-training token grid
-    (csrc/zoe_model.inl zoe_resample_table) against the oracle's F.interpolate restatement of MiDaS `_get_rel_pos_bias`."""
+    (csrc/zoe_model.cu zoe_resample_table) against the oracle's F.interpolate restatement of MiDaS `_get_rel_pos_bias`."""
     import ctypes
     import torch
     import torch.nn.functional as F
