@@ -616,6 +616,27 @@ int nb200_apply_rgb_noise(const float* rgb, int B, int C, int H, int W, const fl
                           int level, float* buffer, int buffer_reset, const double* params_host, int light_decay, int out_bits,
                           void* out, void* stream);
 
+/* Planar YUV <-> integer RGB, the frame conversions the reference leaves to libswscale at both ends of its video path
+ * (nunif/utils/video.py:621-639 to_ndarray(format="rgb24" | "rgb48le", ...), :763-850 frame.reformat(format=pix_fmt, ...)).
+ * A frame is one buffer of `frame_stride` elements: Y [H][W], then U and V (Cb, Cr) [ceil(H/sy)][ceil(W/sx)], each row
+ * pitch equal to its width; 8-bit planes are uint8, 10- / 16-bit planes uint16 (little-endian, code in the low bits).
+ * Layouts (sx x sy): NB200_YUV420 2x2, NB200_YUV422 2x1, NB200_YUV444 1x1 (yuv420p / yuvj420p / yuv420p10le, ...);
+ * NB200_GBR: the G, B, R planes of gbrp / gbrp10le / gbrp16le (no matrix, full range).
+ * Matrix: Kr, Kb of ITU-R BT.601 (0.299, 0.114), BT.709 (0.2126, 0.0722), BT.2020 NCL (0.2627, 0.0593).
+ * Range: NB200_RANGE_LIMITED Y 16-235, Cb / Cr 16-240 (x 2^(bits-8)); NB200_RANGE_FULL 0 .. 2^bits-1, chroma zero at 2^(bits-1).
+ * RGB is always full range, HWC [B][H][W][3] uint8 (rgb_bits 8) or uint16 (rgb_bits 16).
+ * fp32 arithmetic, round to nearest even, clamp to the code range.
+ * nb200_yuv_to_rgb: each chroma sample is replicated over its sx x sy luma block; bits 8 or 10.
+ * nb200_rgb_to_yuv: each chroma sample is the mean of the unrounded full-resolution Cb / Cr of its block (fewer samples at an
+ *   odd edge); bits 8 or 10, or 16 for NB200_GBR; the padding after V up to frame_stride is zeroed. */
+enum { NB200_YUV420 = 0, NB200_YUV422 = 1, NB200_YUV444 = 2, NB200_GBR = 3 };
+enum { NB200_MATRIX_BT601 = 0, NB200_MATRIX_BT709 = 1, NB200_MATRIX_BT2020 = 2 };
+enum { NB200_RANGE_LIMITED = 0, NB200_RANGE_FULL = 1 };
+int nb200_yuv_to_rgb(const void* planes, int layout, int bits, int matrix, int range, int frame_stride, int B, int H, int W,
+                     int rgb_bits, void* out, void* stream);
+int nb200_rgb_to_yuv(const void* rgb, int rgb_bits, int B, int H, int W, int layout, int bits, int matrix, int range,
+                     int frame_stride, void* planes, void* stream);
+
 /* DepthAnything batch_preprocess (iw3/depth_anything_model.py:69-110): size rule (host,
  * integers) and the fused antialiased-bilinear resize + clamp + ImageNet normalise:
  * x [B][3][H][W] fp32 in [0,1] -> out [B][3][new_h][new_w] fp32. */

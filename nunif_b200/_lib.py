@@ -108,6 +108,8 @@ SIGNATURES = {
     "nb200_hwc_to_chw_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_chw_f32_to_hwc": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_hdr2sdr": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_double), c_int, c_void_p, c_void_p]),
+    "nb200_yuv_to_rgb": (c_int, [c_void_p] + [c_int] * 9 + [c_void_p, c_void_p]),
+    "nb200_rgb_to_yuv": (c_int, [c_void_p] + [c_int] * 9 + [c_void_p, c_void_p]),
     "nb200_rgb_noise": (c_int, [ctypes.c_uint64, ctypes.c_uint32, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_apply_rgb_noise": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, ctypes.c_uint64, ctypes.c_uint32, c_int,
                                       c_void_p, c_int, ctypes.POINTER(c_double), c_int, c_int, c_void_p, c_void_p]),

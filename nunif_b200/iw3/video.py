@@ -9,7 +9,21 @@ When the normaliser looks ahead (``get_ema_buffer_size() > 1``) the reference pa
 ``round(clamp(x * 255))`` uint8 (uint16 for a 16-bit ``--pix-fmt`` or source) and uploads it again on release.  The
 engine keeps those frames on the device instead, in a ring of HWC uint8 / uint16 slots allocated once per frame shape
 (``SourceRing``), with the same quantisation: the warp sees the same source pixels as in the reference.  With buffer
-size 1 the queue holds the preprocessed float frames, as the reference's does."""
+size 1 the queue holds the preprocessed float frames, as the reference's does.
+
+With ``nunif_b200.nunif.video.FrameBatchPipeline`` the caller's loop can hand over the decoded planes and receive the
+encoder's planes, so that neither colour conversion runs on the host:
+
+    pix_fmt, source, target = configure_colorspace(input_stream, args.colorspace, args.pix_fmt)
+    cb = bind_batch_frame_callback(depth_model, side_model, segment_pts, args)
+    pipe = FrameBatchPipeline(lambda x: cb(x, next_pts(len(x))), args.batch_size,
+                              use_16bit=pix_fmt_requires_16bit(pix_fmt), source=source, target=target)
+    for frame in container.decode(input_stream):
+        for planes in pipe(frame.to_ndarray()):
+            output_container.mux(output_stream.encode(av.VideoFrame.from_ndarray(planes, format=pix_fmt)))
+    for planes in pipe.finish():
+        ...   # encode as above; then cb(None, None, True) flushes the EMA look-ahead as float frames, which the caller
+              # quantises (chw_float_to_hwc) and converts (rgb_to_yuv(..., *target)) itself"""
 from collections import deque
 
 import torch

@@ -57,9 +57,11 @@ def make_frame_callback(ctx, args):
     return frame_callback
 
 
-def make_video_pipeline(ctx, args, batch_size, use_16bit=False, depth=3, seed=None):
+def make_video_pipeline(ctx, args, batch_size, use_16bit=False, depth=3, seed=None, source=None, target=None):
     """The video path of ui_utils.py:150-178 on the engine: make_frame_callback in a FrameBatchPipeline whose output stage
-    adds the temporal grain (``grain_strength``, ``grain_speed``) when ``args.grain`` is set and quantises for the encoder."""
+    adds the temporal grain (``grain_strength``, ``grain_speed``) when ``args.grain`` is set and quantises for the encoder.
+    ``source`` / ``target``: the (pix_fmt, colorspace, color_range) of the decoded and the encoded frames
+    (nunif_b200.nunif.video.configure_colorspace), so that the pipeline takes and returns plane arrays."""
     grain = (args.grain_strength, args.grain_speed, seed) if args.grain else None
     return FrameBatchPipeline(make_frame_callback(ctx, args), batch_size, device=args.state["device"], depth=depth,
-                              use_16bit=use_16bit, grain=grain)
+                              use_16bit=use_16bit, grain=grain, source=source, target=target)
