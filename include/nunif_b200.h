@@ -166,6 +166,11 @@ int nb200_zoedepth_forward(nb200_model* m, const float* x, int B, int H, int W, 
 /* Host-only helper of the same path: the per-block relative-position table ((2g-1)^2 + 3 rows x heads, learned on a g x g token
  * grid) resampled for a ph x pw grid as MiDaS backbones/beit.py `_get_rel_pos_bias` does (bilinear, the 3 class-token rows kept). */
 int nb200_zoe_rel_pos_table(const float* table, int g, int heads, int ph, int pw, float* out);
+/* Host-only helper of the Depth-Anything / ZoeD_Any path: dinov2 `interpolate_pos_encoding` (interpolate_offset 0.1) of the
+ * learned position table [1 + grid^2][dim] (class row first) for a ph x pw token grid -> out [1 + ph*pw][dim]: the class row
+ * copied, the grid bicubic resampled (A = -0.75, align_corners=False, scale factors (ph + 0.1) / grid, (pw + 0.1) / grid) in fp32
+ * as ATen does, or copied when ph == pw == grid. */
+int nb200_vit_pos_table_f32(const float* table, int grid, int dim, int ph, int pw, float* out);
 
 /* iw3.depth_aa (iw3/models/depth_aa.py:46-87; applied by batch_infer when depth_aa is set, iw3/depth_anything_model.py:153-154):
  * x [B][1][H][W] fp32 -> out, same shape.  mode 0 = forward in eval mode (clamp to [0,1]), 1 = infer (normalise by the
@@ -548,6 +553,31 @@ int nb200_depth_aa_prep_f16(const float* x, const float* minmax, int B, int H, i
 int nb200_depth_aa_out_f32(const void* tok, const float* x, const float* minmax, int B, int H, int W, int ph1, int pw1, int Hh,
                            int Wh, const float* weight, const float* bias, int clamp, float* out, void* stream);
 
+/* The depth networks' own kernels around their GEMMs (csrc/depth_kernels.h, zoe_kernels.h, where each is specified): device
+ * pointers throughout.  Each refuses a shape its kernel cannot take before any launch.
+ *   da_patch_im2col:     x [B][3][H][W] fp32 -> A [B*ph*pw][kpad] fp16, 14-px patches, k = (c*14 + ky)*14 + kx, columns
+ *                        588..kpad-1 zero; H, W multiples of 14, kpad >= 588.
+ *   zoe_patch_im2col:    the same with 16-px patches (BEiT), A [B*ph*pw][768]; H, W multiples of 16.
+ *   vit_assemble_tokens: T [B*P][dim] fp16, cls [dim], pos [1+P][dim] -> x32 [B][1+P][dim] fp32 = cat(cls, T) + pos; pos NULL:
+ *                        no position table (BEiT).
+ *   zoe_add_cast:        x32 [n] += delta [n] fp16 (may be NULL: x32 is not written), out fp16 = x32; n % 4 == 0.
+ *   zoe_readout_concat:  F [B][1+P][dim] fp16 -> A [B*P][2 dim] = cat(F[b][1+n], F[b][0]); dim % 8 == 0.
+ *   dpt_depth_to_space4: T [B*h*w][16 c] fp16, column (dy*4 + dx)*c + co -> out [B][4h][4w][cpad], channels c..cpad-1 zero.
+ *   dpt_im2col_s2:       x [B][h][w][C] fp16 -> A [B*ho*wo][9 C], ho = (h+1)/2, k = (ky*3 + kx)*C + c, taps of a 3x3 stride-2
+ *                        pad-1 conv (zeros outside); C % 8 == 0.
+ *   dpt_relu_add:        y = relu(x); with x0 and s (both or neither): s = x0 + x; fp16 [n], n % 8 == 0.
+ *   dpt_head_final:      depth [npix] fp32 = relu(fp16(x . w + bias)), x [npix][C] fp16, w [C] fp32; C == 32. */
+int nb200_da_patch_im2col_f16(const float* x, int B, int H, int W, int kpad, void* A, void* stream);
+int nb200_zoe_patch_im2col_f16(const float* x, int B, int H, int W, void* A, void* stream);
+int nb200_vit_assemble_tokens_f32(const void* T, const float* cls, const float* pos, float* x32, int B, int P, int dim,
+                                  void* stream);
+int nb200_zoe_add_cast_f16(float* x32, const void* delta, void* out, long long n, void* stream);
+int nb200_zoe_readout_concat_f16(const void* F, int B, int P, int dim, void* A, void* stream);
+int nb200_dpt_depth_to_space4_f16(const void* T, int B, int h, int w, int c, int cpad, void* out, void* stream);
+int nb200_dpt_im2col_s2_f16(const void* x, int B, int h, int w, int C, void* A, void* stream);
+int nb200_dpt_relu_add_f16(const void* x, const void* x0, void* y, void* s, long long n, void* stream);
+int nb200_dpt_head_final_f32(const void* x, long long npix, int C, const float* w, float bias, float* depth, void* stream);
+
 /* shifted-window attention core between the qkv and proj Linears
  * (torchvision swin_transformer.py:166-221), window 6x6, 6 heads.
  * qkv: three dense planes q | k | v, each [B][H][W][C] fp16 (how the engine's qkv GEMM writes them)
@@ -728,6 +758,8 @@ int nb200_profile_dump(char* buf, size_t cap);   /* one CSV line per timed launc
  *   bit 4 (on = 16): bwarp bwdelta aaresize fwarp (nb200_backward_warp / _conv with the kernel path taken, the learned-delta
  *                   warps nb200_backward_warp_delta / _f16 / _sym, nb200_depth_resize_aa, and nb200_forward_warp / _conv with
  *                   its depth-resize path: 0 none, 1 column table, 2 generic taps)
+ *   bit 5 (on = 32): dapatch zpatch datok ztok zcast zreadout d2s4 im2s2 reluadd headfin (the depth networks' patch im2col,
+ *                   token assembly, ZoeD_N's hook cast and readout concat, and the DPT reassemble, fusion and output kernels)
  * A line is `kind,name=value,name=value,...`: the launch's fields without its pointers, named where the host code writes
  * them.  Values are integers (flags 0 or 1) or fp32 values printed with 9 significant digits.  recorded_launches_named copies
  * the lines (NUL-terminated) like nb200_profile_dump; recorded_launches copies them without the names (`kind,value,...`, the

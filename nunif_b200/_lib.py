@@ -85,6 +85,7 @@ SIGNATURES = {
     "nb200_depth_anything_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_zoedepth_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_zoe_rel_pos_table": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "nb200_vit_pos_table_f32": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "nb200_depth_aa": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "nb200_mlbw_delta": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "nb200_mlbw_num_layers": (c_int, [c_void_p]),
@@ -191,6 +192,15 @@ SIGNATURES = {
     "nb200_depth_aa_out_f32": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 7 + [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
     "nb200_swin_mlp_fused_y_f16": (c_int, [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "nb200_da_patch_im2col_f16": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p, c_void_p]),
+    "nb200_zoe_patch_im2col_f16": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_void_p]),
+    "nb200_vit_assemble_tokens_f32": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p]),
+    "nb200_zoe_add_cast_f16": (c_int, [c_void_p] * 3 + [ctypes.c_longlong, c_void_p]),
+    "nb200_zoe_readout_concat_f16": (c_int, [c_void_p] + [c_int] * 3 + [c_void_p, c_void_p]),
+    "nb200_dpt_depth_to_space4_f16": (c_int, [c_void_p] + [c_int] * 5 + [c_void_p, c_void_p]),
+    "nb200_dpt_im2col_s2_f16": (c_int, [c_void_p] + [c_int] * 4 + [c_void_p, c_void_p]),
+    "nb200_dpt_relu_add_f16": (c_int, [c_void_p] * 4 + [ctypes.c_longlong, c_void_p]),
+    "nb200_dpt_head_final_f32": (c_int, [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_float, c_void_p, c_void_p]),
     "nb200_record_launches": (c_int, [c_int]),
     "nb200_recorded_launches": (c_int, [c_char_p, c_size_t]),
     "nb200_recorded_launches_named": (c_int, [c_char_p, c_size_t]),

@@ -181,11 +181,11 @@ extern "C" int nb200_profile_dump(char* buf, size_t cap) {
     return 0;
 }
 
-// Launch recorder: a non-zero mask (REC_GEMMS | REC_AUX | REC_CONV | REC_STEREO | REC_WARP bits, common.cuh) clears the record and starts appending
+// Launch recorder: a non-zero mask (REC_GEMMS | REC_AUX | REC_CONV | REC_STEREO | REC_WARP | REC_DEPTH bits, common.cuh) clears the record and starts appending
 // the kinds it selects, 0 stops (the record stays readable).  Host only: a launch made while it is off costs one relaxed
 // atomic load.
 extern "C" int nb200_record_launches(int on) {
-    NB_CHECK((on & ~(REC_GEMMS | REC_AUX | REC_CONV | REC_STEREO | REC_WARP)) == 0, "unknown recorder bits");
+    NB_CHECK((on & ~(REC_GEMMS | REC_AUX | REC_CONV | REC_STEREO | REC_WARP | REC_DEPTH)) == 0, "unknown recorder bits");
     std::lock_guard<std::mutex> lk(g_rec_mu);
     if (on) g_rec.clear();
     g_rec_enabled.store(on);

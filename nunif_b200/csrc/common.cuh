@@ -66,8 +66,9 @@ struct ProfScope {
 // the kinds: REC_GEMMS the GEMM, ViT attention and fused Swin block; REC_AUX the WABlock core, add + LayerNorm, DPT upsample
 // and ZoeDepth bins head; REC_CONV the waifu2x stem / tail / head convolutions, the SE block, to_image and the SOD REBNCONV;
 // REC_STEREO the input / output stages of row_flow_v3, mlbw and depth_aa, the fused row_flow_v2 kernel and the hole mask;
-// REC_WARP the backward and forward stereo warps and the antialiased depth resize.
-enum { REC_GEMMS = 1, REC_AUX = 2, REC_CONV = 4, REC_STEREO = 8, REC_WARP = 16 };
+// REC_WARP the backward and forward stereo warps and the antialiased depth resize; REC_DEPTH the depth networks' patch
+// embedding, token assembly, hook cast and readout concat, and the DPT reassemble, fusion and output kernels.
+enum { REC_GEMMS = 1, REC_AUX = 2, REC_CONV = 4, REC_STEREO = 8, REC_WARP = 16, REC_DEPTH = 32 };
 extern std::atomic<int> g_rec_enabled;
 inline bool rec_on(int kinds = REC_GEMMS) { return (g_rec_enabled.load(std::memory_order_relaxed) & kinds) != 0; }
 // one field of a recorded line: integers and flags print as integers, floating-point values with 9 significant digits

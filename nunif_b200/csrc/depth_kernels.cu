@@ -368,6 +368,7 @@ __global__ void __launch_bounds__(256) head_final_kernel(const __half* __restric
 
 // ------------------------------------------------------------------------------------------ host wrappers
 int da_patch_im2col(cudaStream_t st, const float* x, int B, int H, int W, __half* A, int kpad) {
+    if (rec_on(REC_DEPTH)) rec_launch("dapatch", {{"B", B}, {"H", H}, {"W", W}, {"kpad", kpad}});
     const int ph = H / PATCH, pw = W / PATCH;
     const long long total = (long long)B * ph * pw * kpad;
     patch_im2col_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(x, A, B, H, W, ph, pw, kpad);
@@ -376,6 +377,7 @@ int da_patch_im2col(cudaStream_t st, const float* x, int B, int H, int W, __half
 }
 
 int da_assemble_tokens(cudaStream_t st, const __half* T, const float* cls, const float* pos, float* X32, int B, int P, int dim) {
+    if (rec_on(REC_DEPTH)) rec_launch("datok", {{"B", B}, {"P", P}, {"dim", dim}});
     const long long total = (long long)B * (P + 1) * dim;
     assemble_tokens_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(T, cls, pos, X32, B, P, dim);
     NB_LAUNCHED();
@@ -417,6 +419,7 @@ int da_attention(cudaStream_t st, const __half* qkv, __half* out, int B, int N, 
 
 int da_relu_add(cudaStream_t st, const __half* x, const __half* x0, __half* y, __half* s, long long n) {
     NB_CHECK(n % 8 == 0, "element count must be a multiple of 8");
+    if (rec_on(REC_DEPTH)) rec_launch("reluadd", {{"n", n}, {"has_sum", s ? 1 : 0}});
     relu_add_kernel<<<(unsigned)cdiv64(n / 8, 256), 256, 0, st>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<const uint4*>(x0),
                                                                   reinterpret_cast<uint4*>(y), reinterpret_cast<uint4*>(s), n / 8);
     NB_LAUNCHED();
@@ -434,6 +437,8 @@ int da_upsample_bilinear(cudaStream_t st, const __half* x, int B, int h, int w, 
 }
 
 int da_depth_to_space4(cudaStream_t st, const __half* T, int B, int h, int w, int c, __half* out, int cpad) {
+    NB_CHECK(cpad >= c, "padded channel count below the channel count");
+    if (rec_on(REC_DEPTH)) rec_launch("d2s4", {{"B", B}, {"h", h}, {"w", w}, {"c", c}, {"cpad", cpad}});
     const long long total = (long long)B * 16 * h * w * cpad;
     depth_to_space4_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(T, out, B, h, w, c, cpad);
     NB_LAUNCHED();
@@ -442,6 +447,7 @@ int da_depth_to_space4(cudaStream_t st, const __half* T, int B, int h, int w, in
 
 int da_im2col_s2(cudaStream_t st, const __half* x, int B, int h, int w, int C, __half* A) {
     NB_CHECK(C % 8 == 0, "channels must be a multiple of 8");
+    if (rec_on(REC_DEPTH)) rec_launch("im2s2", {{"B", B}, {"h", h}, {"w", w}, {"C", C}});
     const int ho = (h + 1) / 2, wo = (w + 1) / 2;   // floor((h + 2 - 3) / 2) + 1
     const long long total = (long long)B * ho * wo * 9 * (C / 8);
     im2col_s2_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(x, A, B, h, w, C, ho, wo);
@@ -451,6 +457,7 @@ int da_im2col_s2(cudaStream_t st, const __half* x, int B, int h, int w, int C, _
 
 int da_head_final(cudaStream_t st, const __half* x, long long npix, int C, const float* wv, float bias, float* depth) {
     NB_CHECK(C == 32, "head_final supports 32 input channels");
+    if (rec_on(REC_DEPTH)) rec_launch("headfin", {{"npix", npix}, {"C", C}});
     head_final_kernel<32><<<(unsigned)cdiv64(npix, 256), 256, 0, st>>>(x, wv, bias, depth, npix);
     NB_LAUNCHED();
     return 0;

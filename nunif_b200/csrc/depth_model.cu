@@ -221,19 +221,18 @@ std::unique_ptr<DaW> pack_dinov2_dpt(Packer& pk, int encoder, const std::string&
 
 // dinov2 interpolate_pos_encoding (interpolate_offset 0.1): bicubic (A = -0.75, align_corners=False) resample of the
 // grid x grid table with scale factors (ph+0.1)/grid, (pw+0.1)/grid; ATen upsample_bicubic2d arithmetic in fp32.
-static void interp_pos_table(const DaW& w, int ph, int pw, std::vector<float>& out) {
-    const int dim = w.vit.dim, g = w.pos_grid;
-    out.assign((size_t)(1 + ph * pw) * dim, 0.f);
-    memcpy(out.data(), w.pos_host.data(), (size_t)dim * 4);
+// table: the learned [1 + g*g][dim] (class row first) -> out [1 + ph*pw][dim]
+static void interp_pos_table(const float* table, int g, int dim, int ph, int pw, float* out) {
+    memcpy(out, table, (size_t)dim * 4);
     if (ph == g && pw == g) {
-        memcpy(out.data() + dim, w.pos_host.data() + dim, (size_t)g * g * dim * 4);
+        memcpy(out + dim, table + dim, (size_t)g * g * dim * 4);
         return;
     }
     const float sy = (float)(1.0 / ((double)(ph + 0.1) / g)), sx = (float)(1.0 / ((double)(pw + 0.1) / g));
     auto cc1 = [](float x) { const float A = -0.75f; return ((A + 2.f) * x - (A + 3.f)) * x * x + 1.f; };
     auto cc2 = [](float x) { const float A = -0.75f; return ((A * x - 5.f * A) * x + 8.f * A) * x - 4.f * A; };
     auto clampi = [](int v, int hi) { return v < 0 ? 0 : (v > hi ? hi : v); };
-    const float* tab = w.pos_host.data() + dim;
+    const float* tab = table + dim;
     for (int oy = 0; oy < ph; ++oy) {
         const float ry = sy * ((float)oy + 0.5f) - 0.5f;
         const int iy = (int)std::floor(ry);
@@ -244,7 +243,7 @@ static void interp_pos_table(const DaW& w, int ph, int pw, std::vector<float>& o
             const int ix = (int)std::floor(rx);
             const float tx = rx - (float)ix;
             const float cx[4] = {cc2(tx + 1.f), cc1(tx), cc1(1.f - tx), cc2((1.f - tx) + 1.f)};
-            float* dst = &out[(size_t)(1 + oy * pw + ox) * dim];
+            float* dst = out + (size_t)(1 + oy * pw + ox) * dim;
             for (int c = 0; c < dim; ++c) {
                 float acc = 0.f;
                 for (int a = 0; a < 4; ++a) {
@@ -408,8 +407,8 @@ int dpt_output(cudaStream_t st, const nb200_model* m, const DptW& d, const DptBu
 
 int da_prepare_pos(DaW& w, cudaStream_t st, int ph, int pw) {
     if (w.pos_dev && w.pos_ph == ph && w.pos_pw == pw) return 0;
-    std::vector<float> tab;
-    interp_pos_table(w, ph, pw, tab);
+    std::vector<float> tab((size_t)(1 + ph * pw) * w.vit.dim);
+    interp_pos_table(w.pos_host.data(), w.pos_grid, w.vit.dim, ph, pw, tab.data());
     if (w.pos_dev) cudaFree(w.pos_dev);
     w.pos_dev = nullptr;
     w.pos_ph = w.pos_pw = 0;
@@ -458,4 +457,74 @@ extern "C" int nb200_depth_anything_forward(nb200_model* m, const float* x, int 
     NB_CHECK(w, "model is not a Depth-Anything network");
     NB_CHECK(B > 0, "empty batch");
     return depth_anything_forward(m, *w, (cudaStream_t)stream, x, B, H, W, depth);
+}
+
+// Host-only: the position table of a ph x pw token grid, as da_prepare_pos builds it for the forward (include/nunif_b200.h).
+extern "C" int nb200_vit_pos_table_f32(const float* table, int grid, int dim, int ph, int pw, float* out) {
+    NB_CHECK(table && out, "null pointer");
+    NB_CHECK(grid > 0 && dim > 0 && ph > 0 && pw > 0, "bad shape");
+    interp_pos_table(table, grid, dim, ph, pw, out);
+    return 0;
+}
+
+// ---- test entry points of the encoder-edge and DPT kernels that only a model forward reaches otherwise
+// (include/nunif_b200.h).  Every check runs before the first CUDA call.
+extern "C" int nb200_da_patch_im2col_f16(const float* x, int B, int H, int W, int kpad, void* A, void* stream) {
+    NB_CHECK(x && A, "null pointer");
+    NB_CHECK(B > 0 && H > 0 && W > 0, "bad shape");
+    NB_CHECK(H % 14 == 0 && W % 14 == 0, "height and width must be multiples of the 14-pixel patch");
+    NB_CHECK(kpad >= 3 * 14 * 14, "kpad below the 588 patch columns");
+    return da_patch_im2col((cudaStream_t)stream, x, B, H, W, (__half*)A, kpad);
+}
+
+extern "C" int nb200_zoe_patch_im2col_f16(const float* x, int B, int H, int W, void* A, void* stream) {
+    NB_CHECK(x && A, "null pointer");
+    NB_CHECK(B > 0 && H > 0 && W > 0, "bad shape");
+    NB_CHECK(H % 16 == 0 && W % 16 == 0, "height and width must be multiples of the 16-pixel patch");
+    return zoe_patch_im2col((cudaStream_t)stream, x, B, H, W, (__half*)A);
+}
+
+extern "C" int nb200_vit_assemble_tokens_f32(const void* T, const float* cls, const float* pos, float* x32, int B, int P, int dim,
+                                             void* stream) {
+    NB_CHECK(T && cls && x32, "null pointer");
+    NB_CHECK(B > 0 && P > 0 && dim > 0, "bad shape");
+    if (!pos) return zoe_assemble_tokens((cudaStream_t)stream, (const __half*)T, cls, x32, B, P, dim);
+    return da_assemble_tokens((cudaStream_t)stream, (const __half*)T, cls, pos, x32, B, P, dim);
+}
+
+extern "C" int nb200_zoe_add_cast_f16(float* x32, const void* delta, void* out, long long n, void* stream) {
+    NB_CHECK(x32 && out, "null pointer");
+    NB_CHECK(n > 0, "bad shape");
+    return zoe_add_cast((cudaStream_t)stream, x32, (const __half*)delta, (__half*)out, n);
+}
+
+extern "C" int nb200_zoe_readout_concat_f16(const void* F, int B, int P, int dim, void* A, void* stream) {
+    NB_CHECK(F && A, "null pointer");
+    NB_CHECK(B > 0 && P > 0 && dim > 0, "bad shape");
+    return zoe_readout_concat((cudaStream_t)stream, (const __half*)F, B, P, dim, (__half*)A);
+}
+
+extern "C" int nb200_dpt_depth_to_space4_f16(const void* T, int B, int h, int w, int c, int cpad, void* out, void* stream) {
+    NB_CHECK(T && out, "null pointer");
+    NB_CHECK(B > 0 && h > 0 && w > 0 && c > 0, "bad shape");
+    return da_depth_to_space4((cudaStream_t)stream, (const __half*)T, B, h, w, c, (__half*)out, cpad);
+}
+
+extern "C" int nb200_dpt_im2col_s2_f16(const void* x, int B, int h, int w, int C, void* A, void* stream) {
+    NB_CHECK(x && A, "null pointer");
+    NB_CHECK(B > 0 && h > 0 && w > 0 && C > 0, "bad shape");
+    return da_im2col_s2((cudaStream_t)stream, (const __half*)x, B, h, w, C, (__half*)A);
+}
+
+extern "C" int nb200_dpt_relu_add_f16(const void* x, const void* x0, void* y, void* s, long long n, void* stream) {
+    NB_CHECK(x && y, "null pointer");
+    NB_CHECK(!x0 == !s, "x0 and s go together");
+    NB_CHECK(n > 0, "bad shape");
+    return da_relu_add((cudaStream_t)stream, (const __half*)x, (const __half*)x0, (__half*)y, (__half*)s, n);
+}
+
+extern "C" int nb200_dpt_head_final_f32(const void* x, long long npix, int C, const float* w, float bias, float* depth, void* stream) {
+    NB_CHECK(x && w && depth, "null pointer");
+    NB_CHECK(npix > 0, "bad shape");
+    return da_head_final((cudaStream_t)stream, (const __half*)x, npix, C, w, bias, depth);
 }

@@ -383,6 +383,7 @@ __global__ void __launch_bounds__(256) zoe_clb_final_kernel(const __half* __rest
 
 // ------------------------------------------------------------------------------------------ host wrappers
 int zoe_patch_im2col(cudaStream_t st, const float* x, int B, int H, int W, __half* A) {
+    if (rec_on(REC_DEPTH)) rec_launch("zpatch", {{"B", B}, {"H", H}, {"W", W}});
     const int ph = H / PATCH, pw = W / PATCH;
     const long long total = (long long)B * ph * pw * 3 * PATCH * PATCH;
     zoe_patch_im2col_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(x, A, B, H, W, ph, pw);
@@ -391,6 +392,7 @@ int zoe_patch_im2col(cudaStream_t st, const float* x, int B, int H, int W, __hal
 }
 
 int zoe_assemble_tokens(cudaStream_t st, const __half* T, const float* cls, float* X32, int B, int P, int dim) {
+    if (rec_on(REC_DEPTH)) rec_launch("ztok", {{"B", B}, {"P", P}, {"dim", dim}});
     const long long total = (long long)B * (P + 1) * dim;
     zoe_assemble_tokens_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(T, cls, X32, B, P, dim);
     NB_LAUNCHED();
@@ -399,6 +401,7 @@ int zoe_assemble_tokens(cudaStream_t st, const __half* T, const float* cls, floa
 
 int zoe_add_cast(cudaStream_t st, float* X32, const __half* delta, __half* out, long long n) {
     NB_CHECK(n % 4 == 0, "element count must be a multiple of 4");
+    if (rec_on(REC_DEPTH)) rec_launch("zcast", {{"n", n}, {"has_delta", delta ? 1 : 0}});
     zoe_add_cast_kernel<<<(unsigned)cdiv64(n / 4, 256), 256, 0, st>>>(reinterpret_cast<float4*>(X32), reinterpret_cast<const uint2*>(delta),
                                                                       reinterpret_cast<uint2*>(out), n / 4);
     NB_LAUNCHED();
@@ -416,6 +419,7 @@ int zoe_expand_rel_bias(cudaStream_t st, const float* table, int ph, int pw, int
 
 int zoe_readout_concat(cudaStream_t st, const __half* F, int B, int P, int dim, __half* A) {
     NB_CHECK(dim % 8 == 0, "embedding dim must be a multiple of 8");
+    if (rec_on(REC_DEPTH)) rec_launch("zreadout", {{"B", B}, {"P", P}, {"dim", dim}});
     const long long total = (long long)B * P * 2 * (dim / 8);
     zoe_readout_concat_kernel<<<(unsigned)cdiv64(total, 256), 256, 0, st>>>(reinterpret_cast<const uint4*>(F), B, P, dim / 8,
                                                                             reinterpret_cast<uint4*>(A));

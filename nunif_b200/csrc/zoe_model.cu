@@ -187,7 +187,7 @@ std::unique_ptr<NetW> pack_zoedepth(Packer& pk) {
 
 // MiDaS beit.py _get_rel_pos_bias: the (2g-1) x (2g-1) learned sub-table -> (2ph-1) x (2pw-1) by ATen's bilinear resample
 // (align_corners=False, no antialias), the 3 class-token rows appended unchanged.  out: [(2ph-1)(2pw-1) + 3][heads]
-static void zoe_resample_table(const std::vector<float>& tab, int g, int heads, int ph, int pw, float* out) {
+static void zoe_resample_table(const float* tab, int g, int heads, int ph, int pw, float* out) {
     const int S = 2 * g - 1, nh = 2 * ph - 1, nw = 2 * pw - 1;
     const float sy = (float)S / (float)nh, sx = (float)S / (float)nw;
     for (int y = 0; y < nh; ++y) {
@@ -217,7 +217,7 @@ static int zoe_prepare_bias(ZoeW& w, cudaStream_t st, int ph, int pw) {
     const int N = ph * pw + 1, ldb = (N + 63) / 64 * 64;
     const size_t rows = (size_t)(2 * ph - 1) * (2 * pw - 1) + 3, per_layer = (size_t)heads * N * ldb;
     std::vector<float> host(rows * heads * depth);
-    for (int i = 0; i < depth; ++i) zoe_resample_table(w.tables[i], w.old_grid, heads, ph, pw, host.data() + (size_t)i * rows * heads);
+    for (int i = 0; i < depth; ++i) zoe_resample_table(w.tables[i].data(), w.old_grid, heads, ph, pw, host.data() + (size_t)i * rows * heads);
     if (w.bias_dev) cudaFree(w.bias_dev);
     w.bias_dev = nullptr; w.bias_ph = w.bias_pw = 0;
     float* tdev = nullptr;
@@ -374,8 +374,7 @@ using namespace nb200;
 extern "C" int nb200_zoe_rel_pos_table(const float* table, int g, int heads, int ph, int pw, float* out) {
     NB_CHECK(table && out, "null pointer");
     NB_CHECK(g > 0 && heads > 0 && ph > 0 && pw > 0, "bad shape");
-    const size_t n = ((size_t)(2 * g - 1) * (2 * g - 1) + 3) * heads;
-    zoe_resample_table(std::vector<float>(table, table + n), g, heads, ph, pw, out);
+    zoe_resample_table(table, g, heads, ph, pw, out);
     return 0;
 }
 

@@ -111,14 +111,14 @@ def test_zoe_preprocess_size_host_rule_bit_exact(lib):
         assert (fh + 2 * p_h, fw + 2 * p_w, p_h, p_w) == (int(oh), int(ow), int(ph), int(pw)), (H, W)
 
 
-def test_launch_recorder_mask_bits_0_to_4(lib):
+def test_launch_recorder_mask_bits_0_to_5(lib):
     """nb200_record_launches takes a mask of the recorded kinds (bit 0: GEMM / attention / Swin, bit 1: the kernels between
     them, bit 2: the waifu2x stem / tail / head convolutions, SE, to_image and the SOD REBNCONV, bit 3: the stereo networks'
-    input / output stages, row_flow_v2 and the hole mask, bit 4: the backward stereo warps and the AA depth resize) and
-    refuses other bits; host only, no device needed."""
-    for on in (1, 2, 3, 4, 7, 8, 15, 16, 31, 0):
+    input / output stages, row_flow_v2 and the hole mask, bit 4: the backward stereo warps and the AA depth resize, bit 5: the
+    depth networks' patch, token, hook-cast, readout and DPT kernels) and refuses other bits; host only, no device needed."""
+    for on in (1, 2, 3, 4, 7, 8, 15, 16, 31, 32, 63, 0):
         assert lib.nb200_record_launches(on) == 0, on
-    for on in (32, 63):
+    for on in (64, 127):
         assert lib.nb200_record_launches(on) != 0, on
         assert b"unknown recorder bits" in lib.nb200_last_error()
     buf = ctypes.create_string_buffer(16)
@@ -145,6 +145,41 @@ def test_stereo_entry_points_refuse_bad_geometry(lib):
         (lambda: lib.nb200_depth_aa_out_f32(d, d, None, 1, 16, 17, 0, 0, 8, 8, d, d, 1, d, None), b"padded width"),
     ]
     assert lib.nb200_record_launches(8) == 0
+    try:
+        for i, (call, msg) in enumerate(cases):
+            assert call() != 0, i
+            assert msg in lib.nb200_last_error(), (i, lib.nb200_last_error())
+    finally:
+        lib.nb200_record_launches(0)
+    buf = ctypes.create_string_buffer(16)
+    assert lib.nb200_recorded_launches(buf, 16) == 0 and buf.value == b""
+
+
+def test_depth_entry_points_refuse_bad_shapes(lib):
+    """The depth networks' kernel entry points refuse, before their first CUDA call, an image that is not a whole number of
+    patches, a patch row narrower than its 588 columns, element counts and widths their vector loads cannot take, a head
+    width other than 32, a channel pad below the channel count, and an x0 without s: dummy host pointers, no device needed,
+    and nothing is recorded."""
+    d = ctypes.create_string_buffer(4096)
+    cases = [
+        (lambda: lib.nb200_da_patch_im2col_f16(d, 1, 28, 27, 640, d, None), b"multiples of the 14-pixel patch"),
+        (lambda: lib.nb200_da_patch_im2col_f16(d, 1, 15, 28, 640, d, None), b"multiples of the 14-pixel patch"),
+        (lambda: lib.nb200_da_patch_im2col_f16(d, 1, 28, 28, 584, d, None), b"kpad below"),
+        (lambda: lib.nb200_zoe_patch_im2col_f16(d, 1, 32, 40, d, None), b"multiples of the 16-pixel patch"),
+        (lambda: lib.nb200_zoe_patch_im2col_f16(d, 1, 14, 32, d, None), b"multiples of the 16-pixel patch"),
+        (lambda: lib.nb200_vit_assemble_tokens_f32(d, d, d, d, 1, 0, 384, None), b"bad shape"),
+        (lambda: lib.nb200_zoe_add_cast_f16(d, d, d, 1026, None), b"multiple of 4"),
+        (lambda: lib.nb200_zoe_add_cast_f16(d, None, d, 6, None), b"multiple of 4"),
+        (lambda: lib.nb200_zoe_readout_concat_f16(d, 1, 4, 100, d, None), b"multiple of 8"),
+        (lambda: lib.nb200_dpt_depth_to_space4_f16(d, 1, 2, 3, 48, 40, d, None), b"padded channel count"),
+        (lambda: lib.nb200_dpt_im2col_s2_f16(d, 1, 3, 3, 12, d, None), b"multiple of 8"),
+        (lambda: lib.nb200_dpt_relu_add_f16(d, d, d, d, 1020, None), b"multiple of 8"),
+        (lambda: lib.nb200_dpt_relu_add_f16(d, None, d, None, 12, None), b"multiple of 8"),
+        (lambda: lib.nb200_dpt_relu_add_f16(d, d, d, None, 16, None), b"x0 and s go together"),
+        (lambda: lib.nb200_dpt_head_final_f32(d, 64, 64, d, 0.5, d, None), b"32 input channels"),
+        (lambda: lib.nb200_dpt_head_final_f32(d, 64, 16, d, 0.5, d, None), b"32 input channels"),
+    ]
+    assert lib.nb200_record_launches(32) == 0
     try:
         for i, (call, msg) in enumerate(cases):
             assert call() != 0, i
